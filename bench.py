@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - decoder frames/s of the wavelet-monodepth hot path on N B200s (contract: see the task brief).
+"""bench.py - decoder frames/s of the wavelet-monodepth hot path on N H100s.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--workload NAME]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--workload NAME] [--dump-outputs DIR]
 
 A "step" is one pass of the sparse wavelet decoder (SparseDepthWaveProgressiveDecoder semantics,
 thresh_ratio 0.05) over one batch of synthetic encoder features.  Headline workload (BASELINE.json
@@ -15,8 +15,10 @@ JSON keys beyond the base contract:
             (double-buffered on a copy stream) and D2H of the step's depth output inside the timed region
   roofline  dominant kernel (by summed device time) : algorithmic bytes / CUDA-event time vs measured HBM peak,
             plus its FLOP rate; roofline_kernels lists the same for every libwmd kernel
-  cpu_baseline  the oracle's port of the reference's CPU path timed on this box's host cores (bounded sample)
+  cpu_baseline  the oracle's port of the reference's CPU path timed on the host's cores (bounded sample)
 `--impl reference` times that CPU path as its own arm (rank 0 only under torchrun).
+`--dump-outputs DIR` writes what the last timed step returned (rank 0's shard) as DIR/<name>.npy, so that two builds can
+be compared output for output on the same seeded inputs.
 """
 import argparse
 import json
@@ -47,7 +49,7 @@ HEAD_KEYS = synth.KITTI_HEAD_KEYS                                               
 SYNTH = synth.BENCH_SYNTH
 THRESH = 0.05
 METRIC, UNIT = "decoder_frames_per_sec", "frames/s"
-FP32_SIMT_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12      # 148 SMs x 128 FMA lanes x 2 flop x max SM clock
+FP32_SIMT_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12       # H100 SXM: 132 SMs x 128 FMA lanes x 2 flop x max SM clock
 
 
 def log(*a):
@@ -73,7 +75,7 @@ def measured_peaks():
                     float(sus) if sus else None)
         except Exception:
             pass
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md 6.65 TB/s, 1.59 PFLOP/s)", None
+    return 3350.0, 989.0, "fallback (NVIDIA H100 SXM data sheet: 3.35 TB/s, 989 TFLOP/s dense BF16 at 700 W)", None
 
 
 # ------------------------------------------------------------------------------------------ clocks
@@ -208,7 +210,7 @@ def conv_layer_table(records, peak_gbs, tf32_peak, steps):
         by, fl = account(name, info)
         rows = min(_as_int(info["count"], info["n"] * info["h"] * info["w"]), info["max_rows"])
         tf = fl / (ms * 1e-3) / 1e12 if ms > 0 else 0.0
-        line = {"engine": ("tcgen05_f16x3" if info.get("f16") else "tcgen05_3xtf32") if name == "conv_rows_tc" else "fp32_fma",
+        line = {"engine": ("wgmma_f16x3" if info.get("f16") else "wgmma_3xtf32") if name == "conv_rows_tc" else "fp32_fma",
                 "taps": info["taps"],
                 "cin": [info["c0"], info["c1"]], "cout": info["cout"], "grid": [info["n"], info["h"], info["w"]],
                 "rows": rows, "us": round(1e3 * ms, 1), "fp32_eq_tflops": round(tf, 1),
@@ -268,24 +270,14 @@ def roofline_from(records, peak_gbs, peak_tf, peak_src, steps, peak_tf_sustained
                 "peak_source": ("measured in this run: cuBLAS TF32 GEMM 8192^3, best of 20 (burst; each launch is timed alone "
                                 "between two events)" if tf32_peak else peak_src + ": bf16_tflops / 2"),
                 "operand_form": "f16x3 (fp16 pairs, opt-in)" if f16_form else "tf32x3",
-                "note": "achieved = algorithmic fp32-equivalent flops (2*taps*Cin*Cout*M_out) / event time. tcgen05.mma.kind::tf32, "
-                        "3 MMAs per fp32 product (hi*hi + hi*lo + lo*hi), fp32 accumulation in TMEM drained every 1024 of K; "
+                "note": "achieved = algorithmic fp32-equivalent flops (2*taps*Cin*Cout*M_out) / event time. wgmma tf32, "
+                        "3 MMAs per fp32 product (hi*hi + hi*lo + lo*hi), fp32 accumulation in registers, epochs of 1024 of K; "
                         "per-layer figures in conv_layers, DESIGN.md 4"}
     else:
         main = dict(hbm_view)
         main.update(kernel=dom, peak_source=peak_src,
                     note="fp32 SIMT kernel; tflops/fp32_frac give the FMA-roof view (%.1f TFLOP/s nominal)" % FP32_SIMT_PEAK_TFLOPS,
                     fp32_frac=round(main["tflops"] / FP32_SIMT_PEAK_TFLOPS, 4))
-    traffic_file = os.path.join(REPO, "profiles", "ncu_traffic.json")
-    if os.path.exists(traffic_file):
-        try:
-            tr = json.load(open(traffic_file))
-            main["traffic"] = tr.get(dom)
-            for name in out:
-                if tr.get(name) is not None:
-                    out[name]["traffic"] = tr[name]
-        except Exception:
-            pass
     # whole step against the HBM roof (north_star: "fraction of the HBM roofline" for the fused decoder): the summed
     # algorithmic bytes of every launch of a step over the summed kernel time
     step_bytes = sum(a["bytes"] for a in agg.values()) / max(steps, 1)
@@ -392,8 +384,8 @@ def cpu_frames_per_sec(wl_name, frames, budget_s=20.0, first_frame=0, batch=None
 
 
 def workload_config(wl_name, world, thresh=None):
-    """Static description of the measured workload: identical in the native and the reference arm (the driver compares
-    the two arms' `config`).  Anything measured (mask densities, op counts) or arm-specific goes elsewhere."""
+    """Static description of the measured workload: identical in the native and the reference arm, so that
+    the two arms' `config` objects show they measured the same work.  Anything measured (mask densities, op counts) or arm-specific goes elsewhere."""
     wl = WORKLOADS[wl_name]
     return {
         "workload": wl_name, "global_batch": wl["per_gpu_batch"] * world, "per_gpu_batch": wl["per_gpu_batch"],
@@ -522,6 +514,30 @@ def measure_tf32_peak(dev):
         torch.backends.cuda.matmul.allow_tf32 = was
 
 
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(path, last):
+    """The last timed step's outputs as path/<name>.npy: every tensor of the decoder's result dict in float32 (masks as
+    0 / 1) and total_ops_per_sample in float64.  An output larger than its share of the 64 MB budget is replaced by a
+    fixed sample of its flattened elements (same seed, same positions in every run) and saved flat."""
+    os.makedirs(path, exist_ok=True)
+    out = last["out"]
+    tensors = {("_".join(str(p) for p in k) if isinstance(k, tuple) else str(k)): v
+               for k, v in out.items() if torch.is_tensor(v)}
+    per_array = DUMP_BUDGET_BYTES // 4 // (len(tensors) + 1)
+    for name, v in sorted(tensors.items()):
+        a = v.detach().float().cpu().numpy()
+        if a.size > per_array:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, per_array, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, name + ".npy"), a)
+    ops = (last.get("ops_result") or {}).get("total_ops_per_sample")
+    if ops is not None:
+        np.save(os.path.join(path, "total_ops_per_sample.npy"), np.asarray(ops, dtype=np.float64))
+    log("outputs of the last timed step -> %s (%d arrays)" % (path, len(tensors) + (ops is not None)))
+
+
 class _Stepper:
     """One bench step = decoder replay (no host wait) + the rank's all-gather started asynchronously; the previous
     step's op count and gathered tensor are consumed while this one runs.  flush() drains the tail."""
@@ -609,6 +625,8 @@ def run_native(args, rank, world, local_rank):
     l0 = _lib.launch_count()
     ms = time_device(main.step, args.steps, 1 if args.warmup else 0, dist, world, flush=main.flush)
     launches = _lib.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     launches -= (1 if args.warmup else 0) * (launches // (args.steps + (1 if args.warmup else 0)))
     if use_graph:
         launches = graph.launches * args.steps                       # kernel nodes replayed inside the timed region
@@ -899,8 +917,8 @@ def run_native(args, rank, world, local_rank):
             "e2e": {"value": round(e2e_value, 1), "unit": UNIT, "h2d_bytes_per_step": e2e_h2d * world,
                     "d2h_bytes_per_step": d2h_bytes * world, "ms_per_step": round(e2e_ms / args.steps, 3),
                     "pcie_floor_ms": round(e2e_h2d / 57e9 * 1e3, 2),
-                    "note": e2e_note + "; pcie_floor_ms = h2d bytes / 57 GB/s (what cudaMemcpyAsync from pinned memory "
-                            "sustains on this box)" + ("; byte counts are the whole job's (rank 0's x %d ranks)" % world if world > 1 else "")},
+                    "note": e2e_note + "; pcie_floor_ms = h2d bytes / 57 GB/s (a nominal PCIe Gen5 x16 rate for "
+                            "cudaMemcpyAsync from pinned memory, not measured)" + ("; byte counts are the whole job's (rank 0's x %d ranks)" % world if world > 1 else "")},
             "e2e_dma": e2e_dma,
             "e2e_variants": e2e_variants,
             "gpu_launches": int(launches_t.item()),
@@ -936,6 +954,8 @@ def main():
                          "sparse levels' maps); the fastest variant is reported as e2e; 'off' skips them")
     ap.add_argument("--no-also", action="store_true")
     ap.add_argument("--no-sweep", action="store_true", help="skip the threshold sweep (configs[2] / configs[4])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

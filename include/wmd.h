@@ -1,5 +1,5 @@
 /*
- * wmd.h - C ABI of libwmd.so: the B200 (sm_100a) wavelet-monodepth decoder hot path.
+ * wmd.h - C ABI of libwmd.so: the H100 (sm_90a) wavelet-monodepth decoder hot path.
  *
  * The reference (nianticlabs/wavelet-monodepth) has no native/FFI layer: its
  * boundary for this path is a Python nn.Module / function API built on ATen ops
@@ -192,21 +192,20 @@ typedef struct wmd_conv_desc {
   float* amax_out;          /* device scalar, or NULL: atomically raised to max |y| of the rows written (zero it before the
                                first producer; both precisions) */
   int32_t rows0;            /* rows allocated in x0, 0 = unknown.  Only used by the tensor-core engine's 1x1 form (taps == 1,
-                               map0 == NULL: output row m reads x0 row m): with rows0 > 0 it loads whole 256-row tiles by TMA
-                               (reads past rows0 are zero-filled) instead of gathering row by row */
+                               map0 == NULL: output row m reads x0 row m): with rows0 > 0 rows past rows0 read zeros */
 } wmd_conv_desc;
 
 int wmd_conv_rows_f32(const wmd_conv_desc* d, wmd_stream_t stream);
 
-/* Tensor-core engine for the same contract: tcgen05.mma.kind::tf32 with a 3xTF32 split (hi*hi + lo*hi + hi*lo,
- * fp32 accumulation in TMEM), so results stay fp32-faithful (<= ~1e-6 relative vs the SIMT kernel).  d->w must
+/* Tensor-core engine for the same contract: wgmma tf32 with a 3xTF32 split (hi*hi + lo*hi + hi*lo,
+ * fp32 accumulation), so results stay fp32-faithful (<= ~1e-6 relative vs the SIMT kernel).  d->w must
  * point to weights packed by wmd_pack_conv_weight_tc_f32 for the same (cout, c0, c1, taps); d->ldw is ignored.
- *   wmd_conv_tc_tile_n(cout)                 N-tile of the kernel for this cout (128 / 64 / 32; the CTA tile is 256 rows x N)
+ *   wmd_conv_tc_tile_n(cout)                 N-tile of the kernel for this cout (128 / 64 / 32; the CTA tile is 128 rows x N)
  *   wmd_conv_tc_weight_floats(...)           size of the packed weight buffer, in floats
  *   wmd_pack_conv_weight_tc_f32(w, packed..) (Cout, c0+c1, kh, kw) -> per (n-tile, 32-channel chunk) fp32
  *                                            shared-memory images [tf32 hi | tf32 lo] of N x 32, K-major, 128-byte swizzled
- * Accumulation runs in epochs of K = 1024 inside TMEM and is drained into fp32 registers with round-to-nearest
- * adds, because the tensor core's own fp32 accumulation rounds toward zero (bias ~6.5e-9 * K relative). */
+ * Accumulation runs in epochs of K = 1024 in the wgmma accumulators, each added into fp32 registers with
+ * round-to-nearest adds, because the tensor core's own fp32 accumulation does not round to nearest (bias ~6.5e-9 * K relative). */
 enum { WMD_PREC_TF32X3 = 0, WMD_PREC_F16X3 = 1 };
 int wmd_conv_tc_tile_n(int cout);
 /* Weights for precision = WMD_PREC_F16X3: 128-byte header (float 0: 1 / s_w) + per (n-tile, 32-channel chunk) one N x 128 B
@@ -235,15 +234,14 @@ int wmd_conv_rows_tc_f32(const wmd_conv_desc* d, wmd_stream_t stream);
  * together; only remainder tiles cut by a range boundary (<= 8 segments) go through the workspace: the LAST segment of
  * a tile to arrive (per-tile arrival counter) sums all of them in slab order - bias first - inside the same kernel, so
  * there is no second pass and the bits do not depend on the arrival order.  Its workspace size does not depend on the
- * layer (4 KiB of counters + SMs x 8 x 256 x 128 floats).  The first 4 KiB of `ws` (any splits) must be ZERO before the
+ * layer (4 KiB of counters + SMs x 8 x 128 x 128 floats).  The first 4 KiB of `ws` (any splits) must be ZERO before the
  * first launch that uses the buffer; every launch leaves them zero. */
 size_t wmd_conv_tc_splitk_ws_bytes(int max_rows, int ldy, int splits);
-/* 3x3 layers gather the A operand once per (channel chunk, dy) and feed the three dx taps from that one shared-memory
- * stage through a per-tile slot table (sparse_conv3x3's nine shifted selections, KITTI/layers.py:445-453, read almost the
- * same rows).  On by default; wmd_conv_tc_set_shared_taps(0) restores one gather per tap (A/B measurements, tests:
- * both forms produce identical bits).  on < 0 only queries.  Returns the previous setting.  Process-wide. */
+/* Shared-tap gather setting (one gather per (channel chunk, dy) feeding the three dx taps).  The sm_90a engine gathers
+ * every tap's rows itself, so the setting does not change what runs or its bits; it is kept for the C ABI.  on < 0 only
+ * queries.  Returns the previous setting.  Process-wide. */
 int wmd_conv_tc_set_shared_taps(int on);
-/* The tcgen05 engine runs one persistent CTA per SM, and such a CTA holds the SM's whole register file: no other kernel -
+/* The tensor-core engine runs one persistent CTA per SM, and such a CTA holds most of the SM's shared memory: no other kernel -
  * an NCCL collective of the previous step in particular - can run beside it.  wmd_conv_tc_set_reserved_sms(n) makes the
  * persistent grid n CTAs smaller so that n SMs stay free (multi-GPU serving: the all-gather of step k then really runs
  * under the convolutions of step k + 1).  0 by default; n < 0 only queries.  Returns the previous setting.  Process-wide;

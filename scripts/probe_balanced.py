@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0, '/root/repo')
+import os, sys; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from wavelet_monodepth_b200 import ops
 from wavelet_monodepth_b200._lib import PAD_REFLECT, ACT_ELU

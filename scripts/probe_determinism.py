@@ -1,6 +1,6 @@
 """Fresh process: two forwards of the sparse decoder, every libwmd op's outputs compared between them (the first forward
 runs every kernel cold: timing-dependent races show up as differences)."""
-import sys; sys.path.insert(0, '/root/repo')
+import os, sys; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from wavelet_monodepth_b200 import kitti_decoders as kd, ops, synth
 DEV = 'cuda'

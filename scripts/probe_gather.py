@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0, '/root/repo')
+import os, sys; sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, torch.nn.functional as F
 from wavelet_monodepth_b200 import ops
 dev = 'cuda'

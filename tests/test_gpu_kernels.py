@@ -178,7 +178,7 @@ def test_pack_weight_layout():
 # ------------------------------------------------------------------------------------------ conv
 @pytest.fixture(params=["simt", "tc"])
 def kind(request):
-    """Both gather-GEMM engines answer to the same contract: fp32 FMA tiles and tcgen05 3xTF32."""
+    """Both gather-GEMM engines answer to the same contract: fp32 FMA tiles and wgmma 3xTF32."""
     return request.param
 
 

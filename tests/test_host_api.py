@@ -98,14 +98,14 @@ def test_bench_byte_accounting_matches_the_survey_formulas():
     assert (by, fl) == (4 * 100 * (32 + 56) + 4 * (64 * 32 + 54 * 64 + 64), 2 * 100 * (32 * 64 + 64 * 54))
     recs = [("conv_rows_tc", 0.2, dict(conv, kind="tc")), ("idwt_haar", 0.01, dict(n=n, c=1, h=h, w=w, disp=True))] * 2
     table = bench.conv_layer_table(recs, 6500.0, 1600.0, 2)
-    assert len(table) == 1 and table[0]["rows"] == m and table[0]["engine"] == "tcgen05_3xtf32"
+    assert len(table) == 1 and table[0]["rows"] == m and table[0]["engine"] == "wgmma_3xtf32"
     main, per_kernel = bench.roofline_from(recs, 6500.0, 1600.0, "test", 2, 1361.0)
     assert main["kernel"] == "conv_rows_tc" and main["bound"] == "tensor" and set(per_kernel) == {"conv_rows_tc", "idwt_haar"}
     assert main["step_view"]["algorithmic_bytes_per_step"] == by_sum(recs, bench) // 2
     assert main["operand_form"] == "tf32x3" and main["peak"] == 800.0            # no tf32 measurement given: bf16 / 2
     # the opt-in fp16-pair operand form is labelled and measured against the fp16 / bf16 tensor peak
     recs16 = [("conv_rows_tc", 0.2, dict(conv, kind="tc", f16=True))] * 2
-    assert bench.conv_layer_table(recs16, 6500.0, 1600.0, 2)[0]["engine"] == "tcgen05_f16x3"
+    assert bench.conv_layer_table(recs16, 6500.0, 1600.0, 2)[0]["engine"] == "wgmma_f16x3"
     main16, _ = bench.roofline_from(recs16, 6500.0, 1600.0, "test", 2, 1361.0, tf32_peak=760.0)
     assert main16["operand_form"].startswith("f16x3") and main16["peak"] == 1600.0
 

@@ -1,113 +1,86 @@
-"""CPU, build container only: INTEGRATION.md section A executed against the UNMODIFIED reference tree.
-
-Skipped when /root/reference is absent (the GPU box).  What is checked is the seam a maintainer of the reference
-touches, not arithmetic:
-  * the three-line swap (package-level names of ``networks.decoders`` + ``sys.modules['pytorch_wavelets']``) makes the
-    reference's own factories build OUR classes: ``network_constructors.make_depth_decoder``
-    (KITTI/networks/network_constructors.py:30-40) and ``Model`` (NYUv2/model.py:47-71);
-  * ``pyt_utils.group_weight`` over ``.convs`` (KITTI/trainer.py:74-75, KITTI/pyt_utils.py:12-29) accepts every value -
-    its assert fails if a module carries a parameter that is not a Conv/Linear weight or bias;
-  * state dicts load STRICTLY in both directions (KITTI/test_simple.py:101-102) and survive the reference's own
-    save / load code paths on disk (KITTI/trainer.py:733-773 pattern, NYUv2/load_save_utils.py:10-39 called as is);
-  * without CUDA the swapped-in decoders fail loudly (no silent CPU path).
+"""CPU: the seam a maintainer of the reference touches (INTEGRATION.md section A), checked against the reference's own
+module layout as oracle/pin_reference_layout.py recorded it from the UNMODIFIED reference tree
+(tests/golden/reference_layout.json).  Not arithmetic:
+  * for every decoder the reference's factories build (KITTI/networks/network_constructors.py:30-40, NYUv2/model.py:47-71)
+    ours has the same class name, state-dict keys and shapes, so the three-line swap builds OUR classes in its place and
+    checkpoints load STRICTLY in both directions (KITTI/test_simple.py:101-102);
+  * ``.convs`` has the reference's keys and every parameter is reachable through it the way ``pyt_utils.group_weight``
+    collects them (KITTI/trainer.py:74-75, KITTI/pyt_utils.py:12-29: Conv/Linear weights and biases only);
+  * checkpoints survive the trainer's save / load code paths on disk (KITTI/trainer.py:733-773 pattern);
+  * without CUDA the decoders fail loudly (no silent CPU path);
+  * the public functions of KITTI/layers.py exist here with the same parameter names.
 """
-import argparse
-import importlib
+import json
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.nn as nn
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present (GPU box)")
+from helpers import GOLDEN
 
-
-def _purge():
-    for name in list(sys.modules):
-        if name in ("layers", "networks", "pyt_utils", "model", "load_save_utils", "pytorch_wavelets") or \
-                name.startswith("networks."):
-            del sys.modules[name]
-    sys.path[:] = [p for p in sys.path if not p.startswith(REF)]
-    importlib.invalidate_caches()
-
-
-@pytest.fixture
-def kitti_tree():
-    """The reference's KITTI tree importable, `pytorch_wavelets` = our wavelets module (swap line 3)."""
-    import wavelet_monodepth_b200.wavelets as w
-    _purge()
-    sys.path.insert(0, os.path.join(REF, "KITTI"))
-    sys.modules["pytorch_wavelets"] = w
-    yield
-    _purge()
-
-
-@pytest.fixture
-def nyu_tree():
-    import wavelet_monodepth_b200.wavelets as w
-    _purge()
-    sys.path.insert(0, os.path.join(REF, "NYUv2"))
-    sys.modules["pytorch_wavelets"] = w
-    yield
-    _purge()
+with open(os.path.join(GOLDEN, "reference_layout.json")) as _f:
+    LAYOUT = json.load(_f)
 
 
 class _Encoder:
-    num_ch_enc = np.array([64, 64, 128, 256, 512])
+    num_ch_enc = np.array(LAYOUT["kitti_num_ch_enc"])
 
 
-def _kitti_opts(**kw):
-    o = argparse.Namespace(use_wavelets=True, use_sparse=False, scales=range(4))
-    o.__dict__.update(kw)
-    return o
-
-
-def _swap_kitti():
-    """INTEGRATION.md A, line 1: rebind the names KITTI/networks/decoders/__init__.py exports."""
-    import networks.decoders as dec
+def _kitti_decoder(case):
     from wavelet_monodepth_b200 import kitti_decoders as kd
-    ref = {n: getattr(dec, n) for n in ("DepthDecoder", "DepthWaveProgressiveDecoder", "SparseDepthWaveProgressiveDecoder")}
-    for n in ref:
-        setattr(dec, n, getattr(kd, n))
-    return ref, kd
+    cls = getattr(kd, LAYOUT["kitti"][case]["class"])
+    return cls(_Encoder.num_ch_enc) if cls is kd.SparseDepthWaveProgressiveDecoder else cls(_Encoder.num_ch_enc, range(4))
 
 
-def test_kitti_factory_builds_our_decoders_and_trainer_param_groups_accept_them(kitti_tree, capsys):
-    ref, kd = _swap_kitti()
-    from networks.network_constructors import make_depth_decoder      # unmodified reference factory
-    from pyt_utils import group_weight                                # unmodified reference helper
-    for opts, cls in ((_kitti_opts(), kd.DepthWaveProgressiveDecoder),
-                      (_kitti_opts(use_sparse=True), kd.SparseDepthWaveProgressiveDecoder),
-                      (_kitti_opts(use_wavelets=False), kd.DepthDecoder)):
-        dec = make_depth_decoder(_Encoder(), opts)
-        assert type(dec) is cls
-        groups = []
-        for _, weights in dec.convs.items():                         # KITTI/trainer.py:74-75
-            group_weight(groups, weights, 1e-4)
-        n_grouped = sum(len(g["params"]) for g in groups)
-        assert n_grouped == len(list(dec.parameters())) > 0          # every parameter is reachable through .convs
-        refdec = ref[cls.__name__](_Encoder.num_ch_enc) if cls is kd.SparseDepthWaveProgressiveDecoder else \
-            ref[cls.__name__](_Encoder.num_ch_enc, range(4))
-        assert list(dec.state_dict().keys()) == list(refdec.state_dict().keys())
-        assert [tuple(v.shape) for v in dec.state_dict().values()] == [tuple(v.shape) for v in refdec.state_dict().values()]
-        assert list(dec.convs.keys()) == list(refdec.convs.keys())
-        # strict loading both ways (KITTI/test_simple.py:101-102)
-        dec.load_state_dict(refdec.state_dict(), strict=True)
-        refdec.load_state_dict(dec.state_dict(), strict=True)
-    capsys.readouterr()
+def _reference_state_dict(entry, seed):
+    """A state dict with the reference module's keys and shapes (what its torch.save would have written), seeded values."""
+    g = torch.Generator().manual_seed(seed)
+    return {k: torch.rand(tuple(s), generator=g) for k, s in zip(entry["keys"], entry["shapes"])}
 
 
-def test_kitti_checkpoints_round_trip_on_disk_through_the_trainers_code_path(kitti_tree, tmp_path):
-    ref, kd = _swap_kitti()
-    ours = kd.SparseDepthWaveProgressiveDecoder(_Encoder.num_ch_enc)
-    theirs = ref["SparseDepthWaveProgressiveDecoder"](_Encoder.num_ch_enc)
-    # trainer.save_model (:733-751): torch.save(model.state_dict(), "<name>.pth")
+def _grouped_params(convs):
+    """Parameters pyt_utils.group_weight collects from the values of ``.convs``: Conv / Linear weights and biases."""
+    n = 0
+    for module in convs.values():
+        for m in module.modules():
+            if isinstance(m, (nn.Linear, nn.Conv2d, nn.Conv3d)):
+                n += 1 + (m.bias is not None)
+    return n
+
+
+def _check_layout(module, entry):
+    assert type(module).__name__ == entry["class"]
+    sd = module.state_dict()
+    assert list(sd.keys()) == entry["keys"], entry["class"]
+    assert [list(v.shape) for v in sd.values()] == entry["shapes"], entry["class"]
+
+
+def test_kitti_factory_builds_our_decoders_and_trainer_param_groups_accept_them():
+    """Every configuration of make_depth_decoder (wavelets, sparse, dense): the class the factory builds, its state dict,
+    ``.convs`` and group_weight's parameter count, and strict loading both ways."""
+    for case, entry in sorted(LAYOUT["kitti"].items()):
+        dec = _kitti_decoder(case)
+        _check_layout(dec, entry)
+        assert [list(k) if isinstance(k, tuple) else k for k in dec.convs.keys()] == entry["convs"], case   # JSON: tuples as lists
+        assert _grouped_params(dec.convs) == entry["grouped_params"] == len(list(dec.parameters())) > 0, case
+        ref_sd = _reference_state_dict(entry, seed=1)
+        dec.load_state_dict(ref_sd, strict=True)                     # reference checkpoint -> ours
+        twin = _kitti_decoder(case)
+        twin.load_state_dict(dec.state_dict(), strict=True)          # ours -> a module with the reference's layout
+        for k, v in ref_sd.items():
+            assert torch.equal(twin.state_dict()[k], v), (case, k)
+
+
+def test_kitti_checkpoints_round_trip_on_disk_through_the_trainers_code_path(tmp_path):
+    entry = LAYOUT["kitti"]["sparse"]
+    ours = _kitti_decoder("sparse")
+    # trainer.save_model (:733-751): torch.save(model.state_dict(), "<name>.pth"); the reference module's file
     torch.save(ours.state_dict(), tmp_path / "depth.pth")
-    torch.save(theirs.state_dict(), tmp_path / "depth_ref.pth")
-    # test_simple.py:101-102: strict load of depth.pth
+    torch.save(_reference_state_dict(entry, seed=2), tmp_path / "depth_ref.pth")
+    # test_simple.py:101-102: strict load of depth.pth into a module with the reference's layout
+    theirs = _kitti_decoder("sparse")
     theirs.load_state_dict(torch.load(tmp_path / "depth.pth", map_location="cpu"))
     for k, v in ours.state_dict().items():
         assert torch.equal(theirs.state_dict()[k], v), k
@@ -123,10 +96,10 @@ def test_kitti_checkpoints_round_trip_on_disk_through_the_trainers_code_path(kit
     ours.load_state_dict(torch.load(tmp_path / "depth_ref.pth"), strict=False)
 
 
-def test_swapped_kitti_decoder_fails_loudly_without_cuda(kitti_tree):
+def test_swapped_kitti_decoder_fails_loudly_without_cuda():
     if torch.cuda.is_available():
         pytest.skip("CUDA present")
-    _, kd = _swap_kitti()
+    from wavelet_monodepth_b200 import kitti_decoders as kd
     from wavelet_monodepth_b200._lib import WmdError
     dec = kd.SparseDepthWaveProgressiveDecoder(_Encoder.num_ch_enc)
     feats = [torch.rand(1, c, 6 << (4 - k), 20 << (4 - k)) for k, c in enumerate(_Encoder.num_ch_enc)]
@@ -134,62 +107,32 @@ def test_swapped_kitti_decoder_fails_loudly_without_cuda(kitti_tree):
         dec(feats, 0.05)
 
 
-def _nyu_opts(**kw):
-    o = argparse.Namespace(encoder_type="densenet", normalize_input=False, pretrained_encoder=False, num_layers=18,
-                           use_wavelets=True, use_sparse=False, use_224=False, dw_waveconv=False, dw_upconv=False)
-    o.__dict__.update(kw)
-    return o
-
-
-def test_nyu_model_builds_our_decoders_and_load_save_utils_round_trip(nyu_tree, tmp_path, capsys):
-    import networks.decoders as dec
+def test_nyu_model_builds_our_decoders_and_load_save_utils_round_trip(tmp_path):
+    """Every decoder NYUv2 Model builds (wavelets, sparse, 224 variants, dense): class, state dict, strict loading both
+    ways and a save / load round trip on disk."""
     from wavelet_monodepth_b200 import nyu_decoders as nd
-    ref = {n: getattr(dec, n) for n in ("Decoder", "DecoderWave", "Decoder224", "DecoderWave224", "SparseDecoderWave")}
-    for n in ref:                                                    # INTEGRATION.md A, line 2
-        setattr(dec, n, getattr(nd, n))
-    from model import Model                                          # unmodified NYUv2/model.py
-    import load_save_utils                                           # unmodified NYUv2/load_save_utils.py
-    cases = ((_nyu_opts(), nd.DecoderWave), (_nyu_opts(use_sparse=True), nd.SparseDecoderWave),
-             (_nyu_opts(use_224=True), nd.DecoderWave224), (_nyu_opts(use_wavelets=False), nd.Decoder),
-             (_nyu_opts(use_wavelets=False, use_224=True), nd.Decoder224))
-    enc_ch = None
-    for opts, cls in cases:
-        m = Model(opts)
-        assert type(m.decoder) is cls
-        enc_ch = list(m.encoder.num_ch_enc)
-        theirs = ref[cls.__name__](enc_features=enc_ch, decoder_width=0.5)
-        assert list(m.decoder.state_dict().keys()) == list(theirs.state_dict().keys()), cls.__name__
-        assert [tuple(v.shape) for v in m.decoder.state_dict().values()] == \
-               [tuple(v.shape) for v in theirs.state_dict().values()]
-        m.decoder.load_state_dict(theirs.state_dict(), strict=True)
-        theirs.load_state_dict(m.decoder.state_dict(), strict=True)
-    # the reference's own save_model / load_model on a model that carries our decoder, then into a pure-reference twin
-    m = Model(_nyu_opts(use_sparse=True))
-    load_save_utils.save_model(m, str(tmp_path), 3)                  # writes models/weights_3/model.pth
-    folder = os.path.join(str(tmp_path), "models", "weights_3")
-    import model as model_module
-    for n in ref:                                                    # back to the reference's classes (model.py bound
-        setattr(model_module, n, ref[n])                             # the names at import time)
-    twin = Model(_nyu_opts(use_sparse=True))
-    assert type(twin.decoder) is ref["SparseDecoderWave"]
-    load_save_utils.load_model(twin, folder)
-    for k, v in m.state_dict().items():
-        assert torch.equal(twin.state_dict()[k], v), k
-    load_save_utils.save_model(twin, str(tmp_path), 4)
-    load_save_utils.load_model(m, os.path.join(str(tmp_path), "models", "weights_4"))
-    capsys.readouterr()
+    for case, entry in sorted(LAYOUT["nyu"].items()):
+        cls = getattr(nd, entry["class"])
+        dec = cls(enc_features=entry["enc_features"], decoder_width=0.5)
+        _check_layout(dec, entry)
+        ref_sd = _reference_state_dict(entry, seed=3)
+        dec.load_state_dict(ref_sd, strict=True)
+        path = tmp_path / ("%s.pth" % case)
+        torch.save(dec.state_dict(), path)                           # load_save_utils.save_model / load_model pattern
+        twin = cls(enc_features=entry["enc_features"], decoder_width=0.5)
+        twin.load_state_dict(torch.load(path), strict=True)
+        for k, v in ref_sd.items():
+            assert torch.equal(twin.state_dict()[k], v), (case, k)
 
 
-def test_functional_api_names_match_the_reference_layers(kitti_tree):
+def test_functional_api_names_match_the_reference_layers():
     """Every public name of the hot path in KITTI/layers.py exists with the same parameter names here."""
     import inspect
-    import layers as ref_layers
     from wavelet_monodepth_b200 import kitti_layers as kl
-    for name in ("Conv3x3", "Conv1x1", "ConvBlock", "upsample", "sparse_select", "make_result", "mask2yx", "mask2idxmap",
-                 "sparse_conv1x1", "sparse_conv3x3", "sparse_upsample"):
-        a, b = getattr(ref_layers, name), getattr(kl, name)
-        if inspect.isclass(a):
+    for name, pa in LAYOUT["kitti_layer_signatures"].items():
+        b = getattr(kl, name)
+        if inspect.isclass(b):
             assert issubclass(b, nn.Module)
-            a, b = a.__init__, b.__init__
-        pa, pb = list(inspect.signature(a).parameters), list(inspect.signature(b).parameters)
+            b = b.__init__
+        pb = list(inspect.signature(b).parameters)
         assert pa == pb[:len(pa)], (name, pa, pb)

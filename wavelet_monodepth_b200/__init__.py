@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of the wavelet-monodepth decoder hot path.
+"""H100-native (sm_90a) implementation of the wavelet-monodepth decoder hot path.
 
 Public surface = the reference's (nianticlabs/wavelet-monodepth) own API for this path:
 

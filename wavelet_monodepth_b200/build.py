@@ -1,8 +1,8 @@
-"""Build libwmd.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libwmd.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m wavelet_monodepth_b200.build [--force] [--verbose]
 
-The shared library is git-ignored but travels to the GPU box with the snapshot.
+The shared library is a build product (git-ignored); build() or this module rebuilds it whenever a source is newer.
 """
 import glob
 import os
@@ -15,8 +15,8 @@ REPO = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libwmd.so")
 
-NVCC_FLAGS = (["-DWMD_TC_DEBUG"] if os.environ.get("WMD_TC_DEBUG") else []) + [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = [
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared",
 ]
 

@@ -1,4 +1,4 @@
-// Shared helpers for libwmd (sm_100a).  Host-side error plumbing + small device utilities.
+// Shared helpers for libwmd (sm_90a).  Host-side error plumbing + small device utilities.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,209 +1,197 @@
-// K5-TC: the gather-GEMM convolution on 5th-gen tensor cores (tcgen05 + TMEM), fp32-faithful via 3xTF32.
+// K5-TC: the gather-GEMM convolution on Hopper tensor cores (wgmma), fp32-faithful via 3xTF32.
 //
-// Same contract as conv_rows_kernel (conv.cu), different engine.  One CTA per SM owns a 256 x N output tile
-// (two UMMA M=128 halves sharing one B tile, N = 128 / 64 / 32) and walks K = (c0 + c1) x taps in 32-channel chunks,
-// the taps of a channel chunk innermost (their source rows overlap: L2 hits).
-// Warp-specialised, mbarrier-pipelined (no CTA-wide barrier inside the K loop):
+// Same contract as conv_rows_kernel (conv.cu), different engine.  A persistent grid (at most one CTA per SM) walks
+// 128 x N output tiles (N = 128 / 64 / 32); a tile's reduction K = (c0 + c1) x taps runs in 32-channel chunks, the
+// taps of a channel chunk innermost (their source rows overlap: L2 hits).  256 threads = two warpgroups, warpgroup h
+// owns tile rows h*64 .. h*64+63 (one wgmma M = 64 each, both share the chunk's weight tile).
 //
-//   gather warps (8-12)
-//     * implicit im2col by the TMA: `cp.async.bulk.tensor.2d...tile::gather4` fetches the 128-byte channel slice of
-//       four arbitrary source rows (indices from the per-tile tap table; row -1 = inactive / padded tap and the
-//       channel tail are zero-filled by the TMA) into a raw fp32, 128B-swizzled shared tile, completion by mbarrier
-//       transaction bytes.  3x3 layers: one fill per (chunk, dy) serves the three dx taps (shared-tap form, below);
-//       1x1 stages over consecutive rows: one tiled load of the whole 256-row box;
-//   weight loader (warp 13)
+//   gather (all 256 threads), TC_STAGES - 1 chunks ahead of the MMAs, cp.async with zero fill
+//     * implicit im2col: the 128-byte channel slice of each tile row's source row (row from the per-tile tap table,
+//       -1 = inactive / padded tap, and the channel tail read zeros) into a raw fp32 stage padded to 144-byte rows, so
+//       that the fragment reads below are free of bank conflicts;
 //     * B (weights) is pre-split, pre-swizzled by wmd_pack_conv_weight_tc_f32 into one [hi | lo] image per (n-tile,
-//       chunk): a single cp.async.bulk per chunk into a 3- or 4-deep ring, B_STAGES - 1 chunks ahead of the MMAs;
-//   split warps (0-7), thread = tile row = TMEM lane
-//     * read the row's 128 bytes back (the swizzle makes this transposed read conflict-free), split x = hi + lo
-//       (hi = x with the 13 low mantissa bits cleared, lo = x - hi: exact) and write hi / lo into TENSOR MEMORY with
-//       tcgen05.st - the MMAs take A from TMEM (".ts" form), because an SS-mode M=128 x N=128 MMA would need the
-//       full 128 B/clk of shared-memory bandwidth three times per k-step;
-//   issuers (warps 14-15, one per M half = one per accumulator)
-//     * whole warp in the loop, one elected lane issues: 4 k-steps x 3 terms (lo*hi + hi*lo + hi*hi) per chunk, then
-//       commits to the mbarriers that recycle the TMEM A stage / shared B stage;
-//   all 16 warps
-//     * the tensor core's fp32 accumulation rounds toward zero, a bias that grows linearly with K (measured
-//       ~6.5e-9 * K relative).  So accumulation runs in EPOCHS of kFlushChunks chunks: a finished epoch is drained
-//       (tcgen05.ld) into per-thread fp32 registers with round-to-nearest adds and the TMEM accumulators are
-//       re-zeroed.  Each thread ends up owning one output row x N/2 channels: bias + activation (picked once per tile,
-//       vector bias loads: the epilogue is instruction bound) + one contiguous store;
-//     * balanced scheduling (long reductions): whole tiles for the full rounds, the (tile, chunk) units of the remainder
-//       dealt out evenly on the device (stream-K); the last segment of a cut tile to arrive sums all segments in slab
-//       order, cooperatively and coalesced.
-// What bounds it (scripts/tc_layer_trace.py, scripts/tc_ablate.py, DESIGN.md 4): the tensor pipe.  24 UTCHMMAs per chunk
-// cost 64 clk each at N = 128 (1536 clk) and ~52 clk at any N <= 64 (an instruction-rate floor); the feed - A 16 KB
-// (shared-tap) + B 32 KB per chunk through an L2 that delivers ~45 B/clk per SM when all SMs stream - fits under it.
-// Optional fp16-pair operand form (F16 = true, wmd_conv_desc.precision): x 2^e = h1 + h2 as fp16, kind::f16 MMAs with K = 16
+//       chunk): K-major, 128-byte swizzled, read by the wgmma straight from shared memory through a descriptor;
+//   multiply (per warpgroup)
+//     * every thread reads its A fragment elements (rows g, g + 8 of its warp's 16, channels t, t + 4 of each k-step)
+//       and splits x = hi + lo (hi = x with the 13 low mantissa bits cleared, lo = x - hi: exact) in registers - the
+//       register-A form of wgmma, so the split never goes back to shared memory;
+//     * 4 k-steps x 3 terms (lo*hi + hi*lo + hi*hi) per chunk, committed and waited as one group;
+//     * the tensor core's fp32 accumulation is not round-to-nearest, a bias that grows with K.  So accumulation runs in
+//       EPOCHS of kFlushChunks chunks: the first MMA of an epoch overwrites the wgmma accumulators, the epoch's end adds
+//       them into per-thread fp32 registers with round-to-nearest adds;
+//   epilogue: bias + activation (picked once per tile) + pair stores;
+//   balanced scheduling (long reductions): whole tiles for the full rounds, the (tile, chunk) units of the remainder
+//     dealt out evenly on the device (stream-K); the last segment of a cut tile to arrive sums all segments in slab
+//     order, cooperatively and coalesced.
+// Optional fp16-pair operand form (F16 = true, wmd_conv_desc.precision): x 2^e = h1 + h2 as fp16, f16 MMAs with K = 16
 // (half the instructions), scale from the sources' max |x| (device scalars), weights' scale in the packed image's header.
-// Shared-tap gather (SH = true, every 3x3 layer): the three dx taps of a (channel chunk, dy) read almost the same source
-// rows - tap dx of tile row r is tap 0 of row r + dx whenever the two output pixels are neighbours in the active list.
-// One raw stage fill per (chunk, dy) therefore serves THREE chunks: slots 0..255 hold the dx = 0 sources of the tile's
-// rows, slots 256.. the few "extra" rows that no centre tap fetches (run ends, list gaps); a per-tile slot table
-// (uint16 per (source, dy, side, row)) tells the split warps which slot feeds each row of the dx = +-1 chunks.  The
-// L2->SM traffic of the A operand and the TMA gather4 count drop ~3x (measured intake limit: ~45 B/clk/SM, at which
-// re-gathering every tap bounds all layers with N <= 64).  A tile whose extras overflow (isolated pixels: > 128 per
-// (source, dy)) falls back to one fill per chunk with identity slots - same code, group size 1.
-// TMEM map (512 columns): [0,2N) accumulators (half h at h*N), [A_COL0,512) A operand: tf32 form stage s, half h at
-// A_COL0 + s*128 + h*64, hi in the first 32 columns, lo in the next 32 (2 stages at N = 128, 3 below); f16 form stage s,
-// half h at A_COL0 + s*64 + h*32, h1 in the first 16 columns, h2 in the next 16 (4 stages).
 #include <cuda_fp16.h>
-#include <cuda.h>   // CUtensorMap + enums only; the encoder is fetched through cudaGetDriverEntryPoint (no -lcuda)
 
 #include "common.cuh"
 
 namespace wmd {
 
-constexpr int TC_BM = 256;                      // rows per CTA tile = 2 UMMA halves of 128
-constexpr int TC_BK = 32;                       // floats per chunk = one 128-byte swizzle-atom row
-constexpr int TC_THREADS = 512;                 // 16 warps: 8 split + 5 gather + 1 weight loader + 2 issuers; all drain (lane quarter w&3, half (w>>2)&1, cols w>>3)
-constexpr int TC_SPLIT_WARPS = 8;               // warps 0-7: warp w owns tile rows (w>>2)*128 + (w&3)*32 + lane (its TMEM lane quarter)
-constexpr int TC_GATHER_WARPS = 5;              // warps 8-12
-constexpr int TC_WLOAD_WARP = 13;               // warp 13: weight (B) loader - keeps the issuers' loop free of the stage-reuse wait
-constexpr int TC_ISSUERS = 2;                   // warps 14-15: one per M half, each the only writer of its accumulator
-constexpr int TC_A_STAGES = 3;                  // raw A tiles in shared memory (two gathers in flight + one being split)
-constexpr int TC_T_STAGES_MAX = 4;              // split A stages in tensor memory: 2 (N = 128) or 3 (N <= 64), 4 in the f16 form, see TcCfg
-constexpr int TC_B_STAGES_MAX = 4;              // [Bhi | Blo] images in shared memory: 3 (N = 128) or 4 (N <= 64)
-constexpr int TC_A_TILE = TC_BM * TC_BK * 4;    // 32 KB raw fp32
+constexpr int TC_BM = 128;                      // rows per CTA tile = 2 warpgroups x wgmma M = 64
+constexpr int TC_BK = 32;                       // floats per chunk = one 128-byte row of a weight image
+constexpr int TC_THREADS = 256;                 // two warpgroups: both gather, each multiplies its 64 rows
+constexpr int TC_STAGES = 4;                    // cp.async ring: three chunks in flight while one is multiplied
+constexpr int TC_A_LD = TC_BK + 4;              // raw A row pitch in floats (144 B: fragment reads hit 32 distinct banks)
+constexpr int TC_A_TILE = TC_BM * TC_A_LD * 4;  // 18 KB raw fp32
 constexpr int TC_TABLES = 2 * 9 * TC_BM * 4;
-constexpr int TC_TMEM_COLS = 512;
-// shared-tap gather (SH): 2 raw stages of 256 tile rows + 128 extra rows
-constexpr int TC_SH_STAGES = 2;
-constexpr int TC_SH_EXTRA = 128;
-constexpr int TC_SH_ROWS = TC_BM + TC_SH_EXTRA;
-constexpr int TC_SH_TILE = TC_SH_ROWS * 128;     // 48 KB
-constexpr int TC_SH_TABLES = 2 * 3 * TC_SH_EXTRA * 4 /* extra source rows */ + 2 * 3 * 2 * TC_BM * 2 /* slots */ + 64 /* counters */;
-constexpr uint16_t kZeroSlot = 0xFFFFu;          // slot-table entry of a tap that reads nothing (inactive / padded source)
 
-// Per N-tile configuration.  Accumulators: M half h at TMEM column h*BN; each is written by exactly one issuer, so the
-// order of the round-toward-zero accumulations - and with it every output bit - is fixed.
-template <int BN, bool SH = false, bool F16 = false>
+// Per N-tile configuration.  A stage holds the chunk's weight image first (its size is a multiple of 4 KB, so every image
+// keeps the 1024-byte alignment of the 128-byte swizzle) and the raw A rows after it.
+template <int BN, bool F16 = false>
 struct TcCfg {
   static constexpr int B_TILE = BN * TC_BK * 4;            // bytes of one of hi / lo (tf32 form)
   // weight image of one chunk: tf32 form [hi: BN x 128 B | lo: BN x 128 B]; f16 form ONE BN x 128 B tile whose rows hold
   // [h1: 32 channels | h2: 32 channels] as fp16
   static constexpr int B_IMG = F16 ? B_TILE : 2 * B_TILE;
-  static constexpr int ACC = BN / 2;                       // accumulator registers per thread: its row x BN/2 columns
-  static constexpr int A_BYTES = SH ? TC_SH_STAGES * TC_SH_TILE : TC_A_STAGES * TC_A_TILE;   // 96 KB either way
-  // Pipeline depth.  The loop split(c) -> MMA(c) -> [TMEM stage free] -> split(c + T) and the weight prefetch
-  // MMA(c-1) done -> load B(c + B - 1) -> MMA(c + B - 1) make the chunk period max(issue, split, (issue + split) / (T-1)...,
-  // (issue + L2 latency) / (B - 1)).  At N = 128 the MMA issue (12 x 64 clk) hides both with T = 2 / B = 3 and TMEM / shared
-  // memory are full; at N <= 64 the issue is short (12 x ~35 clk per half) and the measured period was twice it
-  // (scripts/tc_layer_trace.py: 1715 clk vs 960 of issue), so those tiles take a third A stage (TMEM columns 128..511 are
-  // free next to <= 128 accumulator columns) and a fourth weight stage.
-  // f16 form: a stage is half as wide (per M half 16 columns of h1 + 16 of h2), so four fit at every N and the split
-  // warps never wait for the MMAs of an earlier chunk; its weight images are half as large: four stages as well.
-  static constexpr int A_STAGE = F16 ? 64 : 128;                    // TMEM columns of one split A stage (both M halves)
-  static constexpr int T_STAGES = F16 ? 4 : (BN <= 64 ? 3 : 2);
-  static constexpr int B_STAGES = (F16 || BN <= 64) ? 4 : 3;
-  static constexpr uint32_t A_COL0 = 512u - T_STAGES * A_STAGE;     // first TMEM column of the split A operand
-  static constexpr size_t SMEM = static_cast<size_t>(A_BYTES) + static_cast<size_t>(B_STAGES) * B_IMG + TC_TABLES +
-                                 (SH ? TC_SH_TABLES : 0) + 1024;
-  static_assert(2 * BN <= static_cast<int>(A_COL0), "accumulators must leave the A operand's TMEM columns free");
+  static constexpr int ACC = BN / 2;                       // accumulator registers per thread (wgmma m64 x BN fragment)
+  static constexpr int STAGE = B_IMG + TC_A_TILE;
+  static constexpr size_t SMEM = static_cast<size_t>(TC_STAGES) * STAGE + TC_TABLES + 1024;
+  static_assert(STAGE % 1024 == 0, "weight images must stay 1024-byte aligned");
+  static_assert(SMEM <= 227 * 1024, "one CTA must fit the shared memory of an SM");
 };
-#ifndef WMD_TC_EXP
-#define WMD_TC_EXP 0                              // timing ablations of scripts/tc_ablate.py (non-zero: results are WRONG)
-#endif
-constexpr int kFlushChunks = 32;                // epoch length: K = 1024 per TMEM accumulation run
-constexpr int32_t kNoRow = -1;                  // tap-table entry of an inactive / padded source: an out-of-bounds TMA row reads zeros
+constexpr int kFlushChunks = 32;                // epoch length: K = 1024 per wgmma accumulation run
+constexpr int32_t kNoRow = -1;                  // tap-table entry of an inactive / padded source: the gather writes zeros
 
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count));
-}
-#ifdef WMD_TC_DEBUG
-__device__ unsigned int g_dbg[4];
-#define MBAR_FAIL(id) do { if (atomicCAS(&g_dbg[0], 0u, (id)) == 0u) { g_dbg[1] = blockIdx.x; g_dbg[2] = threadIdx.x; } return; } while (0)
-#define MBAR_SPINS (1u << 21)
-#else
-#define MBAR_FAIL(id) __trap()
-#define MBAR_SPINS (1u << 28)
-#endif
-// -DWMD_TC_TRACE (scripts/tc_trace.py builds a separate library): CTA 0 records clock64() at fixed points of the
-// first kTraceChunks chunks for split warp 0, gather warp 8 and issuer 0.
-#ifdef WMD_TC_TRACE
-constexpr int kTraceChunks = 256, kTraceSlots = 8;
-__device__ long long g_trace[3 * kTraceSlots * kTraceChunks];
-#define TC_TRACE(role, slot, c) do { if (blockIdx.x == 0 && lane == 0 && (c) < kTraceChunks) \
-    g_trace[((role) * kTraceSlots + (slot)) * kTraceChunks + (c)] = clock64(); } while (0)
-// per-tile timeline of CTA 0 (thread 0 = split warp 0): tile top, tables built, first raw A landed, chunk loop done,
-// last epoch complete, drained, stored, end-of-tile barrier passed
-constexpr int kTraceTiles = 64, kTileSlots = 12;   // slots 8..10: inside the table build (init, tap tables, slot tables)
-__device__ long long g_tile_trace[kTraceTiles * kTileSlots];
-#define TC_TILE_TRACE(slot) do { if (blockIdx.x == 0 && tid == 0 && tile_iter < kTraceTiles) \
-    g_tile_trace[tile_iter * kTileSlots + (slot)] = clock64(); } while (0)
-#else
-#define TC_TRACE(role, slot, c) do {} while (0)
-#define TC_TILE_TRACE(slot) do {} while (0)
-#endif
-// bounded spin: a protocol bug traps instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, uint32_t id = 0) {
-  uint32_t done = 0;
-  for (uint32_t spin = 0; spin < MBAR_SPINS; ++spin) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}\n"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (done) return;
-  }
-  MBAR_FAIL(id);
-}
-// one non-blocking look (per-lane result; the user votes when it consumes it).  Issued a few hundred clocks before the
-// answer is needed - the ~200 clk round trip of a barrier query then overlaps other work; a `false` just means the
-// blocking wait still has to run
-__device__ __forceinline__ uint32_t mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(done)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return done;
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory");
-}
+// cp.async writes through the generic proxy, wgmma reads shared memory through the async proxy
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+// keeps a register that an asynchronous wgmma reads or writes live and unmoved across the wait
+__device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 "version 1"); rows are 128 bytes, 8-row groups
-// are 1024 bytes apart (SBO), LBO is the canonical 1 for swizzled K-major operands.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma); rows are 128 bytes, 8-row groups are 1024 bytes
+// apart (SBO), LBO is unused by swizzled K-major operands.  A k-step inside the 128-byte row advances the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// D[tmem] (+)= A[tmem] * B[smem]^T : A is 128 lanes x 8 tf32 columns in tensor memory, B a K-major smem tile
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-// same with fp16 operands (kind::f16): A is 128 lanes x 16 halves = 8 columns in tensor memory
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
+// D (+)= A * B^T for one warpgroup: D = 64 x BN fp32 fragment, A = 64 x K fragment in registers (tf32: K = 8, f16: K = 16),
+// B = K-major shared-memory tile behind `bdesc`.  scale_d == 0 overwrites D.
+template <int BN, bool F16>
+struct Wgmma;
+template <> struct Wgmma<128, false> {
+  static __device__ __forceinline__ void mma(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+};
+template <> struct Wgmma<64, false> {
+  static __device__ __forceinline__ void mma(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+};
+template <> struct Wgmma<32, false> {
+  static __device__ __forceinline__ void mma(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+};
+template <> struct Wgmma<128, true> {
+  static __device__ __forceinline__ void mma(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+};
+template <> struct Wgmma<64, true> {
+  static __device__ __forceinline__ void mma(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+};
+template <> struct Wgmma<32, true> {
+  static __device__ __forceinline__ void mma(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+        "}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d)
+        : "memory");
+  }
+};
+
 // two floats -> packed fp16 pair, round to nearest even, saturating at +-65504 (a stray out-of-range value must not turn
 // into inf - inf = NaN in the remainder piece); `lo` lands in bits 0..15 (the lower K index)
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
@@ -221,15 +209,6 @@ __device__ __forceinline__ float f16_hi_to_f32(uint32_t pair) {
   asm("{\n\t.reg .f16 l, h;\n\tmov.b32 {l, h}, %1;\n\tcvt.f32.f16 %0, h;\n\t}\n" : "=f"(f) : "r"(pair));
   return f;
 }
-// one lane of a converged warp
-__device__ __forceinline__ bool elect_one() {
-  uint32_t p;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}\n" : "=r"(p));
-  return p != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
-}
 
 __device__ __forceinline__ float tf32_rna(float x) {
   uint32_t r;
@@ -237,54 +216,12 @@ __device__ __forceinline__ float tf32_rna(float x) {
   return __uint_as_float(r);
 }
 
-// this thread's TMEM lane (warp quarter base + lane), 8 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};\n" ::"r"(taddr), "r"(v[0]),
-               "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-      "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_zero16(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};\n" ::"r"(taddr),
-      "r"(z)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  // the load and its wait are ONE asm statement: with two, the compiler may schedule uses of v[] between them (the wait
-  // has no register dependence on the load's outputs) and read registers the asynchronous load has not written yet -
-  // seen as a timing-dependent wrong accumulator slice on a cold first launch
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar)
-      : "memory");
-}
-
 // Balanced mode plan, shared by the conv kernel and the reduce pass (both derive it from the device-side row count).
 // All but the last full round of tiles run data-parallel (whole tiles); the last full round and the partial round
 // after it - between 1 and 2 x CTAs - 1 tiles - are cut stream-K style into equal ranges of U units per CTA.  Merging
 // the last full round in keeps the ranges long (>= one tile's reduction), so a tile has <= 2 segments; only when
 // there is no full round at all (fewer tiles than CTAs) the ranges are shorter: U >= nchunks/6, <= 7 segments.
-constexpr int kBalSlabs = 8;                    // workspace slabs: CTAs x kBalSlabs tiles of 256 x N floats
+constexpr int kBalSlabs = 8;                    // workspace slabs: CTAs x kBalSlabs tiles of TC_BM x N floats
 constexpr int kBalCounterBytes = 4096;          // balanced mode: per stream-K tile arrival counters at the head of the workspace
 struct BalPlan {
   long long rem_tile0;                          // first stream-K tile
@@ -304,67 +241,21 @@ __host__ __device__ __forceinline__ BalPlan bal_plan(long long tiles, long long 
   return p;
 }
 
-template <int BN, bool SH, bool F16>
+template <int BN, bool F16>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_conv_desc d, const float* __restrict__ wtc,
-                                                                     const int splits, float* __restrict__ partial,
-                                                                     const __grid_constant__ CUtensorMap tm0,
-                                                                     const __grid_constant__ CUtensorMap tm1) {
-  using Cfg = TcCfg<BN, SH, F16>;
+                                                                     const int splits, float* __restrict__ partial) {
+  using Cfg = TcCfg<BN, F16>;
   constexpr int TC_B_TILE = Cfg::B_TILE;
   constexpr int B_IMG = Cfg::B_IMG;                         // bytes of one chunk's weight image
   constexpr int ACC = Cfg::ACC;
-  constexpr int TC_T_STAGES = Cfg::T_STAGES;
-  constexpr int TC_B_STAGES = Cfg::B_STAGES;
+  constexpr int STAGE = Cfg::STAGE;
   extern __shared__ unsigned char smem_dyn[];
-  __shared__ __align__(8) uint64_t bar_raw_full[TC_A_STAGES];   // raw A tile of the stage has landed (TMA transaction bytes)
-  __shared__ __align__(8) uint64_t bar_raw_empty[TC_A_STAGES];  // ... has been read by the 8 split warps
-  __shared__ __align__(8) uint64_t bar_asplit[TC_T_STAGES_MAX]; // split A of the TMEM stage is stored (8 split warps)
-  __shared__ __align__(8) uint64_t bar_mma[TC_T_STAGES_MAX];    // chunk's MMAs done (2 issuers): TMEM A stage + B stage reusable
-  __shared__ __align__(8) uint64_t bar_b[TC_B_STAGES_MAX]; // weight image of the stage has landed (bulk copy)
-  __shared__ __align__(8) uint64_t bar_bfree[TC_B_STAGES_MAX];  // chunk's MMAs done (2 issuers): weight stage reusable
-  __shared__ __align__(8) uint64_t bar_epoch;              // accumulation epoch complete (4 issuers)
-  __shared__ uint32_t tmem_base_slot;
   __shared__ int s_fixup;                                  // balanced mode: segments of the tile to reduce here (0 = not the last)
 
-  // warp index through a shuffle: provably warp-uniform, so the role branches and everything the issuer warps
-  // compute from it stay on the uniform datapath (see the issuer section)
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~static_cast<uintptr_t>(1023));
-  unsigned char* sA_base = base;
-  unsigned char* sB_base = base + Cfg::A_BYTES;
-  int32_t* tab0 = reinterpret_cast<int32_t*>(sB_base + TC_B_STAGES * B_IMG);   // [tap][row]: source row in x0, -1 = none
-  int32_t* tab1 = tab0 + 9 * TC_BM;                                                    // ... in x1
-  // shared-tap gather tables (SH): extra source rows [src][dy][128], slots [src][dy][side][row], counters [src*3+dy], [6] = overflow
-  int32_t* xtra = tab1 + 9 * TC_BM;
-  uint16_t* slots = reinterpret_cast<uint16_t*>(xtra + 2 * 3 * TC_SH_EXTRA);
-  int* nx = reinterpret_cast<int*>(slots + 2 * 3 * 2 * TC_BM);
-
-  if (tid == 0) {
-    for (int s = 0; s < TC_A_STAGES; ++s) {
-      mbar_init(smem_u32(&bar_raw_full[s]), 1);               // one expect_tx arrival; the gathers complete the bytes
-      mbar_init(smem_u32(&bar_raw_empty[s]), TC_SPLIT_WARPS);
-    }
-    for (int s = 0; s < TC_T_STAGES; ++s) {
-      mbar_init(smem_u32(&bar_asplit[s]), TC_SPLIT_WARPS);
-      mbar_init(smem_u32(&bar_mma[s]), TC_ISSUERS);
-    }
-    for (int s = 0; s < TC_B_STAGES; ++s) {
-      mbar_init(smem_u32(&bar_b[s]), 1);
-      mbar_init(smem_u32(&bar_bfree[s]), TC_ISSUERS);
-    }
-    mbar_init(smem_u32(&bar_epoch), TC_ISSUERS);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&tmem_base_slot)),
-                 "r"(static_cast<uint32_t>(TC_TMEM_COLS))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = tmem_base_slot;
+  int32_t* tab0 = reinterpret_cast<int32_t*>(base + TC_STAGES * STAGE);   // [tap][row]: source row in x0, -1 = none
+  int32_t* tab1 = tab0 + 9 * TC_BM;                                        // ... in x1
 
   // F16: operands are fed as fp16 pairs.  Activations are scaled by a power of two chosen from the sources' max |x| (device
   // scalars written by their producers: layout moves, earlier convolutions) so that max |x| s lies in (2^13, 2^14] - no
@@ -395,29 +286,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   const long long tiles = static_cast<long long>((rows + TC_BM - 1) / TC_BM) * n_tiles;
   const int Hs = d.H >> d.shift0, Ws = d.W >> d.shift0;
   const bool aligned_rows = (d.taps == 1 && d.map0 == nullptr);
-  const bool tiled_rows = aligned_rows && d.rows0 > 0;         // tm0 then has a 256-row box (launch_tc)
-  // instruction descriptor: D=f32, A=B=tf32, both K-major, N = BN, M = 128
-  // (F16: A = B = f16, format code 0, K = 16 per instruction)
-  constexpr uint32_t kFmt = F16 ? 0u : 2u;
-  constexpr uint32_t kIdesc = (1u << 4) | (kFmt << 7) | (kFmt << 10) | (static_cast<uint32_t>(BN >> 3) << 17) |
-                              (static_cast<uint32_t>(128 >> 4) << 24);
+  // rows each source holds: a row index past them reads zeros (a 1x1 stage over its own rows may run past x0's end)
+  const long long rows_x0 = (aligned_rows && d.rows0 > 0) ? d.rows0 : static_cast<long long>(d.N) * Hs * Ws;
+  const long long rows_x1 = static_cast<long long>(d.N) * HW;
 
-  // drain / store ownership (all 16 warps): TMEM lane quarter, M half, column half (ACC = BN/2 columns of every copy)
-  const int my_q = warp & 3, my_half = (warp >> 2) & 1, my_ch = warp >> 3;
-  const int my_row = my_half * 128 + my_q * 32 + lane;          // row within the CTA tile
-  const uint32_t lane_field = static_cast<uint32_t>(my_q * 32) << 16;
-  const uint32_t my_acc_addr = tmem_acc + lane_field + static_cast<uint32_t>(my_half * BN + my_ch * ACC);
-  uint32_t mma_rounds = 0;                                       // chunks issued so far by this CTA (all tiles)
-  uint32_t epochs = 0;                                           // epoch commits so far
-  uint32_t fill_rounds = 0;                                      // SH: raw-stage fills so far by this CTA (all tiles)
-
-  // accumulators start (and are left by every drain) at zero: every MMA accumulates
-#pragma unroll
-  for (int cc = 0; cc < ACC; cc += 16) tmem_zero16(my_acc_addr + static_cast<uint32_t>(cc));
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
+  // fragment ownership: warpgroup wg, warp wq of it; rows row_a and row_a + 8 of the tile, columns 8j + 2 t4 + {0, 1}
+  const int wg = warp >> 2, wq = warp & 3, t4 = lane & 3;
+  const int row_a = wg * 64 + wq * 16 + (lane >> 2);
 
   // Work decomposition.  A "unit" is one 32-channel chunk of one output tile.
   //   splits >= 1 : every tile's reduction is cut into `splits` equal ranges (split-K); splits == 1 = whole tiles.
@@ -436,9 +311,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   const long long u_end = balanced ? min(rem_units, u + U) : 0;
   long long item = blockIdx.x;
   const long long items = balanced ? rem_tile0 : tiles * splits;
-  int tile_iter = -1;
   while (true) {
-    ++tile_iter;
     long long tile;
     int cb, ce, slab;
     bool whole;
@@ -469,21 +342,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     const int m0 = static_cast<int>(tile / n_tiles) * TC_BM;
     const int nt = static_cast<int>(tile % n_tiles);
     const int n0 = nt * BN;
-    // rows / bias 16-byte aligned: the epilogue's vector form for the quads inside cout
-    const bool al_ok = (d.ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(d.y) & 15) == 0) &&
-                       ((reinterpret_cast<uintptr_t>(d.bias) & 15) == 0);
-    TC_TILE_TRACE(0);
+    // rows / bias 8-byte aligned: the epilogue's pair form for the pairs inside cout
+    const bool al_ok = (d.ldy % 2 == 0) && ((reinterpret_cast<uintptr_t>(d.y) & 7) == 0) &&
+                       ((reinterpret_cast<uintptr_t>(d.bias) & 7) == 0);
 
-    if (SH) {                                      // extras default to "no row" (the tail of a 4-row load group), counters to 0
-      for (int e = tid; e < 2 * 3 * TC_SH_EXTRA; e += TC_THREADS) xtra[e] = kNoRow;
-      if (tid < 8) nx[tid] = 0;
-    }
-    TC_TILE_TRACE(8);
-    // thread t: tile row t % 256, taps [t / 256 * 5, ...): the output pixel is read and decoded once per row, the taps'
+    // thread t: tile row t % 128, taps [t / 128 * 5, ...): the output pixel is read and decoded once per row, the taps'
     // gate / map lookups are independent loads
     {
       const int r = tid & (TC_BM - 1);
-      const int t_lo = (tid >> 8) * 5, t_hi = min(d.taps, t_lo + 5);
+      const int t_lo = (tid >> 7) * 5, t_hi = min(d.taps, t_lo + 5);
       const int m = m0 + r;
       int n = 0, y = 0, x = 0;
       const bool live = m < rows;
@@ -498,7 +365,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       // Two rounds of loads for the thread's (up to) five taps instead of one dependent chain per tap: first every tap's
       // coordinates and its three look-ups (gate byte, source-0 index map, source-1 index map) are issued together - the maps
       // are read whether or not the gate turns out to be set, their indices are valid for every in-range coordinate - then
-      // the results are combined.  (One tap at a time cost ~800 clk per tap: 3.3-5.0k clk of a 5-10k clk table build.)
+      // the results are combined.
       constexpr int kTapsPerThread = 5;
       int qv[kTapsPerThread];                        // source-1 pixel of the tap, -1 = out of range / dead row
       uint8_t gv[kTapsPerThread];
@@ -534,525 +401,182 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
         const int tap = t_lo + k;
         if (tap < t_hi) {
           const bool ok = qv[k] >= 0 && gv[k] != 0;
-          tab0[tap * TC_BM + r] = (ok && m0v[k] >= 0) ? m0v[k] : kNoRow;
-          tab1[tap * TC_BM + r] = ok ? m1v[k] : kNoRow;
+          tab0[tap * TC_BM + r] = (ok && m0v[k] >= 0 && m0v[k] < rows_x0) ? m0v[k] : kNoRow;
+          tab1[tap * TC_BM + r] = (ok && m1v[k] < rows_x1) ? m1v[k] : kNoRow;
         }
       }
     }
-    TC_TILE_TRACE(9);
     __syncthreads();
-    TC_TILE_TRACE(10);
-    // SH: slot tables of the dx = -1 / +1 taps.  Tap (dy, dx) of tile row r reads source row s; if the centre tap of row
-    // r + dx reads the same s (the two output pixels are neighbours in the list) the row is already in slot r + dx of the
-    // (chunk, dy) stage, otherwise it becomes an extra (slot 256 + k).  Extras past the capacity switch the whole tile to
-    // one fill per chunk (group size 1).
-    int gsz = 1;
-    if (SH) {
-      const int nsrc = d.c1 > 0 ? 2 : 1;
-      for (int e = tid; e < nsrc * 3 * 2 * TC_BM; e += TC_THREADS) {
-        const int r = e % TC_BM;
-        int t = e / TC_BM;
-        const int side = t & 1; t >>= 1;
-        const int dy = t % 3, src = t / 3;
-        const int dx = side ? 1 : -1;
-        const int32_t* tb = src ? tab1 : tab0;
-        const int32_t sidx = tb[(dy * 3 + 1 + dx) * TC_BM + r];
-        uint16_t slot = kZeroSlot;
-        bool extra = false;
-        if (sidx >= 0) {
-          const int rn = r + dx;
-          if (rn >= 0 && rn < TC_BM && tb[(dy * 3 + 1) * TC_BM + rn] == sidx) {
-            slot = static_cast<uint16_t>(rn);
-          } else {
-            extra = true;
-          }
-        }
-        // a warp's 32 entries share (source, dy, side): ONE shared-memory atomic per warp reserves its extras' slots
-        // (run ends are common in sparse tiles; one atomic per entry serialised on six counters)
-        const unsigned xm = __ballot_sync(0xffffffffu, extra);
-        if (xm) {
-          int base_k = 0;
-          if (lane == __ffs(xm) - 1) base_k = atomicAdd(&nx[src * 3 + dy], __popc(xm));
-          base_k = __shfl_sync(0xffffffffu, base_k, __ffs(xm) - 1);
-          if (extra) {
-            const int k = base_k + __popc(xm & ((1u << lane) - 1u));
-            if (k < TC_SH_EXTRA) {
-              xtra[(src * 3 + dy) * TC_SH_EXTRA + k] = sidx;
-              slot = static_cast<uint16_t>(TC_BM + k);
-            } else {
-              nx[6] = 1;
-            }
-          }
-        }
-        slots[((src * 3 + dy) * 2 + side) * TC_BM + r] = slot;
-      }
-      __syncthreads();
-      gsz = nx[6] ? 1 : 3;
-    }
-    // raw-stage fills of this segment: fill index (tile-relative) of chunk c is c / gsz
-    const int f0 = cb / gsz;
-    const int nfills = (ce - 1) / gsz - f0 + 1;
-    const uint32_t fround0 = fill_rounds;
-    TC_TILE_TRACE(1);
 
     const unsigned char* wtile = reinterpret_cast<const unsigned char*>(wtc) +
                                  (F16 ? 128 : 0) + static_cast<long long>(nt) * nchunks * B_IMG;   // f16 images follow a 128-byte header
-    const uint32_t round0 = mma_rounds;
+
+    // Chunk c of the tile into stage s: the weight image as it is, and the implicit im2col - for every tile row the
+    // 32-channel slice of its tap's source row (channel chunk outermost, taps innermost: the nine taps of a chunk re-read
+    // (almost) the same rows while they are hot in L2).  No row / channels past C: zero fill.
+    auto load_chunk = [&](int c, int s) {
+      unsigned char* st = base + s * STAGE;
+      const unsigned char* wsrc = wtile + static_cast<long long>(c) * B_IMG;
+#pragma unroll
+      for (int i = 0; i < B_IMG / 16 / TC_THREADS; ++i) {
+        const int o = (tid + i * TC_THREADS) * 16;
+        cp_async16(st + o, wsrc + o, 16);
+      }
+      const int rr = c / d.taps;
+      const int tap = c - rr * d.taps;
+      const bool src1 = rr >= nch0;
+      const int col = (src1 ? rr - nch0 : rr) * TC_BK;
+      const float* x = src1 ? d.x1 : d.x0;
+      const long long ld = src1 ? d.ld1 : d.ld0;
+      const int csrc = src1 ? d.c1 : d.c0;
+      const int32_t* tab = (src1 ? tab1 : tab0) + tap * TC_BM;
+      float* sa = reinterpret_cast<float*>(st + B_IMG);
+#pragma unroll
+      for (int i = 0; i < TC_BM * 8 / TC_THREADS; ++i) {
+        const int pc = tid + i * TC_THREADS, r = pc >> 3, q = pc & 7;
+        const int32_t srow = tab[r];
+        const int cc = col + 4 * q;
+        const int bytes = srow >= 0 ? min(16, max(0, (csrc - cc) * 4)) : 0;
+        cp_async16(sa + r * TC_A_LD + 4 * q, bytes ? x + srow * ld + cc : x, bytes);
+      }
+    };
 
     float acc[ACC];
 #pragma unroll
     for (int j = 0; j < ACC; ++j) acc[j] = 0.f;
+    float dacc[ACC];                              // the wgmma accumulators of the running epoch
+#pragma unroll
+    for (int j = 0; j < ACC; ++j) dacc[j] = 0.f;
     float out_max = 0.f;                          // max |y| this thread stores in this tile (-> d.amax_out)
 
-    // drains this thread's slice (its row, ACC columns of every issuer's copy) with round-to-nearest adds, re-zeroes it
-    auto drain = [&]() {
 #pragma unroll
-      for (int cc = 0; cc < ACC; cc += 16) {
-        uint32_t v[16];
-        tmem_ld16(my_acc_addr + static_cast<uint32_t>(cc), v);
+    for (int s = 0; s < TC_STAGES - 1; ++s) {
+      if (s < len) load_chunk(cb + s, s);
+      cp_async_commit();                          // empty groups keep the wait counts uniform
+    }
+    for (int i = 0; i < len; ++i) {
+      cp_async_wait<TC_STAGES - 2>();             // this thread's copies of chunk i have landed
+      fence_proxy_async();
+      __syncthreads();                            // everyone's have; both warpgroups are done with chunk i - 1
+      if (i + TC_STAGES - 1 < len) load_chunk(cb + i + TC_STAGES - 1, (i + TC_STAGES - 1) % TC_STAGES);
+      cp_async_commit();
+      const unsigned char* st = base + (i % TC_STAGES) * STAGE;
+      const float* sa = reinterpret_cast<const float*>(st + B_IMG);
+      const uint64_t b0 = wgmma_desc_sw128(smem_u32(st));
+      const uint32_t keep = (i % kFlushChunks) != 0;    // the first MMA of an epoch overwrites the accumulators
+      if (F16) {
+        // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
+        // precision of the tf32 hi / lo pair.  Fragment of k-step ks: rows (r, r + 8) x channels 16 ks + 2 t4 + {0, 1}, + 8
+        uint32_t h1[TC_BK / 16][4], h2[TC_BK / 16][4];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) acc[cc + j] += __uint_as_float(v[j]);
-        tmem_zero16(my_acc_addr + static_cast<uint32_t>(cc));
-      }
-      asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-    };
-
-    // epoch boundary (every role, top of chunk c): the accumulation run that ended with chunk c-1 is drained by all
-    // 16 warps before any MMA of chunk c is issued
-    auto epoch_boundary = [&](int c) {
-      if ((c % kFlushChunks) == 0 && c > 0) {
-        mbar_wait(smem_u32(&bar_epoch), (epochs - 1) & 1, 0x10000u + round0 + c);
-        tc_fence_after();
-        drain();
-        tc_fence_before();
-        __syncthreads();
-        tc_fence_after();
-      }
-    };
-
-    // Implicit im2col through the TMA: every `tile::gather4` load fetches the 128-byte channel slice of FOUR arbitrary
-    // source rows (row indices from the tap table; -1 and channels past C are zero-filled by the TMA) into 512
-    // contiguous, 128B-swizzled bytes of the raw stage and completes on the stage's mbarrier.  A chunk is 64 loads:
-    // gather warp g issues groups g, g+5, ...  One load costs the issuing warp ~140 clk here - that is the TMA unit's
-    // queue, not the warp.  Everything a load needs except the four row indices is made provably warp-uniform
-    // (shuffles), so ptxas keeps it in uniform registers across the unrolled loop; per load that leaves one LDS.128 +
-    // four R2URs.
-    const uint32_t sA_u = __shfl_sync(0xffffffffu, smem_u32(sA_base), 0);
-    const int gw = warp - TC_SPLIT_WARPS;                               // gather warp index (valid for warps 8-12)
-    // ---- one-fill-per-chunk form (SH = false): chunk c -> raw stage round % 3, rows = the tap's table
-    constexpr int kMaxLoadsPerWarp = (TC_BM / 4 + TC_GATHER_WARPS - 1) / TC_GATHER_WARPS;
-    auto gather_chunk = [&](int c, uint32_t round) {
-      const uint32_t st = round % TC_A_STAGES;
-      if (tiled_rows) {
-        // 1x1 stages read tile rows m0 .. m0+255 of x0 as they are: ONE tiled TMA load (box = 256 rows x 32 channels, tm0 is
-        // encoded with that box by the host) instead of 64 four-row gathers - 690 vs 974 clk per chunk measured
-        // (scripts/bench_cu/tma_tile_rate.cu) and no issue pressure.  Rows past the tensor / channels past C read zeros.
-        if (gw == 0 && elect_one()) {
-          const uint32_t bar = smem_u32(&bar_raw_full[st]);
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(static_cast<uint32_t>(TC_A_TILE)) : "memory");
-          asm volatile(
-              "cp.async.bulk.tensor.2d.shared::cta.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(
-                  sA_u + st * TC_A_TILE),
-              "l"(reinterpret_cast<uint64_t>(&tm0)), "r"(c * TC_BK), "r"(m0), "r"(bar)
-              : "memory");
-        }
-        return;
-      }
-      const int rr = c / d.taps;                  // channel chunk outermost, taps innermost: the nine taps of a
-      const int tap = c - rr * d.taps;            // chunk re-read (almost) the same rows while they are hot in L2
-      const bool src1 = rr >= nch0;
-      const int col = __shfl_sync(0xffffffffu, (src1 ? rr - nch0 : rr) * TC_BK, 0);
-      const uint32_t tab_u = __shfl_sync(0xffffffffu, smem_u32((src1 ? tab1 : tab0) + tap * TC_BM + 4 * gw), 0);
-      const uint64_t tmp = reinterpret_cast<uint64_t>(src1 ? &tm1 : &tm0);
-      const uint64_t tm_u = (static_cast<uint64_t>(__shfl_sync(0xffffffffu, static_cast<uint32_t>(tmp >> 32), 0)) << 32) |
-                            __shfl_sync(0xffffffffu, static_cast<uint32_t>(tmp), 0);
-      const uint32_t bar = __shfl_sync(0xffffffffu, smem_u32(&bar_raw_full[st]), 0);
-      const uint32_t dst_u = __shfl_sync(0xffffffffu, sA_u + st * TC_A_TILE + gw * 512, 0);
-      if (gw == 0 && elect_one())
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(static_cast<uint32_t>(TC_A_TILE)) : "memory");
+        for (int ks = 0; ks < TC_BK / 16; ++ks) {
 #pragma unroll
-      for (int i = 0; i < kMaxLoadsPerWarp; ++i) {
-        if (gw + i * TC_GATHER_WARPS < TC_BM / 4) {
-          int4 r4;
-          asm("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];\n"
-              : "=r"(r4.x), "=r"(r4.y), "=r"(r4.z), "=r"(r4.w)
-              : "r"(tab_u + static_cast<uint32_t>(i * TC_GATHER_WARPS * 16)));
-          if (elect_one())
-            asm volatile(
-                "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];\n" ::"r"(
-                    dst_u + static_cast<uint32_t>(i * TC_GATHER_WARPS * 512)),
-                "l"(tm_u), "r"(col), "r"(r4.x), "r"(r4.y), "r"(r4.z), "r"(r4.w), "r"(bar)
-                : "memory");
-        }
-      }
-    };
-    // ---- shared-tap form (SH = true): fill `fr` (tile-relative) = chunks fr*gsz .. of one (channel chunk, dy); slots
-    // 0..255 <- the centre tap's table, slots 256.. <- the (source, dy)'s extras; stage = global fill round % 2
-    constexpr int kMaxFillLoads = (TC_SH_ROWS / 4 + TC_GATHER_WARPS - 1) / TC_GATHER_WARPS;
-    auto issue_fill = [&](int fr, uint32_t fround) {
-      const uint32_t st = fround % TC_SH_STAGES;
-      const int c = fr * gsz;
-      const int rr = c / 9;
-      const int tap = c - rr * 9;                 // gsz == 3: the (dy, dx = -1) tap, centre = tap + 1; gsz == 1: the tap itself
-      const bool src1 = rr >= nch0;
-      const int sd = (src1 ? 3 : 0) + tap / 3;
-      const int col = __shfl_sync(0xffffffffu, (src1 ? rr - nch0 : rr) * TC_BK, 0);
-      const int ctap = gsz == 3 ? tap + 1 : tap;
-      const int ne = gsz == 3 ? min(nx[sd], TC_SH_EXTRA) : 0;
-      const int ngroups = __shfl_sync(0xffffffffu, TC_BM / 4 + ((ne + 3) >> 2), 0);
-      const uint32_t tab_u = __shfl_sync(0xffffffffu, smem_u32((src1 ? tab1 : tab0) + ctap * TC_BM), 0);
-      const uint32_t xtr_u = __shfl_sync(0xffffffffu, smem_u32(xtra + sd * TC_SH_EXTRA) - static_cast<uint32_t>(TC_BM * 4), 0);
-      const uint64_t tmp = reinterpret_cast<uint64_t>(src1 ? &tm1 : &tm0);
-      const uint64_t tm_u = (static_cast<uint64_t>(__shfl_sync(0xffffffffu, static_cast<uint32_t>(tmp >> 32), 0)) << 32) |
-                            __shfl_sync(0xffffffffu, static_cast<uint32_t>(tmp), 0);
-      const uint32_t bar = __shfl_sync(0xffffffffu, smem_u32(&bar_raw_full[st]), 0);
-      const uint32_t dst_u = __shfl_sync(0xffffffffu, sA_u + st * TC_SH_TILE, 0);
-      if (gw == 0 && elect_one())
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(static_cast<uint32_t>(ngroups * 512)) : "memory");
-#pragma unroll
-      for (int i = 0; i < kMaxFillLoads; ++i) {
-        const int g = gw + i * TC_GATHER_WARPS;   // warp-uniform
-        if (g < ngroups) {
-          int4 r4;
-          asm("ld.shared.v4.s32 {%0, %1, %2, %3}, [%4];\n"
-              : "=r"(r4.x), "=r"(r4.y), "=r"(r4.z), "=r"(r4.w)
-              : "r"((g < TC_BM / 4 ? tab_u : xtr_u) + static_cast<uint32_t>(g * 16)));
-          if (elect_one())
-            asm volatile(
-                "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];\n" ::"r"(
-                    dst_u + static_cast<uint32_t>(g * 512)),
-                "l"(tm_u), "r"(col), "r"(r4.x), "r"(r4.y), "r"(r4.z), "r"(r4.w), "r"(bar)
-                : "memory");
-        }
-      }
-    };
-
-    if (warp < TC_SPLIT_WARPS) {
-      // =================================================================================== split warps
-      // raw fp32 row (128 B of the smem stage) -> hi / lo in tensor memory.  Thread = tile row `my_row` = TMEM lane.
-      // running position of chunk cb + c: tap, source, place in its fill group, fill round (no divisions in the loop)
-      int tapi = cb % 9, rri = cb / 9;
-      int gpos = cb % gsz;
-      uint32_t fround = fround0;
-      uint32_t pre_raw = 0, pre_mma = 0;              // early looks at THIS chunk's barriers, taken during the previous chunk
-      for (int c = 0; c < len; ++c) {
-        const uint32_t round = round0 + c;
-        const uint32_t ts = round % TC_T_STAGES;
-        epoch_boundary(c);
-        if (warp == 0) TC_TRACE(0, 0, c);
-        const unsigned char* rowp;
-        uint32_t swz;                                   // row's swizzle key (slot & 7)
-        uint32_t release_bar = 0;                       // raw stage to hand back after this chunk (0 = keep)
-        bool zero_row = false;
-        if (SH) {
-          const uint32_t st = fround % TC_SH_STAGES;
-          if ((c == 0 || gpos == 0) && !__all_sync(0xffffffffu, pre_raw != 0u)) mbar_wait(smem_u32(&bar_raw_full[st]), (fround / TC_SH_STAGES) & 1, 0x20000u + round);
-          int slot = my_row;
-          if (gsz == 3 && gpos != 1) slot = slots[(((rri >= nch0 ? 3 : 0) + tapi / 3) * 2 + (gpos >> 1)) * TC_BM + my_row];
-          zero_row = slot == kZeroSlot;
-          if (zero_row) slot = my_row;
-          rowp = sA_base + st * TC_SH_TILE + slot * 128;
-          swz = static_cast<uint32_t>(slot & 7);
-          if (gpos == gsz - 1 || c == len - 1) release_bar = smem_u32(&bar_raw_empty[st]);
-          if (++gpos == gsz) { gpos = 0; ++fround; }
-          if (++tapi == 9) { tapi = 0; ++rri; }
-        } else {
-          const uint32_t rs = round % TC_A_STAGES;
-          if (!__all_sync(0xffffffffu, pre_raw != 0u)) mbar_wait(smem_u32(&bar_raw_full[rs]), (round / TC_A_STAGES) & 1, 0x20000u + round);
-          rowp = sA_base + rs * TC_A_TILE + my_row * 128;
-          swz = static_cast<uint32_t>(my_row & 7);
-          release_bar = smem_u32(&bar_raw_empty[rs]);
-        }
-        if (warp == 0) TC_TRACE(0, 1, c);
-        if (c == 0) TC_TILE_TRACE(2);
-        // N <= 64: the row's 128 bytes first (the raw stage is ready), then the wait for the TMEM A stage - the
-        // shared-memory latency overlaps the barrier's.  N = 128 keeps 64 accumulator registers per thread and has no
-        // room for the whole row: it reads 64 bytes at a time after the wait.
-        constexpr bool kEarly = BN <= 64;
-        uint4 rawv[kEarly ? 8 : 1];
-        if (kEarly) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            rawv[kEarly ? q : 0] = *reinterpret_cast<const uint4*>(rowp + ((static_cast<uint32_t>(q) ^ swz) << 4));   // swizzle: conflict-free
-            if (SH && zero_row) rawv[kEarly ? q : 0] = make_uint4(0u, 0u, 0u, 0u);
+          for (int e = 0; e < 4; ++e) {
+            const float2 v = *reinterpret_cast<const float2*>(sa + (row_a + (e & 1) * 8) * TC_A_LD + ks * 16 + 2 * t4 + (e >> 1) * 8);
+            const float b0f = v.x * ascale, b1f = v.y * ascale;
+            const uint32_t p = pack_f16x2(b0f, b1f);
+            h1[ks][e] = p;
+            h2[ks][e] = pack_f16x2(b0f - f16_lo_to_f32(p), b1f - f16_hi_to_f32(p));
           }
         }
-        // TMEM A stage free?  It was read by the MMAs of round - T_STAGES.
-        if (round >= TC_T_STAGES && !__all_sync(0xffffffffu, pre_mma != 0u)) mbar_wait(smem_u32(&bar_mma[ts]), ((round - TC_T_STAGES) / TC_T_STAGES) & 1, 0x28000u + round);
-        tc_fence_after();
-        if (kEarly) {
-          // hand the raw stage back only once the row has provably arrived in registers: one dependent use of every
-          // loaded word precedes the arrive (a release does not wait for outstanding shared-memory loads by itself)
-          uint32_t touch = 0;
+        wgmma_fence();
+        // rows of the weight tile: [h1: 64 B | h2: 64 B]; a k-step is 16 channels = 32 B
 #pragma unroll
-          for (int q = 0; q < 8; ++q) touch |= rawv[kEarly ? q : 0].x ^ rawv[kEarly ? q : 0].y ^ rawv[kEarly ? q : 0].z ^ rawv[kEarly ? q : 0].w;
-          asm volatile("" ::"r"(touch) : "memory");
-          __syncwarp();
-          if (lane == 0 && release_bar) mbar_arrive(release_bar);       // raw stage may be overwritten
+        for (int ks = 0; ks < TC_BK / 16; ++ks) {
+          const uint64_t bh = b0 + static_cast<uint64_t>(2 * ks);
+          const uint64_t bl = bh + 4u;
+          Wgmma<BN, true>::mma(dacc, h2[ks], bh, ks == 0 ? keep : 1u);   // lo*hi
+          Wgmma<BN, true>::mma(dacc, h1[ks], bl, 1u);                    // hi*lo
+          Wgmma<BN, true>::mma(dacc, h1[ks], bh, 1u);                    // hi*hi
         }
-        if (warp == 0) TC_TRACE(0, 2, c);
-        const uint32_t ta = tmem_acc + lane_field + Cfg::A_COL0 + ts * Cfg::A_STAGE + static_cast<uint32_t>(my_half * (Cfg::A_STAGE / 2));
+        wgmma_commit();
+        wgmma_wait_all();
 #pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {              // 16 channels at a time
-          uint4 v4[4];
+        for (int ks = 0; ks < TC_BK / 16; ++ks)
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            if (kEarly) {
-              v4[q] = rawv[kEarly ? 4 * hf + q : 0];
-            } else if (WMD_TC_EXP == 2 || WMD_TC_EXP == 3) {
-              v4[q] = make_uint4(round, swz, ts, 4u * hf + q);   // ablation: no shared-memory row reads
-            } else {
-              v4[q] = *reinterpret_cast<const uint4*>(rowp + ((static_cast<uint32_t>(4 * hf + q) ^ swz) << 4));
-              if (SH && zero_row) v4[q] = make_uint4(0u, 0u, 0u, 0u);
-            }
-          }
-          if (F16) {
-            // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
-            // precision of the tf32 hi / lo pair; two halves per 32-bit TMEM column, lower channel in the lower half
-            uint32_t h1[8], h2[8];
-#if WMD_TC_EXP >= 1 && WMD_TC_EXP <= 3
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {              // ablation: no conversion arithmetic
-              h1[2 * q] = v4[q].x; h1[2 * q + 1] = v4[q].y; h2[2 * q] = v4[q].z; h2[2 * q + 1] = v4[q].w;
-            }
-#else
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float b0 = __uint_as_float(v4[q].x) * ascale, b1 = __uint_as_float(v4[q].y) * ascale;
-              const float b2 = __uint_as_float(v4[q].z) * ascale, b3 = __uint_as_float(v4[q].w) * ascale;
-              const uint32_t p0 = pack_f16x2(b0, b1), p1 = pack_f16x2(b2, b3);
-              h1[2 * q] = p0;
-              h1[2 * q + 1] = p1;
-              h2[2 * q] = pack_f16x2(b0 - f16_lo_to_f32(p0), b1 - f16_hi_to_f32(p0));
-              h2[2 * q + 1] = pack_f16x2(b2 - f16_lo_to_f32(p1), b3 - f16_hi_to_f32(p1));
-            }
-#endif
-            tmem_st8(ta + static_cast<uint32_t>(8 * hf), h1);
-            tmem_st8(ta + 16u + static_cast<uint32_t>(8 * hf), h2);
-          } else {
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint32_t raw[4] = {v4[q].x, v4[q].y, v4[q].z, v4[q].w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                hi[4 * q + e] = raw[e] & 0xFFFFE000u;                                                    // tf32 by truncation
-                lo[4 * q + e] = __float_as_uint(__uint_as_float(raw[e]) - __uint_as_float(hi[4 * q + e]));   // exact remainder
-              }
-            }
-            tmem_st16(ta + static_cast<uint32_t>(16 * hf), hi);
-            tmem_st16(ta + 32u + static_cast<uint32_t>(16 * hf), lo);
-          }
-        }
-        if (!kEarly) {
-          __syncwarp();
-          if (lane == 0 && release_bar) mbar_arrive(release_bar);       // raw stage may be overwritten
-        }
-        if (warp == 0) TC_TRACE(0, 3, c);
-        // early look at the next chunk's barriers: the queries' latency overlaps the tcgen05.st drain below
-        pre_raw = pre_mma = 0;
-        if (c + 1 < len) {
-          const uint32_t nr = round + 1;
-          if (nr >= TC_T_STAGES) pre_mma = mbar_test(smem_u32(&bar_mma[nr % TC_T_STAGES]), ((nr - TC_T_STAGES) / TC_T_STAGES) & 1);
-          if (SH) {                                   // gpos / fround already describe chunk c + 1
-            if (gpos == 0) pre_raw = mbar_test(smem_u32(&bar_raw_full[fround % TC_SH_STAGES]), (fround / TC_SH_STAGES) & 1);
-          } else {
-            pre_raw = mbar_test(smem_u32(&bar_raw_full[nr % TC_A_STAGES]), (nr / TC_A_STAGES) & 1);
-          }
-        }
-        if (WMD_TC_EXP != 3) asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bar_asplit[ts]));
-        if (warp == 0) TC_TRACE(0, 4, c);
-        if (((c + 1) % kFlushChunks == 0) || (c == len - 1)) epochs += 1;
-      }
-    } else if (warp < TC_SPLIT_WARPS + TC_GATHER_WARPS) {
-      // =================================================================================== gather warps
-      // the raw stages are free at the start of a tile (every split of the previous tile has completed)
-      if (SH) {
-        issue_fill(f0, fround0);
-        if (nfills > 1) issue_fill(f0 + 1, fround0 + 1);
-        int gpos = cb % gsz, j = 0;                      // chunk's place in its fill group, fill index within the segment
-        for (int c = 0; c < len; ++c) {
-          epoch_boundary(c);
-          if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 0, c);
-          // at the first chunk of fill j >= 1 the stage of fill j - 1 is about to be released: refill it with fill j + 1
-          if (gpos == 0 && j >= 1 && j + 1 < nfills) {
-            const uint32_t fr2 = fround0 + static_cast<uint32_t>(j + 1);
-            mbar_wait(smem_u32(&bar_raw_empty[fr2 % TC_SH_STAGES]), ((fr2 / TC_SH_STAGES) - 1) & 1, 0x30000u + fr2);
-            if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 1, c);
-            issue_fill(f0 + j + 1, fr2);
-          }
-          if (++gpos == gsz) { gpos = 0; ++j; }
-          if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 2, c);
-          if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 3, c);
-          if (((c + 1) % kFlushChunks == 0) || (c == len - 1)) epochs += 1;
-        }
+          for (int e = 0; e < 4; ++e) { reg_fence(h1[ks][e]); reg_fence(h2[ks][e]); }
       } else {
-        gather_chunk(cb, round0);
-        if (len > 1) gather_chunk(cb + 1, round0 + 1);
-        for (int c = 0; c < len; ++c) {
-          const uint32_t round = round0 + c;
-          epoch_boundary(c);
-          if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 0, c);
-          if (c + 2 < len) {
-            const uint32_t r2 = round + 2, st2 = r2 % TC_A_STAGES;
-            // stage st2 was last filled for round r2-3: wait until the split warps have read it
-            if (c + 2 >= TC_A_STAGES) mbar_wait(smem_u32(&bar_raw_empty[st2]), ((r2 - TC_A_STAGES) / TC_A_STAGES) & 1, 0x30000u + round);
-            if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 1, c);
-            gather_chunk(cb + c + 2, r2);
-          }
-          if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 2, c);
-          if (warp == TC_SPLIT_WARPS) TC_TRACE(1, 3, c);
-          if (((c + 1) % kFlushChunks == 0) || (c == len - 1)) epochs += 1;
-        }
-      }
-    } else if (warp == TC_WLOAD_WARP) {
-      // =================================================================================== weight loader
-      // One [hi | lo] image per chunk, B_STAGES - 1 chunks ahead of the MMAs, a single cp.async.bulk each.  The stage
-      // of chunk c + B - 1 is the one chunk c - 1 used: it is free when both issuers' MMAs of chunk c - 1 have
-      // completed (bar_bfree, committed by the issuers: its next completion after chunk c - 1 is chunk c - 1 + B, which
-      // needs the very load issued here - no phase can be skipped).  A warp of its own, so that this wait is not in
-      // the issuers' loop.
-      const uint32_t sB_u = __shfl_sync(0xffffffffu, smem_u32(sB_base), 0);
-      if (elect_one()) {
-        const unsigned char* w0 = wtile + static_cast<long long>(cb) * B_IMG;
-        // the first B_STAGES - 1 weight images (their stages are free: every MMA of the previous tile has completed)
-        for (int k = 0; k < TC_B_STAGES - 1 && k < len; ++k)
-          bulk_g2s(sB_u + ((round0 + k) % TC_B_STAGES) * B_IMG, w0 + static_cast<long long>(k) * B_IMG, B_IMG,
-                   smem_u32(&bar_b[(round0 + k) % TC_B_STAGES]));
-      }
-      __syncwarp();
-      for (int c = 0; c < len; ++c) {
-        const uint32_t round = round0 + c;
-        epoch_boundary(c);
-        if (c + TC_B_STAGES - 1 < len) {
-          // c == 0: the stage belonged to the previous tile's last chunk - free since the tile's closing barrier
-          if (c >= 1) mbar_wait(smem_u32(&bar_bfree[(round - 1) % TC_B_STAGES]), ((round - 1) / TC_B_STAGES) & 1, 0x50000u + round);
-          if (elect_one()) {
-            const uint32_t ns = (round + TC_B_STAGES - 1) % TC_B_STAGES;
-            bulk_g2s(sB_u + ns * B_IMG, wtile + static_cast<long long>(cb + c + TC_B_STAGES - 1) * B_IMG, B_IMG,
-                     smem_u32(&bar_b[ns]));
-          }
-          __syncwarp();
-        }
-        if (((c + 1) % kFlushChunks == 0) || (c == len - 1)) epochs += 1;
-      }
-    } else {
-      // =================================================================================== issuers
-      // The whole warp runs the loop and one elected lane issues.  Written this way (warp-uniform control flow,
-      // operands derived from warp-uniform values) ptxas keeps the MMA operands in uniform registers and emits the
-      // UTCHMMAs back to back: ~78 clk per instruction.  A `lane == 0` branch instead makes it wrap every MMA in an
-      // ELECT / R2UR.BROADCAST / BRA.U.ANY loop: ~210 clk (scripts/bench_cu/mma_rate*.cu).
-      const int ih = warp - (TC_WLOAD_WARP + 1);                    // this issuer's M half = its accumulator
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_acc, 0);
-      const uint32_t sB_u = __shfl_sync(0xffffffffu, smem_u32(sB_base), 0);
-      const uint32_t dh = tmem_u + static_cast<uint32_t>(ih * BN);
-      for (int c = 0; c < len; ++c) {
-        const uint32_t round = round0 + c;
-        const uint32_t ts = round % TC_T_STAGES;
-        const uint32_t bs = round % TC_B_STAGES;
-        epoch_boundary(c);
-        if (ih == 0) TC_TRACE(2, 0, c);
-        mbar_wait(smem_u32(&bar_b[bs]), (round / TC_B_STAGES) & 1, 0x48000u + round);        // weight image has landed (long ago)
-        if (ih == 0) TC_TRACE(2, 1, c);
-        mbar_wait(smem_u32(&bar_asplit[ts]), (round / TC_T_STAGES) & 1, 0x40000u + round);   // split A of this chunk is in TMEM
-        if (ih == 0) TC_TRACE(2, 2, c);
-        tc_fence_after();
-        const uint64_t b0 = umma_desc_sw128(sB_u + bs * B_IMG);
-        const uint32_t ah = tmem_u + Cfg::A_COL0 + ts * Cfg::A_STAGE + static_cast<uint32_t>(ih * (Cfg::A_STAGE / 2));
-        if (elect_one()) {
-          if (F16) {
-            // rows of the weight tile: [h1: 64 B | h2: 64 B]; a k-step is 16 channels = 32 B; A: h1 columns 0..15, h2 16..31
+        // fragment of k-step ks: rows (r, r + 8) x channels 8 ks + t4, + 4; tf32 hi by truncation, exact remainder lo
+        uint32_t hi[TC_BK / 8][4], lo[TC_BK / 8][4];
 #pragma unroll
-            for (int ks = 0; ks < TC_BK / 16; ++ks) {
-              const uint64_t bh = b0 + static_cast<uint64_t>(2 * ks);
-              const uint64_t bl = bh + 4u;
-              const uint32_t a = ah + static_cast<uint32_t>(8 * ks);
-              umma_f16_ts(dh, a + 16u, bh, kIdesc, 1u);    // lo*hi
-              umma_f16_ts(dh, a, bl, kIdesc, 1u);          // hi*lo
-              umma_f16_ts(dh, a, bh, kIdesc, 1u);          // hi*hi
-            }
-          } else {
+        for (int ks = 0; ks < TC_BK / 8; ++ks) {
 #pragma unroll
-            for (int ks = 0; ks < TC_BK / 8; ++ks) {
-              const uint64_t bh = b0 + static_cast<uint64_t>(2 * ks);
-              const uint64_t bl = bh + static_cast<uint64_t>(TC_B_TILE >> 4);
-              const uint32_t a = ah + static_cast<uint32_t>(8 * ks);
-              umma_tf32_ts(dh, a + 32u, bh, kIdesc, 1u);     // lo*hi
-              umma_tf32_ts(dh, a, bl, kIdesc, 1u);           // hi*lo
-              umma_tf32_ts(dh, a, bh, kIdesc, 1u);           // hi*hi
-            }
+          for (int e = 0; e < 4; ++e) {
+            const float v = sa[(row_a + (e & 1) * 8) * TC_A_LD + ks * 8 + t4 + (e >> 1) * 4];
+            hi[ks][e] = __float_as_uint(v) & 0xFFFFE000u;
+            lo[ks][e] = __float_as_uint(v - __uint_as_float(hi[ks][e]));
           }
-          umma_commit(smem_u32(&bar_mma[ts]));             // TMEM A stage reusable
-          umma_commit(smem_u32(&bar_bfree[bs]));           // weight stage reusable
-          if (((c + 1) % kFlushChunks == 0) || (c == len - 1)) umma_commit(smem_u32(&bar_epoch));
         }
-        __syncwarp();
-        if (ih == 0) TC_TRACE(2, 3, c);
-        if (((c + 1) % kFlushChunks == 0) || (c == len - 1)) epochs += 1;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < TC_BK / 8; ++ks) {
+          const uint64_t bh = b0 + static_cast<uint64_t>(2 * ks);
+          const uint64_t bl = bh + static_cast<uint64_t>(TC_B_TILE >> 4);
+          Wgmma<BN, false>::mma(dacc, lo[ks], bh, ks == 0 ? keep : 1u);  // lo*hi
+          Wgmma<BN, false>::mma(dacc, hi[ks], bl, 1u);                   // hi*lo
+          Wgmma<BN, false>::mma(dacc, hi[ks], bh, 1u);                   // hi*hi
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+#pragma unroll
+        for (int ks = 0; ks < TC_BK / 8; ++ks)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) { reg_fence(hi[ks][e]); reg_fence(lo[ks][e]); }
+      }
+#pragma unroll
+      for (int j = 0; j < ACC; ++j) reg_fence(dacc[j]);
+      if (((i + 1) % kFlushChunks == 0) || (i == len - 1)) {
+#pragma unroll
+        for (int j = 0; j < ACC; ++j) acc[j] += dacc[j];
       }
     }
-    mma_rounds = round0 + static_cast<uint32_t>(len);
-    fill_rounds = fround0 + static_cast<uint32_t>(nfills);
-    TC_TILE_TRACE(3);
+    cp_async_wait<0>();
 
-    // ---- last epoch + epilogue (all 16 warps): bias, activation, one contiguous 256-byte store per thread
-    {
-      mbar_wait(smem_u32(&bar_epoch), (epochs - 1) & 1, 0x60000u + mma_rounds);
-      tc_fence_after();
-      TC_TILE_TRACE(4);
-      drain();
-      TC_TILE_TRACE(5);
+    // ---- epilogue: bias, activation, pair stores.  acc[4 j + 2 h + e] = row row_a + 8 h, column 8 j + 2 t4 + e
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int my_row = row_a + 8 * h;
       const int m = m0 + my_row;
       if (m < rows && !whole) {
         // raw partial sums of this segment (bias / activation are applied by the reduce pass)
-        if (balanced) {                                // compact workspace: [remainder tile][slab][256 rows][BN]
-          float* pr = partial + kBalCounterBytes / 4 + ((rem_t * plan.slabs + slab) * TC_BM + my_row) * BN + my_ch * ACC;
+        if (balanced) {                                // compact workspace: [remainder tile][slab][TC_BM rows][BN]
+          float* pr = partial + kBalCounterBytes / 4 + ((rem_t * plan.slabs + slab) * TC_BM + my_row) * BN + 2 * t4;
 #pragma unroll
-          for (int j = 0; j < ACC; j += 4) __stcg(reinterpret_cast<float4*>(pr + j), make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]));
+          for (int j = 0; j < BN / 8; ++j) __stcg(reinterpret_cast<float2*>(pr + 8 * j), make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
         } else {                                       // split-K: [slab][max_rows][ldy]
           float* pr = partial + kBalCounterBytes / 4 + (static_cast<long long>(slab) * d.max_rows + m) * d.ldy;
 #pragma unroll
-          for (int j = 0; j < ACC; j += 4) {
-            const int co = n0 + my_ch * ACC + j;     // ldy % 4 == 0: a quad that starts below cout stays inside the row
-            if (co < d.cout) *reinterpret_cast<float4*>(pr + co) = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
+          for (int j = 0; j < BN / 8; ++j) {
+            const int co = n0 + 8 * j + 2 * t4;      // ldy % 4 == 0: a pair that starts below cout stays inside the row
+            if (co < d.cout) *reinterpret_cast<float2*>(pr + co) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
           }
         }
       } else if (m < rows) {
         float* yr = d.y + static_cast<long long>(m) * d.ldy;
-        // The epilogue is instruction bound (64 outputs per thread at N = 128): the activation is picked once per tile, not
-        // per element (act is a kernel argument), quads that lie inside cout take vector bias loads and no per-element
-        // bounds; only a quad that straddles cout goes element by element.
+        // The activation is picked once per tile, not per element (act is a kernel argument); pairs that lie inside cout
+        // take vector bias loads and no per-element bounds.
         const float ap = d.act_param;
         auto store_all = [&](auto actf) {
 #pragma unroll
-          for (int j = 0; j < ACC; j += 4) {
-            const int co = n0 + my_ch * ACC + j;
-            if (al_ok && co + 3 < d.cout) {
-              const float4 bq = d.bias ? __ldg(reinterpret_cast<const float4*>(d.bias + co)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              float4 o;
+          for (int j = 0; j < BN / 8; ++j) {
+            const int co = n0 + 8 * j + 2 * t4;
+            const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+            if (al_ok && co + 1 < d.cout) {
+              const float2 bq = d.bias ? __ldg(reinterpret_cast<const float2*>(d.bias + co)) : make_float2(0.f, 0.f);
+              float2 o;
               if (F16) {                               // out_scale is a power of two: the product is exact
-                o.x = fmaf(acc[j], out_scale, bq.x); o.y = fmaf(acc[j + 1], out_scale, bq.y);
-                o.z = fmaf(acc[j + 2], out_scale, bq.z); o.w = fmaf(acc[j + 3], out_scale, bq.w);
+                o.x = fmaf(a0, out_scale, bq.x); o.y = fmaf(a1, out_scale, bq.y);
               } else {
-                o.x = acc[j] + bq.x; o.y = acc[j + 1] + bq.y; o.z = acc[j + 2] + bq.z; o.w = acc[j + 3] + bq.w;
+                o.x = a0 + bq.x; o.y = a1 + bq.y;
               }
-              o.x = actf(o.x); o.y = actf(o.y); o.z = actf(o.z); o.w = actf(o.w);
-              out_max = fmaxf(fmaxf(out_max, fabsf(o.x)), fmaxf(fabsf(o.y), fmaxf(fabsf(o.z), fabsf(o.w))));
-#if WMD_TC_EXP == 5                               // ablation: same stores, but into a 2 MB window that stays in L2
-              *reinterpret_cast<float4*>(d.y + ((static_cast<long long>(m) * d.ldy + co) & 0x7FFFCll)) = o;
-#elif WMD_TC_EXP == 6                             // ablation: no store at all (the arithmetic survives through out_max)
-              if (o.x == 123456.f) *reinterpret_cast<float4*>(yr + co) = o;
-#else
-              *reinterpret_cast<float4*>(yr + co) = o;
-#endif
-            } else if (co < d.cout) {
+              o.x = actf(o.x); o.y = actf(o.y);
+              out_max = fmaxf(out_max, fmaxf(fabsf(o.x), fabsf(o.y)));
+              *reinterpret_cast<float2*>(yr + co) = o;
+            } else {
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
+              for (int e = 0; e < 2; ++e) {
                 if (co + e < d.cout) {
-                  const float a = F16 ? __fmul_rn(acc[j + e], out_scale) : acc[j + e];
+                  const float a = F16 ? __fmul_rn(e ? a1 : a0, out_scale) : (e ? a1 : a0);
                   const float o = actf(a + (d.bias ? __ldg(d.bias + co + e) : 0.f));
                   out_max = fmaxf(out_max, fabsf(o));
                   yr[co + e] = o;
@@ -1158,18 +682,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       for (int o = 16; o > 0; o >>= 1) out_max = fmaxf(out_max, __shfl_xor_sync(0xffffffffu, out_max, o));
       if (lane == 0 && out_max > __ldcg(d.amax_out)) atomicMax(reinterpret_cast<unsigned*>(d.amax_out), __float_as_uint(out_max));   // most warps skip the atomic
     }
-    TC_TILE_TRACE(6);
-    tc_fence_before();
-    __syncthreads();   // accumulators drained + re-zeroed by every warp, tap tables free
-    tc_fence_after();
-    TC_TILE_TRACE(7);
-  }
-
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_acc),
-                 "r"(static_cast<uint32_t>(TC_TMEM_COLS))
-                 : "memory");
+    __syncthreads();   // tap tables and stages free for the next tile
   }
 }
 
@@ -1340,54 +853,17 @@ __global__ void finish_header_tc16_kernel(unsigned char* out) {
 
 static int tc_tile_n(int cout) { return cout >= 96 ? 128 : (cout >= 48 ? 64 : 32); }
 
-// TMA descriptor of a source: 2-D fp32 tensor [rows][C] with row pitch ld floats, box = one row x 32 channels,
-// 128-byte swizzle, zero fill outside (inactive taps are row -1; a channel tail reads zeros)
-typedef CUresult (*TmEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static int make_rows_map(CUtensorMap* tm, const float* x, int C, long long rows, int ld, int box_rows = 1) {
-  static TmEncodeFn encode = nullptr;
-  if (!encode) {
-    cudaDriverEntryPointQueryResult q;
-    void* fn = nullptr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn) return WMD_ERR_UNSUPPORTED;
-    encode = reinterpret_cast<TmEncodeFn>(fn);
-  }
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(rows < 1 ? 1 : rows)};
-  const cuuint64_t gstr[1] = {static_cast<cuuint64_t>(ld) * 4};
-  const cuuint32_t box[2] = {TC_BK, static_cast<cuuint32_t>(box_rows)}, estr[2] = {1, 1};
-  const CUresult rc = encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(x), gdim, gstr, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return rc == CUDA_SUCCESS ? WMD_OK : WMD_ERR_UNSUPPORTED;
-}
-
 static int g_reserved_sms = 0;     // SMs the persistent grid leaves free (for a collective's kernel on multi-GPU runs)
-static int g_shared_taps = 1;      // 3x3 layers: one raw-stage fill per (chunk, dy) shared by the three dx taps (tuning / A-B knob)
+static int g_shared_taps = 1;      // kept for the C ABI: every tap gathers its own rows in this engine
 
-template <int BN, bool SH, bool F16>
+template <int BN, bool F16>
 static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStream_t stream) {
-  using Cfg = TcCfg<BN, SH, F16>;
-  CUtensorMap tm0, tm1;
-  {
-    const long long px = static_cast<long long>(d.N) * d.H * d.W;
-    const long long rows0 = static_cast<long long>(d.N) * (d.H >> d.shift0) * (d.W >> d.shift0);
-    // 1x1 stage over its own rows (taps == 1, no index map): the kernel loads whole 256-row tiles
-    const bool tiled = (d.taps == 1 && d.map0 == nullptr && d.rows0 > 0);
-    int rc = make_rows_map(&tm0, d.x0, d.c0, tiled ? d.rows0 : rows0, d.ld0, tiled ? TC_BM : 1);
-    if (rc != WMD_OK) return rc;
-    if (d.c1 > 0) {
-      rc = make_rows_map(&tm1, d.x1, d.c1, px, d.ld1);
-      if (rc != WMD_OK) return rc;
-    } else {
-      tm1 = tm0;
-    }
-  }
+  using Cfg = TcCfg<BN, F16>;
   static bool attr_done[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_done[dev]) {   // outside the cache: set it on every launch
-    int rc = record(cudaFuncSetAttribute(conv_rows_tc_kernel<BN, SH, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    int rc = record(cudaFuncSetAttribute(conv_rows_tc_kernel<BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          static_cast<int>(Cfg::SMEM)));
     if (rc != WMD_OK) return rc;
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
@@ -1395,7 +871,7 @@ static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStr
   const long long tiles = static_cast<long long>(ceil_div(d.max_rows, TC_BM)) * ceil_div(d.cout, BN) * (splits > 0 ? splits : 1);
   const long long cap = sm_count() - g_reserved_sms > 1 ? sm_count() - g_reserved_sms : 1;
   const int grid = splits == 0 ? static_cast<int>(cap) : static_cast<int>(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap);
-  conv_rows_tc_kernel<BN, SH, F16><<<grid, TC_THREADS, Cfg::SMEM, stream>>>(d, d.w, splits, partial, tm0, tm1);
+  conv_rows_tc_kernel<BN, F16><<<grid, TC_THREADS, Cfg::SMEM, stream>>>(d, d.w, splits, partial);
   int rc = launched();
   if (rc != WMD_OK || splits <= 1) return rc;      // whole tiles, or balanced: the kernel's own fix-up finishes cut tiles
   const int nchunks = d.taps * ((d.c0 + TC_BK - 1) / TC_BK + (d.c1 + TC_BK - 1) / TC_BK);
@@ -1407,15 +883,6 @@ static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStr
 }
 
 }  // namespace wmd
-
-#ifdef WMD_TC_TRACE
-extern "C" int wmd_debug_tc_trace(long long* host_out) {
-  return cudaMemcpyFromSymbol(host_out, wmd::g_trace, sizeof(wmd::g_trace)) == cudaSuccess ? 0 : 1;
-}
-extern "C" int wmd_debug_tc_tile_trace(long long* host_out) {
-  return cudaMemcpyFromSymbol(host_out, wmd::g_tile_trace, sizeof(wmd::g_tile_trace)) == cudaSuccess ? 0 : 1;
-}
-#endif
 
 extern "C" int wmd_conv_tc_tile_n(int cout) { return wmd::tc_tile_n(cout); }
 
@@ -1539,14 +1006,12 @@ extern "C" int wmd_conv_rows_tc_splitk_f32(const wmd_conv_desc* dp, int splits, 
     if (splits == 0 && nchunks < 2) splits = 1;   // nothing to balance inside a one-chunk reduction
   }
   float* partial = static_cast<float*>(ws);
-  const bool sh = d.taps == 9 && g_shared_taps != 0;
   const bool f16 = d.precision == WMD_PREC_F16X3;
   if (f16) WMD_REQUIRE(d.amax0 != nullptr && (d.c1 == 0 || d.amax1 != nullptr), WMD_ERR_ARG);
   if (f16) WMD_REQUIRE(splits <= 1, WMD_ERR_UNSUPPORTED);   // tc_reduce_kernel sums unscaled slabs: tf32 operands only
   cudaStream_t st = as_stream(stream);
-#define WMD_TC_LAUNCH(BN_)                                                                                              \
-  return f16 ? (sh ? launch_tc<BN_, true, true>(d, splits, partial, st) : launch_tc<BN_, false, true>(d, splits, partial, st)) \
-             : (sh ? launch_tc<BN_, true, false>(d, splits, partial, st) : launch_tc<BN_, false, false>(d, splits, partial, st))
+#define WMD_TC_LAUNCH(BN_) \
+  return f16 ? launch_tc<BN_, true>(d, splits, partial, st) : launch_tc<BN_, false>(d, splits, partial, st)
   switch (tc_tile_n(d.cout)) {
     case 128: WMD_TC_LAUNCH(128);
     case 64: WMD_TC_LAUNCH(64);

@@ -5,17 +5,16 @@
 //   Wz  (54, N1)        the heads' 3x3 stages factored into per-row tap products (ops.head_tap_weight): 9 taps x 6 groups
 //   z   rows (M, 56)    consumed by head_gather_kernel (9 x 6-float gather-sum, sigma difference, scatter)
 //
-// Run as two gather-GEMM launches these stages are per-tile-overhead bound on the tcgen05 engine (4-8 chunk reductions:
-// tile prologue + epilogue cost more than the MMAs, scripts/tc_tile_trace.py) and the intermediate t (M x N1) makes a
+// Run as two gather-GEMM launches these stages are per-tile-overhead bound on the tensor-core engine (4-8 chunk
+// reductions: tile prologue + epilogue cost more than the MMAs) and the intermediate t (M x N1) makes a
 // round trip through HBM.  Fused, a row costs C floats read + 56 written (SURVEY 8d puts the low-channel heads on the HBM
 // roof); both weight matrices stay in shared memory for the life of the persistent CTA and t never leaves registers:
 // the accumulator fragment of GEMM1's n8-tile j IS the A fragment of GEMM2's k-slab j (the k index of an MMA is a dummy,
 // so it is permuted to match: logical k = t <- column 2t, k = t+4 <- column 2t+1 of the C fragment).
 //
 // Math: warp-level mma.sync m16n8k8 tf32, fp32-faithful 3xTF32 (lo*hi + hi*lo + hi*hi, x split by truncation with an
-// exact remainder, weights pre-split with round-to-nearest by the pack kernel).  The chained operands of a 128-row tile
-// do not fit tensor memory next to two accumulators (A1 2C + D1 N1 + A2 2*N1 + D2 64 columns), which is why this stage
-// is not on tcgen05; it is a bandwidth-side fusion, the tensor work per byte is small (K <= 128).
+// exact remainder, weights pre-split with round-to-nearest by the pack kernel).  It is a bandwidth-side fusion: the
+// tensor work per byte is small (K <= 128).
 #include "common.cuh"
 
 namespace wmd {

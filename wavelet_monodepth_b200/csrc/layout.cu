@@ -12,8 +12,7 @@ constexpr int kTT = 32;
 // line per pixel).  The 129-float row pitch makes the transposed shared-memory reads conflict-free.
 // Tile of the two streaming moves (nchw_to_rows, gather_rows_list): LC channels x LP pixels, template parameters.  The read
 // side is contiguous along pixels (LP * 4 bytes per channel row), the write side along channels (LC * 4 bytes per pixel
-// row).  Measured on B200 (scripts/layout_bench.py, bench shapes): the dense transpose is fastest at 32 x 128 (4.0 / 5.9
-// TB/s on f4 / skip4), the list gather at 128 x 32 (2.0 -> 2.5 TB/s at level 2, 1.6 -> 1.8 at level 1).
+// row).  The dense transpose uses 32 x 128, the list gather 128 x 32 (A/B of tile shapes: scripts/layout_bench.py).
 template <int LC, int LP>
 struct LayoutTile {
   static constexpr int kLQ = LC / 4;             // float4 lanes that cover one pixel row of the tile

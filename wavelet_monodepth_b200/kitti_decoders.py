@@ -9,7 +9,7 @@ Contract kept (SURVEY 8b): ``.convs`` OrderedDict keyed by tuples, ``.decoder = 
 (state-dict names ``decoder.0 .. decoder.16``), ``inverse_wt`` sub-module with the IDWT tap buffers,
 ``forward(input_features[, thresh_ratio[, sparse_scales]]) -> dict`` with the reference's keys, ``self.outputs``.
 
-What is different underneath (B200-first, DESIGN.md):
+What is different underneath (H100-native, DESIGN.md):
   * inference runs natively end to end in a pixel-major row layout: encoder maps are transposed once
     (or used zero-copy when channels_last), every conv is the gather-GEMM kernel, heads + IDWT + disp are
     fused kernels, and no intermediate dense tensor or index tensor of the reference is materialised;
@@ -178,9 +178,9 @@ class _WaveDecoderBase(nn.Module):
         # (list-based gather-transpose: bytes scale with the mask density, 16-50 % on the bench) and upconv(i,1) reaches them
         # through S3's index map (wmd_conv_desc.map1).  The skip map may then be a pinned HOST tensor.  WMD_COMPACT_SKIP=0/1
         self.compact_skip = os.environ.get("WMD_COMPACT_SKIP", "1") == "1"
-        # ... at the levels where it pays on a device-resident map: measured (scripts/probe_gather.py, B200) the list-based
-        # gather moves ~2 TB/s of useful bytes against 6.5 TB/s for the whole-map transpose, so it wins below ~30 % mask
-        # density - levels 2 and 1 (16-28 % on the bench), not level 3 (50 %).  A pinned-host skip map always takes it.
+        # ... at the levels where it pays on a device-resident map: the list-based gather moves fewer useful bytes per second
+        # than the whole-map transpose (scripts/probe_gather.py), so it wins only at low mask density - levels 2 and 1
+        # (16-28 % on the bench), not level 3 (50 %).  A pinned-host skip map always takes it.
         self.compact_skip_levels = tuple(int(v) for v in os.environ.get("WMD_COMPACT_SKIP_LEVELS", "1,2").split(",") if v)
         # tail of every level as one kernel: head gather-sum -> yh -> IDWT -> disp -> next level's threshold
         # (wmd_head_idwt_f32; WMD_FUSED_TAIL=0/1).  Bit-identical to the head_gather + idwt_haar + range_thresh chain.

@@ -501,16 +501,14 @@ def scatter_rows(rows, c, pixels, count, n, h, w, max_rows=None, out=None):
 
 
 def tc_splits(max_rows, cout, nchunks, device, ldy=None):
-    """Scheduling mode of the tcgen05 engine for one launch: 1 = whole tiles, 0 = balanced (data-parallel + stream-K).
+    """Scheduling mode of the tensor-core (wgmma) engine for one launch: 1 = whole tiles, 0 = balanced (data-parallel + stream-K).
 
-    One CTA per SM runs equal (256-row x N-channel) tiles, so with few tiles per SM the last round is mostly idle
-    (320 tiles on 148 SMs = 72 %; the sparse levels' tile count is only known on the device) and a layer with fewer
+    At most one CTA per SM runs equal (128-row x N-channel) tiles, so with few tiles per SM the last round is mostly idle
+    (320 tiles on 132 SMs = 81 %; the sparse levels' tile count is only known on the device) and a layer with fewer
     tiles than SMs leaves SMs dark.  Balanced mode runs the full rounds as whole tiles and deals the (tile, chunk)
     units of the remainder tiles out evenly on the device; only those tiles go through the fixed-order reduce pass
-    (workspace: CTAs x 8 x 256 x 128 floats).  The extra pass only pays for long reductions - measured on B200
-    (scripts/conv_layers_bench.py, R50 1024x320): bs32 upconv(4,0) 0.67 -> 0.45 ms, upconv(4,1) 1.27 -> 1.02,
-    upconv(3,1) 0.69 -> 0.60, upconv(2,1) 0.61 -> 0.57; reductions of <= 72 chunks (and the 1x1 head stages) lose
-    10-20 % at every batch size."""
+    (workspace: CTAs x 8 x 128 x 128 floats).  The extra pass only pays for long reductions, so it is used from
+    TC_BALANCE_MIN_CHUNKS chunks on (per-layer times: scripts/conv_layers_env.py)."""
     return 0 if nchunks >= TC_BALANCE_MIN_CHUNKS else 1
 
 
@@ -518,7 +516,7 @@ TC_BALANCE_MIN_CHUNKS = int(__import__("os").environ.get("WMD_TC_BALANCE_MIN_CHU
 
 
 class PackedW:
-    """A conv weight packed for one of the two gather-GEMM engines ('simt' fp32 FMA, 'tc' tcgen05 3xTF32)."""
+    """A conv weight packed for one of the two gather-GEMM engines ('simt' fp32 FMA, 'tc' wgmma 3xTF32)."""
     __slots__ = ("data", "kind", "taps", "c0", "c1", "cout", "data16")
 
     def __init__(self, data, kind, taps, c0, c1, cout, data16=None):
@@ -527,17 +525,16 @@ class PackedW:
 
 
 TC_MIN_K = 128        # shallower reductions (1x1 heads of the fine levels) do not amortise the tile prologue
-TC_MIN_COUT = 32      # tcgen05 tiles are 256 x {128, 64, 32}; below that the FMA tiles / head kernel take over
+TC_MIN_COUT = 32      # tensor-core tiles are 128 x {128, 64, 32}; below that the FMA tiles / head kernel take over
 
 
 def default_conv_precision():
-    """Operand form of the tcgen05 engine: env WMD_CONV_PRECISION = tf32x3 (default) | f16x3.
+    """Operand form of the tensor-core engine: env WMD_CONV_PRECISION = tf32x3 (default) | f16x3.
 
     Both are fp32-faithful error-compensated splits with fp32 accumulation (22 mantissa bits per operand, three MMAs per
     product).  f16x3 feeds fp16 pairs of power-of-two scaled operands - half the MMA instructions - and needs the max |x|
     of each source (tracked on the device by the producers, see conv_rows amax*); launches that lack it use tf32x3.
-    Opt-in: on B200 the conversion work of the split warps, not the tensor pipe, bounds the kernel in that form, so it is
-    only ~4 % faster per layer while the max tracking costs more than that elsewhere (DESIGN.md 4)."""
+    Opt-in: it costs the max tracking in every producer; its speed on H100 has not been measured."""
     import os
     return os.environ.get("WMD_CONV_PRECISION", "tf32x3")
 
@@ -545,7 +542,7 @@ def default_conv_precision():
 def default_conv_kind():
     """Engine used when a caller does not ask for one: env WMD_CONV_IMPL = auto | simt | tc.
 
-    auto (default): tcgen05 3xTF32 for cout >= 32 (every upconv / 1x1 head stage of the decoders), fp32 FMA
+    auto (default): wgmma 3xTF32 for cout >= 32 (every upconv / 1x1 head stage of the decoders), fp32 FMA
     tiles below."""
     import os
     return os.environ.get("WMD_CONV_IMPL", "auto")

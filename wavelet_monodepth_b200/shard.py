@@ -134,7 +134,7 @@ class PeerGather(OverlappedGather):
     after it; OverlappedGather has the same rule with one step less slack).
 
     Falls back to the NCCL form (the parent class) when peer access, IPC or the start-up self-check fails.  Opt-in
-    (make_gather): on the B200 pool the DMA engines move only 25 GB/s into IPC-mapped peer memory."""
+    (make_gather): whether copy engines beat NCCL's SM kernels here depends on the platform's peer-copy rate."""
 
     SLOTS = 3
 
@@ -232,10 +232,9 @@ class PeerGather(OverlappedGather):
 def make_gather(n_global, group=None):
     """The overlapped all-gather of this build: NCCL (OverlappedGather); env WMD_PEER_GATHER=1 selects the copy-engine form.
 
-    PeerGather is correct on the B200 pool (scripts/peer_gather_check.py: even and ragged shards, 12 overlapped steps) but
-    a loss there: cudaMemcpyPeerAsync / tensor.copy_ into IPC-mapped peer memory moves 25 GB/s (scripts/peer_copy_probe.py,
-    NV18 topology) where NCCL's SM kernels reach 380 GB/s - 2.3 ms against 0.22 ms per 2 x 42 MB gather.  It stays opt-in
-    for platforms whose DMA engines run at NVLink speed."""
+    PeerGather is checked by scripts/peer_gather_check.py (even and ragged shards, 12 overlapped steps) and its copy rate
+    by scripts/peer_copy_probe.py; neither has been measured on H100.  It stays opt-in for platforms whose DMA engines
+    run at NVLink speed."""
     import os
     if os.environ.get("WMD_PEER_GATHER", "0") == "1" and dist.is_initialized() and dist.get_backend(group) == "nccl":
         return PeerGather(n_global, group)
