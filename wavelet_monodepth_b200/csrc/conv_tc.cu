@@ -2,24 +2,32 @@
 //
 // Same contract as conv_rows_kernel (conv.cu), different engine.  A persistent grid (at most one CTA per SM) walks
 // 128 x N output tiles (N = 128 / 64 / 32); a tile's reduction K = (c0 + c1) x taps runs in 32-channel chunks, the
-// taps of a channel chunk innermost (their source rows overlap: L2 hits).  256 threads = two warpgroups, warpgroup h
-// owns tile rows h*64 .. h*64+63 (one wgmma M = 64 each, both share the chunk's weight tile).
+// taps of a channel chunk innermost (their source rows overlap: L2 hits).  384 threads, warp-specialised: one producer
+// warpgroup fills a TC_STAGES-deep ring of shared-memory stages, two consumer warpgroups multiply; consumer warpgroup h
+// owns tile rows h*64 .. h*64+63 (one wgmma M = 64 each, both share the chunk's weight tile).  Producer and consumers
+// step through the same work walk (TcWalk) and hand stages over with mbarriers (full[s]: stage filled, empty[s]: both
+// consumers are done with it), so the ring runs on across tile boundaries: the producer builds the next tile's tap table
+// and fills its first chunks while the consumers finish the current tile and run its epilogue.
 //
-//   gather (all 256 threads), TC_STAGES - 1 chunks ahead of the MMAs, cp.async with zero fill
-//     * implicit im2col: the 128-byte channel slice of each tile row's source row (row from the per-tile tap table,
-//       -1 = inactive / padded tap, and the channel tail read zeros) into a raw fp32 stage padded to 144-byte rows, so
-//       that the fragment reads below are free of bank conflicts;
+//   produce (warpgroup 0, setmaxnreg down to 40 registers)
 //     * B (weights) is pre-split, pre-swizzled by wmd_pack_conv_weight_tc_f32 into one [hi | lo] image per (n-tile,
-//       chunk): K-major, 128-byte swizzled, read by the wgmma straight from shared memory through a descriptor;
-//   multiply (per warpgroup)
+//       chunk): K-major, 128-byte swizzled, contiguous - one bulk copy (cp.async.bulk, completion counted in bytes on
+//       full[s]); the wgmma reads it straight from shared memory through a descriptor;
+//     * implicit im2col: the 128-byte channel slice of each tile row's source row (row from the per-tile tap table,
+//       -1 = inactive / padded tap, and the channel tail read zeros) by cp.async with zero fill into a raw fp32 stage
+//       padded to 144-byte rows, so that the fragment reads below are free of bank conflicts; each producer thread's
+//       copies arrive on full[s] when they land (cp.async.mbarrier.arrive.noinc);
+//   multiply (per consumer warpgroup, setmaxnreg up to 232 registers)
 //     * every thread reads its A fragment elements (rows g, g + 8 of its warp's 16, channels t, t + 4 of each k-step)
 //       and splits x = hi + lo (hi = x with the 13 low mantissa bits cleared, lo = x - hi: exact) in registers - the
 //       register-A form of wgmma, so the split never goes back to shared memory;
-//     * 4 k-steps x 3 terms (lo*hi + hi*lo + hi*hi) per chunk, committed and waited as one group;
+//     * 4 k-steps x 3 terms (lo*hi + hi*lo + hi*hi) per chunk, committed as one group; the fragments of chunk i + 1 are
+//       read and split into the other of two register sets while chunk i's group runs (wgmma.wait_group 1);
 //     * the tensor core's fp32 accumulation is not round-to-nearest, a bias that grows with K.  So accumulation runs in
 //       EPOCHS of kFlushChunks chunks: the first MMA of an epoch overwrites the wgmma accumulators, the epoch's end adds
 //       them into per-thread fp32 registers with round-to-nearest adds;
-//   epilogue: bias + activation (picked once per tile) + pair stores;
+//   epilogue (consumers only, named barriers over their 256 threads): bias + activation (picked once per tile) + pair
+//     stores;
 //   balanced scheduling (long reductions): whole tiles for the full rounds, the (tile, chunk) units of the remainder
 //     dealt out evenly on the device (stream-K); the last segment of a cut tile to arrive sums all segments in slab
 //     order, cooperatively and coalesced.
@@ -33,11 +41,21 @@ namespace wmd {
 
 constexpr int TC_BM = 128;                      // rows per CTA tile = 2 warpgroups x wgmma M = 64
 constexpr int TC_BK = 32;                       // floats per chunk = one 128-byte row of a weight image
-constexpr int TC_THREADS = 256;                 // two warpgroups: both gather, each multiplies its 64 rows
-constexpr int TC_STAGES = 4;                    // cp.async ring: three chunks in flight while one is multiplied
+constexpr int TC_PRODUCERS = 128;               // warpgroup 0: tap tables and copies
+constexpr int TC_CONSUMERS = 256;               // warpgroups 1, 2: each multiplies its 64 rows, both run the epilogue
+constexpr int TC_THREADS = TC_PRODUCERS + TC_CONSUMERS;
+// setmaxnreg: every thread starts with the launch allocation (64 K registers / 384 threads, in steps of 8 = 168); the
+// consumers' increase waits until the producer's decrease has returned enough registers to the pool
+constexpr int TC_LAUNCH_REGS = (65536 / (TC_PRODUCERS + TC_CONSUMERS)) & ~7;
+constexpr int TC_PRODUCER_REGS = 40;
+constexpr int TC_CONSUMER_REGS = 232;
+constexpr int TC_STAGES = 4;                    // ring of chunk stages between the producer and the consumers
 constexpr int TC_A_LD = TC_BK + 4;              // raw A row pitch in floats (144 B: fragment reads hit 32 distinct banks)
 constexpr int TC_A_TILE = TC_BM * TC_A_LD * 4;  // 18 KB raw fp32
-constexpr int TC_TABLES = 2 * 9 * TC_BM * 4;
+constexpr int TC_TABLES = 2 * 9 * TC_BM * 4;    // one tap table: [source][tap][row]
+constexpr int TC_BARRIERS = 2 * TC_STAGES * 8;  // full[s], empty[s]
+static_assert(TC_PRODUCERS * (TC_LAUNCH_REGS - TC_PRODUCER_REGS) >= TC_CONSUMERS * (TC_CONSUMER_REGS - TC_LAUNCH_REGS),
+              "the consumers cannot take more registers than the producer gives back");
 
 // Per N-tile configuration.  A stage holds the chunk's weight image first (its size is a multiple of 4 KB, so every image
 // keeps the 1024-byte alignment of the 128-byte swizzle) and the raw A rows after it.
@@ -49,21 +67,52 @@ struct TcCfg {
   static constexpr int B_IMG = F16 ? B_TILE : 2 * B_TILE;
   static constexpr int ACC = BN / 2;                       // accumulator registers per thread (wgmma m64 x BN fragment)
   static constexpr int STAGE = B_IMG + TC_A_TILE;
-  static constexpr size_t SMEM = static_cast<size_t>(TC_STAGES) * STAGE + TC_TABLES + 1024;
+  static constexpr size_t SMEM = static_cast<size_t>(TC_STAGES) * STAGE + TC_TABLES + TC_BARRIERS + 1024;
   static_assert(STAGE % 1024 == 0, "weight images must stay 1024-byte aligned");
   static_assert(SMEM <= 227 * 1024, "one CTA must fit the shared memory of an SM");
 };
 constexpr int kFlushChunks = 32;                // epoch length: K = 1024 per wgmma accumulation run
+static_assert(kFlushChunks % 2 == 0, "an epoch starts on register set 0");
 constexpr int32_t kNoRow = -1;                  // tap-table entry of an inactive / padded source: the gather writes zeros
 
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-// cp.async writes through the generic proxy, wgmma reads shared memory through the async proxy
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+template <int N>   // until at most N committed groups of this warpgroup are pending
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+
+// mbarriers in shared memory (phase parity waits), the bulk copy that counts its bytes on one, and named barriers
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n"
+      "WMD_MBAR_WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra WMD_MBAR_WAIT;\n}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+// arrives on `bar` once every cp.async this thread has issued so far has landed; .noinc: the arrival is one of the
+// barrier's expected count
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void bulk_copy_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
+               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
+}
+constexpr int kProducerBar = 1, kConsumerBar = 2;   // named barrier ids (0 is __syncthreads)
 // keeps a register that an asynchronous wgmma reads or writes live and unmoved across the wait
 __device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
@@ -241,6 +290,67 @@ __host__ __device__ __forceinline__ BalPlan bal_plan(long long tiles, long long 
   return p;
 }
 
+// Work decomposition of one CTA.  A "unit" is one 32-channel chunk of one output tile.
+//   splits >= 1 : every tile's reduction is cut into `splits` equal ranges (split-K); splits == 1 = whole tiles.
+//   splits == 0 : BALANCED (data-parallel + stream-K, see bal_plan): all but the last full round run whole tiles;
+//                 the units of the remaining tiles are dealt out to all CTAs in equal contiguous ranges of U
+//                 units, so the SMs finish together however many tiles the (device-side) row count yields, and
+//                 only tiles cut by a range boundary pay for partial sums.
+// Segments that do not cover a whole tile write raw partial sums to the workspace; tc_reduce_kernel sums a tile's
+// segments in a fixed order and applies bias + activation, so results stay deterministic.
+// The producer and the consumers each step through their own copy of the walk: the same items in the same order.
+struct TcItem {
+  long long tile;
+  long long rem_t;                              // remainder-tile index (balanced partials)
+  int cb, ce;                                   // chunk range [cb, ce) of the tile's reduction
+  int slab;                                     // workspace slab of a partial segment
+  bool whole;                                   // the range is the whole reduction: the output rows are written here
+};
+struct TcWalk {
+  long long U, u, u_end, item, items, rem_tile0;
+  int splits, nchunks;
+  __device__ __forceinline__ TcWalk(long long tiles, int splits_, int nchunks_, const BalPlan& plan)
+      : splits(splits_), nchunks(nchunks_) {
+    const bool balanced = splits == 0;
+    rem_tile0 = balanced ? plan.rem_tile0 : 0;                          // first stream-K tile
+    const long long rem_units = balanced ? (tiles - rem_tile0) * nchunks : 0;
+    U = plan.U;
+    u = balanced ? static_cast<long long>(blockIdx.x) * U : 0;
+    u_end = balanced ? min(rem_units, u + U) : 0;
+    item = blockIdx.x;
+    items = balanced ? rem_tile0 : tiles * splits;
+  }
+  __device__ __forceinline__ bool next(TcItem& w) {
+    w.rem_t = 0;
+    if (splits == 0 && item < items) {                                  // data-parallel rounds
+      w.tile = item;
+      w.cb = 0; w.ce = nchunks; w.slab = 0; w.whole = true;
+      item += gridDim.x;
+    } else if (splits == 0) {                                           // stream-K over the remainder tiles
+      if (u >= u_end) return false;
+      w.rem_t = u / nchunks;
+      w.tile = rem_tile0 + w.rem_t;
+      w.cb = static_cast<int>(u - w.rem_t * nchunks);
+      w.ce = static_cast<int>(min(static_cast<long long>(nchunks), w.cb + (u_end - u)));
+      w.slab = static_cast<int>(blockIdx.x - (w.rem_t * nchunks) / U);
+      w.whole = (w.cb == 0 && w.ce == nchunks);
+      u += w.ce - w.cb;
+    } else {
+      if (item >= items) return false;
+      w.tile = item / splits;
+      w.slab = static_cast<int>(item - w.tile * splits);
+      w.cb = static_cast<int>(static_cast<long long>(w.slab) * nchunks / splits);
+      w.ce = static_cast<int>(static_cast<long long>(w.slab + 1) * nchunks / splits);
+      w.whole = (splits == 1);
+      item += gridDim.x;
+    }
+    return true;
+  }
+};
+
+template <int V>
+struct Ic { static constexpr int value = V; };   // a compile-time register-set index
+
 template <int BN, bool F16>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_conv_desc d, const float* __restrict__ wtc,
                                                                      const int splits, float* __restrict__ partial) {
@@ -252,10 +362,159 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   extern __shared__ unsigned char smem_dyn[];
   __shared__ int s_fixup;                                  // balanced mode: segments of the tile to reduce here (0 = not the last)
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  // the role as a warp-uniform value (a lane-0 broadcast): the consumers' wgmma run on paths the compiler knows do not
+  // diverge inside a warp, and are not serialised
+  const int warpgroup = __shfl_sync(0xffffffffu, tid / 128, 0);
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~static_cast<uintptr_t>(1023));
   int32_t* tab0 = reinterpret_cast<int32_t*>(base + TC_STAGES * STAGE);   // [tap][row]: source row in x0, -1 = none
   int32_t* tab1 = tab0 + 9 * TC_BM;                                        // ... in x1
+  uint64_t* full = reinterpret_cast<uint64_t*>(base + TC_STAGES * STAGE + TC_TABLES);   // stage s holds its chunk
+  uint64_t* empty = full + TC_STAGES;                                                    // both consumers are done with s
+
+  const long long HW = static_cast<long long>(d.H) * d.W;
+  const int total_px = static_cast<int>(static_cast<long long>(d.N) * HW);
+  int rows = d.pixels ? *d.count : total_px;
+  rows = __shfl_sync(0xffffffffu, min(rows, d.max_rows), 0);   // warp-uniform, and so is the whole work walk
+  const int nch0 = (d.c0 + TC_BK - 1) / TC_BK, nch1 = (d.c1 + TC_BK - 1) / TC_BK;
+  const int per_tap = nch0 + nch1;
+  const int nchunks = d.taps * per_tap;
+  const int n_tiles = (d.cout + BN - 1) / BN;
+  const long long tiles = static_cast<long long>((rows + TC_BM - 1) / TC_BM) * n_tiles;
+  const bool balanced = (splits == 0);
+  const BalPlan plan = bal_plan(tiles, gridDim.x, nchunks);
+  TcWalk walk(tiles, splits, nchunks, plan);
+  TcItem it;
+
+  if (tid == 0) {
+#pragma unroll
+    for (int s = 0; s < TC_STAGES; ++s) {
+      mbar_init(full + s, TC_PRODUCERS + 1);               // every producer thread's copies + the weight image's bytes
+      mbar_init(empty + s, TC_CONSUMERS / 32);             // one arrival per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warpgroup == 0) {
+    // ================================================================ producer: tap tables, weight images, A rows
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(TC_PRODUCER_REGS));
+    const int Hs = d.H >> d.shift0, Ws = d.W >> d.shift0;
+    const bool aligned_rows = (d.taps == 1 && d.map0 == nullptr);
+    // rows each source holds: a row index past them reads zeros (a 1x1 stage over its own rows may run past x0's end)
+    const long long rows_x0 = (aligned_rows && d.rows0 > 0) ? d.rows0 : static_cast<long long>(d.N) * Hs * Ws;
+    const long long rows_x1 = static_cast<long long>(d.N) * HW;
+    const unsigned char* wimg = reinterpret_cast<const unsigned char*>(wtc) + (F16 ? 128 : 0);   // f16 images follow a 128-byte header
+    uint32_t g = 0;                                        // chunks this CTA has issued: stage g % TC_STAGES, use g / TC_STAGES
+    while (walk.next(it)) {
+      const int m0 = static_cast<int>(it.tile / n_tiles) * TC_BM;
+      const int nt = static_cast<int>(it.tile % n_tiles);
+      // The previous tile's copies have all been issued (they read the table when they are issued): one table is enough,
+      // and it is built while the consumers still multiply the previous tile's last chunks.
+      named_bar_sync(kProducerBar, TC_PRODUCERS);
+      // thread t: tile row t; the output pixel is read and decoded once per row.  Taps in rounds of two: first every
+      // tap's coordinates and its three look-ups (gate byte, source-0 index map, source-1 index map) are issued together -
+      // the maps are read whether or not the gate turns out to be set, their indices are valid for every in-range
+      // coordinate - then the results are combined.
+      {
+        const int r = tid;
+        const int m = m0 + r;
+        int n = 0, y = 0, x = 0;
+        const bool live = m < rows;
+        if (live) {
+          const unsigned p = static_cast<unsigned>(d.pixels ? d.pixels[m] : m);     // < 2^31 (checked by the host): 32-bit divisions
+          const unsigned hw = static_cast<unsigned>(HW);
+          n = static_cast<int>(p / hw);
+          const unsigned rem = p - static_cast<unsigned>(n) * hw;
+          y = static_cast<int>(rem / static_cast<unsigned>(d.W));
+          x = static_cast<int>(rem - static_cast<unsigned>(y) * static_cast<unsigned>(d.W));
+        }
+        constexpr int kTapsPerRound = 2;
+#pragma unroll 1
+        for (int t_lo = 0; t_lo < d.taps; t_lo += kTapsPerRound) {
+          const int t_hi = min(d.taps, t_lo + kTapsPerRound);
+          int qv[kTapsPerRound];                   // source-1 pixel of the tap, -1 = out of range / dead row
+          uint8_t gv[kTapsPerRound];
+          int32_t m0v[kTapsPerRound], m1v[kTapsPerRound];
+#pragma unroll
+          for (int k = 0; k < kTapsPerRound; ++k) {
+            const int tap = t_lo + k;
+            qv[k] = -1;
+            gv[k] = 1;
+            m0v[k] = kNoRow;
+            m1v[k] = kNoRow;
+            if (live && tap < t_hi) {
+              int qy = y, qx = x;
+              if (d.taps == 9) { qy += tap / 3 - 1; qx += tap % 3 - 1; }
+              bool ok = pad_coord(qy, d.H, d.pad_mode);
+              ok = pad_coord(qx, d.W, d.pad_mode) && ok;
+              if (ok) {
+                const int q = (n * d.H + qy) * d.W + qx;
+                qv[k] = q;
+                if (d.gate) gv[k] = d.gate[q];
+                m1v[k] = d.map1 ? d.map1[q] : q;    // -1 (not in the compact skip list) = kNoRow
+                if (aligned_rows) {
+                  m0v[k] = m;
+                } else {
+                  const int qs = (n * Hs + (qy >> d.shift0)) * Ws + (qx >> d.shift0);
+                  m0v[k] = d.map0 ? d.map0[qs] : qs;
+                }
+              }
+            }
+          }
+#pragma unroll
+          for (int k = 0; k < kTapsPerRound; ++k) {
+            const int tap = t_lo + k;
+            if (tap < t_hi) {
+              const bool ok = qv[k] >= 0 && gv[k] != 0;
+              tab0[tap * TC_BM + r] = (ok && m0v[k] >= 0 && m0v[k] < rows_x0) ? m0v[k] : kNoRow;
+              tab1[tap * TC_BM + r] = (ok && m1v[k] < rows_x1) ? m1v[k] : kNoRow;
+            }
+          }
+        }
+      }
+      named_bar_sync(kProducerBar, TC_PRODUCERS);
+
+      // Chunk c of the tile into stage s: the weight image as it is (one bulk copy), and the implicit im2col - for every
+      // tile row the 32-channel slice of its tap's source row (channel chunk outermost, taps innermost: the nine taps of
+      // a chunk re-read (almost) the same rows while they are hot in L2).  No row / channels past C: zero fill.
+      const unsigned char* wtile = wimg + static_cast<long long>(nt) * nchunks * B_IMG;
+#pragma unroll 1
+      for (int c = it.cb; c < it.ce; ++c, ++g) {
+        const int s = static_cast<int>(g % TC_STAGES);
+        if (g >= TC_STAGES) mbar_wait(empty + s, ((g / TC_STAGES) - 1) & 1);
+        unsigned char* st = base + s * STAGE;
+        if (tid == 0) {
+          mbar_arrive_expect_tx(full + s, B_IMG);
+          bulk_copy_g2s(st, wtile + static_cast<long long>(c) * B_IMG, B_IMG, full + s);
+        }
+        const int rr = c / d.taps;
+        const int tap = c - rr * d.taps;
+        const bool src1 = rr >= nch0;
+        const int col = (src1 ? rr - nch0 : rr) * TC_BK;
+        const float* x = src1 ? d.x1 : d.x0;
+        const long long ld = src1 ? d.ld1 : d.ld0;
+        const int csrc = src1 ? d.c1 : d.c0;
+        const int32_t* tab = (src1 ? tab1 : tab0) + tap * TC_BM;
+        float* sa = reinterpret_cast<float*>(st + B_IMG);
+#pragma unroll
+        for (int i = 0; i < TC_BM * 8 / TC_PRODUCERS; ++i) {
+          const int pc = tid + i * TC_PRODUCERS, r = pc >> 3, q = pc & 7;
+          const int32_t srow = tab[r];
+          const int cc = col + 4 * q;
+          const int bytes = srow >= 0 ? min(16, max(0, (csrc - cc) * 4)) : 0;
+          cp_async16(sa + r * TC_A_LD + 4 * q, bytes ? x + srow * ld + cc : x, bytes);
+        }
+        cp_async_mbar_arrive(full + s);
+      }
+    }
+    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    return;
+  }
+
+  // ================================================================== consumers: multiply, epilogue, stream-K fix-up
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(TC_CONSUMER_REGS));
+  const int ctid = tid - TC_PRODUCERS;
 
   // F16: operands are fed as fp16 pairs.  Activations are scaled by a power of two chosen from the sources' max |x| (device
   // scalars written by their producers: layout moves, earlier convolutions) so that max |x| s lies in (2^13, 2^14] - no
@@ -275,262 +534,133 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     ascale = ldexpf(1.f, e);
     out_scale = ldexpf(1.f, -e) * __ldg(wtc);    // header word 0: 1 / weight scale
   }
-  const long long HW = static_cast<long long>(d.H) * d.W;
-  const int total_px = static_cast<int>(static_cast<long long>(d.N) * HW);
-  int rows = d.pixels ? *d.count : total_px;
-  rows = min(rows, d.max_rows);
-  const int nch0 = (d.c0 + TC_BK - 1) / TC_BK, nch1 = (d.c1 + TC_BK - 1) / TC_BK;
-  const int per_tap = nch0 + nch1;
-  const int nchunks = d.taps * per_tap;
-  const int n_tiles = (d.cout + BN - 1) / BN;
-  const long long tiles = static_cast<long long>((rows + TC_BM - 1) / TC_BM) * n_tiles;
-  const int Hs = d.H >> d.shift0, Ws = d.W >> d.shift0;
-  const bool aligned_rows = (d.taps == 1 && d.map0 == nullptr);
-  // rows each source holds: a row index past them reads zeros (a 1x1 stage over its own rows may run past x0's end)
-  const long long rows_x0 = (aligned_rows && d.rows0 > 0) ? d.rows0 : static_cast<long long>(d.N) * Hs * Ws;
-  const long long rows_x1 = static_cast<long long>(d.N) * HW;
 
-  // fragment ownership: warpgroup wg, warp wq of it; rows row_a and row_a + 8 of the tile, columns 8j + 2 t4 + {0, 1}
-  const int wg = warp >> 2, wq = warp & 3, t4 = lane & 3;
+  // fragment ownership: consumer warpgroup wg, warp wq of it; rows row_a and row_a + 8 of the tile, columns 8j + 2 t4 + {0, 1}
+  const int wg = ctid >> 7, wq = (ctid >> 5) & 3, t4 = lane & 3;
   const int row_a = wg * 64 + wq * 16 + (lane >> 2);
+  // rows / bias 8-byte aligned: the epilogue's pair form for the pairs inside cout
+  const bool al_ok = (d.ldy % 2 == 0) && ((reinterpret_cast<uintptr_t>(d.y) & 7) == 0) &&
+                     ((reinterpret_cast<uintptr_t>(d.bias) & 7) == 0);
 
-  // Work decomposition.  A "unit" is one 32-channel chunk of one output tile.
-  //   splits >= 1 : every tile's reduction is cut into `splits` equal ranges (split-K); splits == 1 = whole tiles.
-  //   splits == 0 : BALANCED (data-parallel + stream-K, see bal_plan): all but the last full round run whole tiles;
-  //                 the units of the remaining tiles are dealt out to all CTAs in equal contiguous ranges of U
-  //                 units, so the SMs finish together however many tiles the (device-side) row count yields, and
-  //                 only tiles cut by a range boundary pay for partial sums.
-  // Segments that do not cover a whole tile write raw partial sums to the workspace; tc_reduce_kernel sums a tile's
-  // segments in a fixed order and applies bias + activation, so results stay deterministic.
-  const bool balanced = (splits == 0);
-  const BalPlan plan = bal_plan(tiles, gridDim.x, nchunks);
-  const long long rem_tile0 = balanced ? plan.rem_tile0 : 0;            // first stream-K tile
-  const long long rem_units = balanced ? (tiles - rem_tile0) * nchunks : 0;
-  const long long U = plan.U;
-  long long u = balanced ? static_cast<long long>(blockIdx.x) * U : 0;
-  const long long u_end = balanced ? min(rem_units, u + U) : 0;
-  long long item = blockIdx.x;
-  const long long items = balanced ? rem_tile0 : tiles * splits;
-  while (true) {
-    long long tile;
-    int cb, ce, slab;
-    bool whole;
-    long long rem_t = 0;                                                // remainder-tile index (balanced partials)
-    if (balanced && item < items) {                                     // data-parallel rounds
-      tile = item;
-      cb = 0; ce = nchunks; slab = 0; whole = true;
-      item += gridDim.x;
-    } else if (balanced) {                                              // stream-K over the remainder tiles
-      if (u >= u_end) break;
-      rem_t = u / nchunks;
-      tile = rem_tile0 + rem_t;
-      cb = static_cast<int>(u - rem_t * nchunks);
-      ce = static_cast<int>(min(static_cast<long long>(nchunks), cb + (u_end - u)));
-      slab = static_cast<int>(blockIdx.x - (rem_t * nchunks) / U);
-      whole = (cb == 0 && ce == nchunks);
-      u += ce - cb;
+  // A fragments of a chunk, two register sets: the next chunk's are read and split while the current one's MMAs run.
+  // tf32: fa = hi, fb = lo; f16: fa = h1, fb = h2.
+  constexpr int KS = F16 ? TC_BK / 16 : TC_BK / 8;          // k-steps per chunk
+  uint32_t fa[2][KS][4], fb[2][KS][4];
+  float acc[ACC];
+  float dacc[ACC];                                         // the wgmma accumulators of the running epoch
+#pragma unroll
+  for (int j = 0; j < ACC; ++j) dacc[j] = 0.f;
+
+  // wait for stage gi % TC_STAGES to hold chunk gi, then read this thread's fragment elements into register set B
+  auto load_frag = [&](auto B, uint32_t gi) {
+    constexpr int b = decltype(B)::value;
+    const int s = static_cast<int>(gi % TC_STAGES);
+    mbar_wait(full + s, (gi / TC_STAGES) & 1);
+    const float* sa = reinterpret_cast<const float*>(base + s * STAGE + B_IMG);
+    if (F16) {
+      // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
+      // precision of the tf32 hi / lo pair.  Fragment of k-step ks: rows (r, r + 8) x channels 16 ks + 2 t4 + {0, 1}, + 8
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 v = *reinterpret_cast<const float2*>(sa + (row_a + (e & 1) * 8) * TC_A_LD + ks * 16 + 2 * t4 + (e >> 1) * 8);
+          const float b0f = v.x * ascale, b1f = v.y * ascale;
+          const uint32_t p = pack_f16x2(b0f, b1f);
+          fa[b][ks][e] = p;
+          fb[b][ks][e] = pack_f16x2(b0f - f16_lo_to_f32(p), b1f - f16_hi_to_f32(p));
+        }
+      }
     } else {
-      if (item >= items) break;
-      tile = item / splits;
-      slab = static_cast<int>(item - tile * splits);
-      cb = static_cast<int>(static_cast<long long>(slab) * nchunks / splits);
-      ce = static_cast<int>(static_cast<long long>(slab + 1) * nchunks / splits);
-      whole = (splits == 1);
-      item += gridDim.x;
-    }
-    const int len = ce - cb;
-    const int m0 = static_cast<int>(tile / n_tiles) * TC_BM;
-    const int nt = static_cast<int>(tile % n_tiles);
-    const int n0 = nt * BN;
-    // rows / bias 8-byte aligned: the epilogue's pair form for the pairs inside cout
-    const bool al_ok = (d.ldy % 2 == 0) && ((reinterpret_cast<uintptr_t>(d.y) & 7) == 0) &&
-                       ((reinterpret_cast<uintptr_t>(d.bias) & 7) == 0);
-
-    // thread t: tile row t % 128, taps [t / 128 * 5, ...): the output pixel is read and decoded once per row, the taps'
-    // gate / map lookups are independent loads
-    {
-      const int r = tid & (TC_BM - 1);
-      const int t_lo = (tid >> 7) * 5, t_hi = min(d.taps, t_lo + 5);
-      const int m = m0 + r;
-      int n = 0, y = 0, x = 0;
-      const bool live = m < rows;
-      if (live && t_lo < t_hi) {
-        const unsigned p = static_cast<unsigned>(d.pixels ? d.pixels[m] : m);     // < 2^31 (checked by the host): 32-bit divisions
-        const unsigned hw = static_cast<unsigned>(HW);
-        n = static_cast<int>(p / hw);
-        const unsigned rem = p - static_cast<unsigned>(n) * hw;
-        y = static_cast<int>(rem / static_cast<unsigned>(d.W));
-        x = static_cast<int>(rem - static_cast<unsigned>(y) * static_cast<unsigned>(d.W));
-      }
-      // Two rounds of loads for the thread's (up to) five taps instead of one dependent chain per tap: first every tap's
-      // coordinates and its three look-ups (gate byte, source-0 index map, source-1 index map) are issued together - the maps
-      // are read whether or not the gate turns out to be set, their indices are valid for every in-range coordinate - then
-      // the results are combined.
-      constexpr int kTapsPerThread = 5;
-      int qv[kTapsPerThread];                        // source-1 pixel of the tap, -1 = out of range / dead row
-      uint8_t gv[kTapsPerThread];
-      int32_t m0v[kTapsPerThread], m1v[kTapsPerThread];
+      // fragment of k-step ks: rows (r, r + 8) x channels 8 ks + t4, + 4; tf32 hi by truncation, exact remainder lo
 #pragma unroll
-      for (int k = 0; k < kTapsPerThread; ++k) {
-        const int tap = t_lo + k;
-        qv[k] = -1;
-        gv[k] = 1;
-        m0v[k] = kNoRow;
-        m1v[k] = kNoRow;
-        if (live && tap < t_hi) {
-          int qy = y, qx = x;
-          if (d.taps == 9) { qy += tap / 3 - 1; qx += tap % 3 - 1; }
-          bool ok = pad_coord(qy, d.H, d.pad_mode);
-          ok = pad_coord(qx, d.W, d.pad_mode) && ok;
-          if (ok) {
-            const int q = (n * d.H + qy) * d.W + qx;
-            qv[k] = q;
-            if (d.gate) gv[k] = d.gate[q];
-            m1v[k] = d.map1 ? d.map1[q] : q;        // -1 (not in the compact skip list) = kNoRow
-            if (aligned_rows) {
-              m0v[k] = m;
-            } else {
-              const int qs = (n * Hs + (qy >> d.shift0)) * Ws + (qx >> d.shift0);
-              m0v[k] = d.map0 ? d.map0[qs] : qs;
-            }
-          }
-        }
-      }
+      for (int ks = 0; ks < KS; ++ks) {
 #pragma unroll
-      for (int k = 0; k < kTapsPerThread; ++k) {
-        const int tap = t_lo + k;
-        if (tap < t_hi) {
-          const bool ok = qv[k] >= 0 && gv[k] != 0;
-          tab0[tap * TC_BM + r] = (ok && m0v[k] >= 0 && m0v[k] < rows_x0) ? m0v[k] : kNoRow;
-          tab1[tap * TC_BM + r] = (ok && m1v[k] < rows_x1) ? m1v[k] : kNoRow;
+        for (int e = 0; e < 4; ++e) {
+          const float v = sa[(row_a + (e & 1) * 8) * TC_A_LD + ks * 8 + t4 + (e >> 1) * 4];
+          fa[b][ks][e] = __float_as_uint(v) & 0xFFFFE000u;
+          fb[b][ks][e] = __float_as_uint(v - __uint_as_float(fa[b][ks][e]));
         }
       }
     }
-    __syncthreads();
-
-    const unsigned char* wtile = reinterpret_cast<const unsigned char*>(wtc) +
-                                 (F16 ? 128 : 0) + static_cast<long long>(nt) * nchunks * B_IMG;   // f16 images follow a 128-byte header
-
-    // Chunk c of the tile into stage s: the weight image as it is, and the implicit im2col - for every tile row the
-    // 32-channel slice of its tap's source row (channel chunk outermost, taps innermost: the nine taps of a chunk re-read
-    // (almost) the same rows while they are hot in L2).  No row / channels past C: zero fill.
-    auto load_chunk = [&](int c, int s) {
-      unsigned char* st = base + s * STAGE;
-      const unsigned char* wsrc = wtile + static_cast<long long>(c) * B_IMG;
+  };
+  auto fence_frag = [&](auto B) {                           // the set stays live and unmoved until its MMAs have retired
+    constexpr int b = decltype(B)::value;
 #pragma unroll
-      for (int i = 0; i < B_IMG / 16 / TC_THREADS; ++i) {
-        const int o = (tid + i * TC_THREADS) * 16;
-        cp_async16(st + o, wsrc + o, 16);
-      }
-      const int rr = c / d.taps;
-      const int tap = c - rr * d.taps;
-      const bool src1 = rr >= nch0;
-      const int col = (src1 ? rr - nch0 : rr) * TC_BK;
-      const float* x = src1 ? d.x1 : d.x0;
-      const long long ld = src1 ? d.ld1 : d.ld0;
-      const int csrc = src1 ? d.c1 : d.c0;
-      const int32_t* tab = (src1 ? tab1 : tab0) + tap * TC_BM;
-      float* sa = reinterpret_cast<float*>(st + B_IMG);
+    for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
-      for (int i = 0; i < TC_BM * 8 / TC_THREADS; ++i) {
-        const int pc = tid + i * TC_THREADS, r = pc >> 3, q = pc & 7;
-        const int32_t srow = tab[r];
-        const int cc = col + 4 * q;
-        const int bytes = srow >= 0 ? min(16, max(0, (csrc - cc) * 4)) : 0;
-        cp_async16(sa + r * TC_A_LD + 4 * q, bytes ? x + srow * ld + cc : x, bytes);
-      }
-    };
+      for (int e = 0; e < 4; ++e) { reg_fence(fa[b][ks][e]); reg_fence(fb[b][ks][e]); }
+  };
+  auto release = [&](uint32_t gi) {                          // this warp is done with the stage of chunk gi
+    if (lane == 0) mbar_arrive(empty + gi % TC_STAGES);
+  };
 
-    float acc[ACC];
+  uint32_t g = 0;                                          // chunks this CTA has consumed
+  while (walk.next(it)) {
+    const int len = it.ce - it.cb;
+    const int m0 = static_cast<int>(it.tile / n_tiles) * TC_BM;
+    const int n0 = static_cast<int>(it.tile % n_tiles) * BN;
+    const long long rem_t = it.rem_t;
+    const int slab = it.slab;
+    const bool whole = it.whole;
 #pragma unroll
     for (int j = 0; j < ACC; ++j) acc[j] = 0.f;
-    float dacc[ACC];                              // the wgmma accumulators of the running epoch
-#pragma unroll
-    for (int j = 0; j < ACC; ++j) dacc[j] = 0.f;
-    float out_max = 0.f;                          // max |y| this thread stores in this tile (-> d.amax_out)
+    float out_max = 0.f;                                   // max |y| this thread stores in this tile (-> d.amax_out)
 
+    // Chunk i of the segment from register set B: its MMAs are issued, then the previous chunk's group is waited for: its
+    // stage goes back to the producer, its register set takes chunk i + 1's fragments.  The first MMA of an epoch
+    // overwrites the accumulators.
+    auto step = [&](auto B, int i) {
+      constexpr int b = decltype(B)::value;
+      const uint32_t gi = g + i;
+      const uint64_t b0 = wgmma_desc_sw128(smem_u32(base + (gi % TC_STAGES) * STAGE));
+      const uint32_t keep = (i % kFlushChunks) != 0;
+      wgmma_fence();
 #pragma unroll
-    for (int s = 0; s < TC_STAGES - 1; ++s) {
-      if (s < len) load_chunk(cb + s, s);
-      cp_async_commit();                          // empty groups keep the wait counts uniform
-    }
-    for (int i = 0; i < len; ++i) {
-      cp_async_wait<TC_STAGES - 2>();             // this thread's copies of chunk i have landed
-      fence_proxy_async();
-      __syncthreads();                            // everyone's have; both warpgroups are done with chunk i - 1
-      if (i + TC_STAGES - 1 < len) load_chunk(cb + i + TC_STAGES - 1, (i + TC_STAGES - 1) % TC_STAGES);
-      cp_async_commit();
-      const unsigned char* st = base + (i % TC_STAGES) * STAGE;
-      const float* sa = reinterpret_cast<const float*>(st + B_IMG);
-      const uint64_t b0 = wgmma_desc_sw128(smem_u32(st));
-      const uint32_t keep = (i % kFlushChunks) != 0;    // the first MMA of an epoch overwrites the accumulators
-      if (F16) {
-        // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
-        // precision of the tf32 hi / lo pair.  Fragment of k-step ks: rows (r, r + 8) x channels 16 ks + 2 t4 + {0, 1}, + 8
-        uint32_t h1[TC_BK / 16][4], h2[TC_BK / 16][4];
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 16; ++ks) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 v = *reinterpret_cast<const float2*>(sa + (row_a + (e & 1) * 8) * TC_A_LD + ks * 16 + 2 * t4 + (e >> 1) * 8);
-            const float b0f = v.x * ascale, b1f = v.y * ascale;
-            const uint32_t p = pack_f16x2(b0f, b1f);
-            h1[ks][e] = p;
-            h2[ks][e] = pack_f16x2(b0f - f16_lo_to_f32(p), b1f - f16_hi_to_f32(p));
-          }
-        }
-        wgmma_fence();
-        // rows of the weight tile: [h1: 64 B | h2: 64 B]; a k-step is 16 channels = 32 B
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 16; ++ks) {
+      for (int ks = 0; ks < KS; ++ks) {
+        if (F16) {
+          // rows of the weight tile: [h1: 64 B | h2: 64 B]; a k-step is 16 channels = 32 B
           const uint64_t bh = b0 + static_cast<uint64_t>(2 * ks);
           const uint64_t bl = bh + 4u;
-          Wgmma<BN, true>::mma(dacc, h2[ks], bh, ks == 0 ? keep : 1u);   // lo*hi
-          Wgmma<BN, true>::mma(dacc, h1[ks], bl, 1u);                    // hi*lo
-          Wgmma<BN, true>::mma(dacc, h1[ks], bh, 1u);                    // hi*hi
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 16; ++ks)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { reg_fence(h1[ks][e]); reg_fence(h2[ks][e]); }
-      } else {
-        // fragment of k-step ks: rows (r, r + 8) x channels 8 ks + t4, + 4; tf32 hi by truncation, exact remainder lo
-        uint32_t hi[TC_BK / 8][4], lo[TC_BK / 8][4];
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 8; ++ks) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float v = sa[(row_a + (e & 1) * 8) * TC_A_LD + ks * 8 + t4 + (e >> 1) * 4];
-            hi[ks][e] = __float_as_uint(v) & 0xFFFFE000u;
-            lo[ks][e] = __float_as_uint(v - __uint_as_float(hi[ks][e]));
-          }
-        }
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 8; ++ks) {
+          Wgmma<BN, true>::mma(dacc, fb[b][ks], bh, ks == 0 ? keep : 1u);   // lo*hi
+          Wgmma<BN, true>::mma(dacc, fa[b][ks], bl, 1u);                    // hi*lo
+          Wgmma<BN, true>::mma(dacc, fa[b][ks], bh, 1u);                    // hi*hi
+        } else {
           const uint64_t bh = b0 + static_cast<uint64_t>(2 * ks);
           const uint64_t bl = bh + static_cast<uint64_t>(TC_B_TILE >> 4);
-          Wgmma<BN, false>::mma(dacc, lo[ks], bh, ks == 0 ? keep : 1u);  // lo*hi
-          Wgmma<BN, false>::mma(dacc, hi[ks], bl, 1u);                   // hi*lo
-          Wgmma<BN, false>::mma(dacc, hi[ks], bh, 1u);                   // hi*hi
+          Wgmma<BN, false>::mma(dacc, fb[b][ks], bh, ks == 0 ? keep : 1u);  // lo*hi
+          Wgmma<BN, false>::mma(dacc, fa[b][ks], bl, 1u);                   // hi*lo
+          Wgmma<BN, false>::mma(dacc, fa[b][ks], bh, 1u);                   // hi*hi
         }
-        wgmma_commit();
-        wgmma_wait_all();
-#pragma unroll
-        for (int ks = 0; ks < TC_BK / 8; ++ks)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) { reg_fence(hi[ks][e]); reg_fence(lo[ks][e]); }
       }
+      wgmma_commit();
+      wgmma_wait<1>();                                     // chunk i - 1 has retired
+      fence_frag(Ic<1 - b>());
+      if (i > 0) release(gi - 1);
+      if (i + 1 < len) load_frag(Ic<1 - b>(), gi + 1);
+    };
+    // Epochs of kFlushChunks chunks counted from the segment start (even: chunk i always uses register set i % 2).  The
+    // accumulators are read only after an epoch's last group has retired, outside any branch, so the compiler keeps the
+    // wgmma of the epoch asynchronous.
+    load_frag(Ic<0>(), g);
+#pragma unroll 1
+    for (int e0 = 0; e0 < len; e0 += kFlushChunks) {
+      const int e1 = min(len, e0 + kFlushChunks);
+#pragma unroll 1
+      for (int i = e0; i < e1; i += 2) {
+        step(Ic<0>(), i);
+        if (i + 1 < e1) step(Ic<1>(), i + 1);
+      }
+      wgmma_wait<0>();
+      fence_frag(Ic<0>());
+      fence_frag(Ic<1>());
 #pragma unroll
       for (int j = 0; j < ACC; ++j) reg_fence(dacc[j]);
-      if (((i + 1) % kFlushChunks == 0) || (i == len - 1)) {
 #pragma unroll
-        for (int j = 0; j < ACC; ++j) acc[j] += dacc[j];
-      }
+      for (int j = 0; j < ACC; ++j) acc[j] += dacc[j];
     }
-    cp_async_wait<0>();
+    release(g + len - 1);
+    g += len;
 
     // ---- epilogue: bias, activation, pair stores.  acc[4 j + 2 h + e] = row row_a + 8 h, column 8 j + 2 t4 + e
 #pragma unroll
@@ -596,16 +726,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     // activation and writes the rows.  No CTA waits for another one and the result does not depend on who is last.
     if (balanced && !whole) {
       __threadfence();
-      __syncthreads();
-      if (tid == 0) {
-        const long long first = (rem_t * nchunks) / U, last = ((rem_t + 1) * nchunks - 1) / U;
+      named_bar_sync(kConsumerBar, TC_CONSUMERS);
+      if (ctid == 0) {
+        const long long first = (rem_t * nchunks) / plan.U, last = ((rem_t + 1) * nchunks - 1) / plan.U;
         const int nseg = static_cast<int>(last - first + 1);
         unsigned* cnt = reinterpret_cast<unsigned*>(partial) + rem_t;
         const unsigned t = atomicAdd(cnt, 1u);
         s_fixup = (t == static_cast<unsigned>(nseg - 1)) ? nseg : 0;
         if (s_fixup) *cnt = 0u;
       }
-      __syncthreads();
+      named_bar_sync(kConsumerBar, TC_CONSUMERS);
       const int nseg = s_fixup;
       if (nseg > 0) {
         __threadfence();
@@ -617,16 +747,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
         constexpr int kQuadsPerRow = BN / 4;
         constexpr int kQuads = TC_BM * kQuadsPerRow;
         constexpr int kUnroll = 4;
-        static_assert(kQuads % (TC_THREADS * kUnroll) == 0, "quads of a tile divide evenly");
+        static_assert(kQuads % (TC_CONSUMERS * kUnroll) == 0, "quads of a tile divide evenly");
         const int tile_rows = min(TC_BM, rows - m0);
         const float ap = d.act_param;
-        for (int base = tid; base < kQuads; base += TC_THREADS * kUnroll) {
+        for (int qbase = ctid; qbase < kQuads; qbase += TC_CONSUMERS * kUnroll) {
           float4 v[kUnroll], bq[kUnroll];
           int r[kUnroll], co[kUnroll];
           bool live[kUnroll];
 #pragma unroll
           for (int q = 0; q < kUnroll; ++q) {
-            const int idx = base + q * TC_THREADS;
+            const int idx = qbase + q * TC_CONSUMERS;
             r[q] = idx / kQuadsPerRow;
             co[q] = n0 + 4 * (idx % kQuadsPerRow);
             live[q] = r[q] < tile_rows && co[q] < d.cout;
@@ -644,11 +774,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
             v[q] = F16 ? make_float4(0.f, 0.f, 0.f, 0.f) : bq[q];
           }
           for (int sidx = 0; sidx < nseg; ++sidx) {
-            const float4* ps = reinterpret_cast<const float4*>(pb + static_cast<long long>(sidx) * TC_BM * BN) + base;
+            const float4* ps = reinterpret_cast<const float4*>(pb + static_cast<long long>(sidx) * TC_BM * BN) + qbase;
 #pragma unroll
             for (int q = 0; q < kUnroll; ++q) {
               if (live[q]) {
-                const float4 pq = __ldcg(ps + q * TC_THREADS);
+                const float4 pq = __ldcg(ps + q * TC_CONSUMERS);
                 v[q].x += pq.x; v[q].y += pq.y; v[q].z += pq.z; v[q].w += pq.w;
               }
             }
@@ -682,7 +812,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       for (int o = 16; o > 0; o >>= 1) out_max = fmaxf(out_max, __shfl_xor_sync(0xffffffffu, out_max, o));
       if (lane == 0 && out_max > __ldcg(d.amax_out)) atomicMax(reinterpret_cast<unsigned*>(d.amax_out), __float_as_uint(out_max));   // most warps skip the atomic
     }
-    __syncthreads();   // tap tables and stages free for the next tile
   }
 }
 
