@@ -190,7 +190,7 @@ typedef struct wmd_conv_desc {
   const float* amax0;       /* device scalars: max |x0|, max |x1| over the rows the launch can read (upper bounds are fine) */
   const float* amax1;
   float* amax_out;          /* device scalar, or NULL: atomically raised to max |y| of the rows written (zero it before the
-                               first producer; both precisions) */
+                               first producer; both precisions, every scheduling mode) */
   int32_t rows0;            /* rows allocated in x0, 0 = unknown.  Only used by the tensor-core engine's 1x1 form (taps == 1,
                                map0 == NULL: output row m reads x0 row m): with rows0 > 0 rows past rows0 read zeros */
 } wmd_conv_desc;
@@ -198,14 +198,16 @@ typedef struct wmd_conv_desc {
 int wmd_conv_rows_f32(const wmd_conv_desc* d, wmd_stream_t stream);
 
 /* Tensor-core engine for the same contract: wgmma tf32 with a 3xTF32 split (hi*hi + lo*hi + hi*lo,
- * fp32 accumulation), so results stay fp32-faithful (<= ~1e-6 relative vs the SIMT kernel).  d->w must
+ * fp32 accumulation), so results stay fp32-faithful: |y - exact| <= 1.7e-5 S, S = |bias| + sum |x w| of the element's
+ * terms (measured worst, same-sign operands, H100; f16x3: 8.6e-6 S, the SIMT kernel: 6.5e-6 S at K = 18432).  d->w must
  * point to weights packed by wmd_pack_conv_weight_tc_f32 for the same (cout, c0, c1, taps); d->ldw is ignored.
  *   wmd_conv_tc_tile_n(cout)                 N-tile of the kernel for this cout (128 / 64 / 32; the CTA tile is 128 rows x N)
  *   wmd_conv_tc_weight_floats(...)           size of the packed weight buffer, in floats
  *   wmd_pack_conv_weight_tc_f32(w, packed..) (Cout, c0+c1, kh, kw) -> per (n-tile, 32-channel chunk) fp32
  *                                            shared-memory images [tf32 hi | tf32 lo] of N x 32, K-major, 128-byte swizzled
  * Accumulation runs in epochs of K = 1024 in the wgmma accumulators, each added into fp32 registers with
- * round-to-nearest adds, because the tensor core's own fp32 accumulation does not round to nearest (bias ~6.5e-9 * K relative). */
+ * round-to-nearest adds, because the tensor core's own fp32 accumulation does not round to nearest (a one-signed bias of
+ * ~1.6e-8 * K of S in tf32x3, ~8.5e-9 * K in f16x3, measured on H100: it stays that of one epoch, not of the whole K). */
 enum { WMD_PREC_TF32X3 = 0, WMD_PREC_F16X3 = 1 };
 int wmd_conv_tc_tile_n(int cout);
 /* Weights for precision = WMD_PREC_F16X3: 128-byte header (float 0: 1 / s_w) + per (n-tile, 32-channel chunk) one N x 128 B

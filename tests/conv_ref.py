@@ -1,0 +1,121 @@
+"""fp64 reference of the gather-GEMM convolution contract (wmd_conv_desc, include/wmd.h), in plain torch.
+
+A direct restatement of the comment above wmd_conv_desc: for output row m (pixel p = pixels[m], or m itself) and tap
+(dy, dx) the input pixel q = p + (dy, dx) is mapped into the image by the pad mode (reflect / replicate), or reads zeros
+(zero padding); the gate zeros both sources at q; source 0 is x0[map0[n, qy >> shift0, qx >> shift0]] (map0 None: that
+pixel's linear index; taps == 1 and map0 None: row m itself, zeros past rows0), source 1 is x1[map1[q]] (map1 None: row q);
+a row index of -1 reads zeros.  Returns y64 = act(bias + A @ W) in float64 and the per-element scale
+S = |bias| + |A| @ |W|, the sum of the magnitudes of every term of the dot product: an fp32-faithful kernel's error is a
+small multiple of 2^-22 S whatever the signs of the operands.
+
+Independent of libwmd and ops.*: index maps are applied with torch indexing, the work is cut into row blocks so that
+K = 9 x 2048 fits in memory, and it runs on whatever device the inputs live on.
+"""
+import torch
+
+PAD_ZERO, PAD_REFLECT, PAD_REPLICATE = 0, 1, 2
+ACT_NONE, ACT_ELU, ACT_LRELU, ACT_SIGMOID = 0, 1, 2, 3
+_f64 = torch.float64
+
+
+def _pad_coord(q, n, pad):
+    """(mapped q, inside) under pad mode `pad`, as pad_coord in csrc/common.cuh."""
+    if pad == PAD_REFLECT:
+        q = q.abs()
+        return torch.where(q >= n, 2 * (n - 1) - q, q), torch.ones_like(q, dtype=torch.bool)
+    if pad == PAD_REPLICATE:
+        return q.clamp(0, n - 1), torch.ones_like(q, dtype=torch.bool)
+    return q.clamp(0, n - 1), (q >= 0) & (q < n)
+
+
+def activate(y, act, act_param=0.0):
+    if act == ACT_ELU:
+        return torch.where(y > 0, y, torch.expm1(y.clamp(max=0)))
+    if act == ACT_LRELU:
+        return torch.where(y > 0, y, y * act_param)
+    if act == ACT_SIGMOID:
+        return torch.sigmoid(y)
+    return y
+
+
+def _take(x, rows, c):
+    """x[rows, :c] in float64 with rows < 0 reading zeros."""
+    ok = rows >= 0
+    v = x[rows.clamp(min=0), :c].to(_f64)
+    return v * ok.unsqueeze(-1)
+
+
+def gather_rows(m, x0, c0, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0, x1=None, c1=0, map1=None, gate=None,
+                pixels=None, rows0=None):
+    """The implicit im2col rows A[m] of output rows `m` (int64 tensor): (len(m), taps, c0 + c1) float64."""
+    dev = m.device
+    p = pixels.to(dev).long()[m] if pixels is not None else m
+    hw = h * w
+    nn, rem = p // hw, p % hw
+    y, x = rem // w, rem % w
+    if taps == 9:
+        dy = torch.arange(9, device=dev) // 3 - 1
+        dx = torch.arange(9, device=dev) % 3 - 1
+    else:
+        dy = dx = torch.zeros(1, dtype=torch.long, device=dev)
+    qy, oky = _pad_coord(y[:, None] + dy[None], h, pad)
+    qx, okx = _pad_coord(x[:, None] + dx[None], w, pad)
+    nn = nn[:, None].expand_as(qy)
+    ok = oky & okx
+    q = (nn * h + qy) * w + qx
+    if gate is not None:
+        ok = ok & (gate.to(dev).reshape(-1)[q] != 0)
+    if taps == 1 and map0 is None:
+        r0 = m[:, None].expand_as(q)
+        if rows0 is not None:
+            r0 = torch.where(r0 < rows0, r0, torch.full_like(r0, -1))
+    else:
+        hs, ws = h >> shift0, w >> shift0
+        qs = (nn * hs + (qy >> shift0)) * ws + (qx >> shift0)
+        r0 = map0.to(dev).reshape(-1).long()[qs] if map0 is not None else qs
+    r0 = torch.where(ok, r0, torch.full_like(r0, -1))
+    a = _take(x0, r0, c0)
+    if c1:
+        r1 = map1.to(dev).reshape(-1).long()[q] if map1 is not None else q
+        r1 = torch.where(ok, r1, torch.full_like(r1, -1))
+        a = torch.cat([a, _take(x1, r1, c1)], -1)
+    return a
+
+
+def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NONE, act_param=0.0, map0=None, shift0=0,
+             x1=None, c1=0, map1=None, gate=None, pixels=None, count=None, max_rows=None, rows0=None, block_elems=1 << 24):
+    """(y64, S) for rows [0, min(count, max_rows)): the arguments of ops.conv_rows, with a plain (cout, c0 + c1, k, k)
+    weight and an optional bias (cout,).  count: int or 1-element tensor (with pixels); rows0 (taps == 1, map0 None
+    only): rows x0 holds, rows past it read zeros (default: x0.shape[0])."""
+    dev = x0.device
+    cout = weight.shape[0]
+    rows = int(count) if pixels is not None else n * h * w
+    if max_rows is not None:
+        rows = min(rows, int(max_rows))
+    if rows0 is None and taps == 1 and map0 is None:
+        rows0 = x0.shape[0]
+    k = taps * (c0 + c1)
+    wk = weight.to(dev, _f64).permute(2, 3, 1, 0).reshape(k, cout)      # [tap][channel] x cout, the order of A
+    wa = wk.abs()
+    b = bias.to(dev, _f64) if bias is not None else torch.zeros(cout, dtype=_f64, device=dev)
+    y64 = torch.empty(rows, cout, dtype=_f64, device=dev)
+    s = torch.empty(rows, cout, dtype=_f64, device=dev)
+    step = max(1, block_elems // max(k, 1))
+    for r in range(0, rows, step):
+        m = torch.arange(r, min(rows, r + step), device=dev)
+        a = gather_rows(m, x0, c0, n, h, w, taps, pad, map0, shift0, x1, c1, map1, gate, pixels, rows0).reshape(len(m), k)
+        y64[r:r + len(m)] = a @ wk + b
+        s[r:r + len(m)] = a.abs() @ wa + b.abs()
+    return activate(y64, act, act_param), s
+
+
+def index_map(mask):
+    """(N, H, W) 0/1 mask -> int32 map: running row index over the batch in (n, y, x) order, -1 where inactive."""
+    flat = mask.reshape(-1) != 0
+    run = torch.cumsum(flat.to(torch.int64), 0) - 1
+    return torch.where(flat, run, torch.full_like(run, -1)).reshape(mask.shape).to(torch.int32)
+
+
+def pixel_list(mask):
+    """(N, H, W) 0/1 mask -> int32 linear indices (n*H + y)*W + x of the active pixels, in order."""
+    return torch.nonzero(mask.reshape(-1) != 0).reshape(-1).to(torch.int32)

@@ -1,0 +1,144 @@
+"""CPU: the fp64 conv-contract reference (tests/conv_ref.py) against torch's conv2d and the sparse-op oracle.
+
+The GPU contract tests (test_gpu_conv_contract.py) measure the kernels' error against this reference, so it has to be
+right on its own: every gather path it restates is checked here against an independent formulation, exactly (fp64
+sums of the same products in a different order: <= 1e-12 relative).
+"""
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+from oracle import sparse_ops as osp
+
+import conv_ref as cr
+
+TOL = 1e-12
+
+
+def rnd(*shape, seed=0, lo=-1.0, hi=1.0):
+    rs = np.random.RandomState(seed)
+    return torch.from_numpy(rs.uniform(lo, hi, size=shape).astype(np.float32))
+
+
+def rows_of(x):
+    """(N, C, H, W) -> pixel-major rows (N*H*W, C)."""
+    return x.permute(0, 2, 3, 1).reshape(-1, x.shape[1]).contiguous()
+
+
+def nchw_of(rows, n, h, w):
+    return rows.reshape(n, h, w, -1).permute(0, 3, 1, 2)
+
+
+def close(got, want):
+    return float((got - want).abs().max()) <= TOL * max(float(want.abs().max()), 1.0)
+
+
+_MODE = {cr.PAD_ZERO: "constant", cr.PAD_REFLECT: "reflect", cr.PAD_REPLICATE: "replicate"}
+
+
+@pytest.mark.parametrize("pad", [cr.PAD_ZERO, cr.PAD_REFLECT, cr.PAD_REPLICATE])
+@pytest.mark.parametrize("n,cin,cout,h,w", [(2, 5, 7, 6, 9), (1, 40, 33, 2, 5), (1, 3, 4, 5, 2)])
+def test_dense_3x3_matches_conv2d(pad, n, cin, cout, h, w):
+    x, wt, b = rnd(n, cin, h, w, seed=1), rnd(cout, cin, 3, 3, seed=2), rnd(cout, seed=3)
+    y64, s = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w, pad=pad)
+    xp = F.pad(x.double(), (1, 1, 1, 1), mode=_MODE[pad])
+    assert close(nchw_of(y64, n, h, w), F.conv2d(xp, wt.double(), b.double()))
+    assert close(nchw_of(s, n, h, w), F.conv2d(xp.abs(), wt.double().abs(), b.double().abs()))
+
+
+@pytest.mark.parametrize("act", [cr.ACT_ELU, cr.ACT_LRELU, cr.ACT_SIGMOID])
+def test_activations_and_1x1(act):
+    n, cin, cout, h, w = 2, 12, 9, 3, 7
+    x, wt, b = rnd(n, cin, h, w, seed=4), rnd(cout, cin, 1, 1, seed=5), rnd(cout, seed=6)
+    y64, _ = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w, taps=1, act=act, act_param=0.2)
+    z = F.conv2d(x.double(), wt.double(), b.double())
+    want = {cr.ACT_ELU: F.elu, cr.ACT_LRELU: lambda t: F.leaky_relu(t, 0.2), cr.ACT_SIGMOID: torch.sigmoid}[act](z)
+    assert close(nchw_of(y64, n, h, w), want)
+
+
+def test_bias_none_and_row_blocks():
+    n, cin, cout, h, w = 1, 7, 5, 9, 11
+    x, wt = rnd(n, cin, h, w, seed=7), rnd(cout, cin, 3, 3, seed=8)
+    y64, s = cr.conv_ref(rows_of(x), cin, wt, None, n, h, w, pad=cr.PAD_REFLECT, block_elems=100)   # two rows per block
+    xp = F.pad(x.double(), (1, 1, 1, 1), mode="reflect")
+    assert close(nchw_of(y64, n, h, w), F.conv2d(xp, wt.double()))
+    assert bool((s >= y64.abs()).all())
+
+
+@pytest.mark.parametrize("pad", [cr.PAD_ZERO, cr.PAD_REFLECT, cr.PAD_REPLICATE])
+@pytest.mark.parametrize("p_in,p_out", [(0.6, 0.5), (0.1, 0.9), (0.0, 0.5)])
+def test_sparse_3x3_matches_oracle(pad, p_in, p_out):
+    """Compact input rows through an index map, outputs at a pixel list (the reference's sparse_conv3x3)."""
+    cin, cout, h, w = 6, 5, 9, 13
+    rs = np.random.RandomState(9)
+    im = torch.from_numpy((rs.uniform(size=(1, 1, h, w)) < p_in).astype(np.float32))
+    om = torch.from_numpy((rs.uniform(size=(1, 1, h, w)) < p_out).astype(np.float32))
+    wt, b = rnd(cout, cin, 3, 3, seed=10), rnd(cout, seed=11)
+    m_in = int(im.sum())
+    xv = rnd(cin * m_in, seed=12)
+    idx, _ = osp.index_map(im)
+    want, _, _ = osp.conv3x3(wt.double(), b.double(), xv.double(), idx, om, padding=_MODE[pad], make_result=False)
+    rows = xv.reshape(cin, m_in).t().contiguous() if m_in else torch.zeros(1, cin)
+    pix = cr.pixel_list(om[0])
+    y64, _ = cr.conv_ref(rows, cin, wt, b, 1, h, w, pad=pad, map0=cr.index_map(im[0]), pixels=pix, count=len(pix))
+    assert y64.shape == (len(pix), cout)
+    assert close(y64.t().reshape(-1), want)
+
+
+def test_upsample_concat_gate_matches_oracle():
+    """Half-resolution compact source 0 (shift0 = 1), dense skip source 1, gate: sparse_upsample + sparse_conv3x3."""
+    c0, cs, cout, h, w = 5, 3, 4, 7, 9
+    rs = np.random.RandomState(13)
+    s0 = torch.from_numpy((rs.uniform(size=(1, 1, h, w)) < 0.3).astype(np.float32))
+    u = F.interpolate(s0, scale_factor=2, mode="nearest")
+    s2, s3, s4 = F.max_pool2d(s0, 5, 1, 2), F.max_pool2d(u, 5, 1, 2), F.max_pool2d(u, 3, 1, 1)
+    m2 = int(s2.sum())
+    xv, skip = rnd(c0 * m2, seed=14), rnd(1, cs, 2 * h, 2 * w, seed=15)
+    wt, b = rnd(cout, c0 + cs, 3, 3, seed=16), rnd(cout, seed=17)
+    map2, _ = osp.index_map(s2)
+    map3, _ = osp.index_map(s3)
+    up, _ = osp.upsample_concat(xv.double(), c0, map2, skip.double(), s3, make_result=False)
+    want, _, _ = osp.conv3x3(wt.double(), b.double(), up, map3, s4, padding="reflect", make_result=False)
+    pix = cr.pixel_list(s4[0])
+    y64, _ = cr.conv_ref(xv.reshape(c0, m2).t().contiguous(), c0, wt, b, 1, 2 * h, 2 * w, map0=cr.index_map(s2[0]),
+                         shift0=1, x1=rows_of(skip), c1=cs, gate=s3[0], pixels=pix, count=len(pix))
+    assert close(y64.t().reshape(-1), want)
+
+
+def test_compact_skip_map1_matches_dense_skip():
+    """x1 holding only the rows of listed pixels (map1) is the same convolution as the dense skip map."""
+    n, c0, c1, cout, h, w = 2, 4, 6, 5, 6, 8
+    rs = np.random.RandomState(18)
+    sel = torch.from_numpy((rs.uniform(size=(n, h, w)) < 0.5).astype(np.uint8))
+    x0, skip = rnd(n, c0, h, w, seed=19), rnd(n, c1, h, w, seed=20)
+    skip = skip * sel[:, None].float()                           # the dense map is zero where the compact one has no row
+    wt, b = rnd(cout, c0 + c1, 3, 3, seed=21), rnd(cout, seed=22)
+    dense, _ = cr.conv_ref(rows_of(x0), c0, wt, b, n, h, w, x1=rows_of(skip), c1=c1)
+    compact = rows_of(skip)[cr.pixel_list(sel).long()]
+    got, _ = cr.conv_ref(rows_of(x0), c0, wt, b, n, h, w, x1=compact, c1=c1, map1=cr.index_map(sel))
+    assert close(got, dense)
+
+
+def test_rows0_reads_zeros_past_the_source_rows():
+    """1x1 form over a source's own rows: output rows past rows0 see only source 1 (here: nothing but the bias)."""
+    n, cin, cout, h, w = 1, 8, 6, 5, 7
+    rows0 = 20
+    x, wt, b = rnd(n, cin, h, w, seed=23), rnd(cout, cin, 1, 1, seed=24), rnd(cout, seed=25)
+    y64, s = cr.conv_ref(rows_of(x)[:rows0], cin, wt, b, n, h, w, taps=1)
+    full = rows_of(F.conv2d(x.double(), wt.double(), b.double()))
+    assert close(y64[:rows0], full[:rows0])
+    assert torch.equal(y64[rows0:], b.double().expand(n * h * w - rows0, cout))
+    assert torch.equal(s[rows0:], b.double().abs().expand(n * h * w - rows0, cout))
+
+
+def test_count_and_max_rows():
+    n, cin, cout, h, w = 1, 3, 2, 4, 4
+    x, wt, b = rnd(n, cin, h, w, seed=26), rnd(cout, cin, 3, 3, seed=27), rnd(cout, seed=28)
+    pix = torch.arange(0, 16, 2, dtype=torch.int32)
+    y8, _ = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w, pixels=pix, count=8)
+    y5, _ = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w, pixels=pix, count=8, max_rows=5)
+    y0, _ = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w, pixels=pix, count=0)
+    assert y8.shape == (8, cout) and torch.equal(y5, y8[:5]) and y0.shape == (0, cout)
+    dense, _ = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w)
+    assert torch.equal(y8, dense[pix.long()])

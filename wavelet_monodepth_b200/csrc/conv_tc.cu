@@ -750,6 +750,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
         static_assert(kQuads % (TC_CONSUMERS * kUnroll) == 0, "quads of a tile divide evenly");
         const int tile_rows = min(TC_BM, rows - m0);
         const float ap = d.act_param;
+        // co is a multiple of 4: the quad load needs a 16-byte aligned bias (the ABI only asks for 4 bytes)
+        const bool bias16 = (reinterpret_cast<uintptr_t>(d.bias) & 15) == 0;
         for (int qbase = ctid; qbase < kQuads; qbase += TC_CONSUMERS * kUnroll) {
           float4 v[kUnroll], bq[kUnroll];
           int r[kUnroll], co[kUnroll];
@@ -762,7 +764,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
             live[q] = r[q] < tile_rows && co[q] < d.cout;
             bq[q] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (live[q] && d.bias) {
-              if (al_ok && co[q] + 3 < d.cout) {
+              if (bias16 && co[q] + 3 < d.cout) {
                 bq[q] = __ldg(reinterpret_cast<const float4*>(d.bias + co[q]));
               } else {
                 bq[q].x = __ldg(d.bias + co[q]);
@@ -856,11 +858,14 @@ __global__ void pack_weight_tc_kernel(const float* __restrict__ w, float* __rest
 // `splits` slabs laid out [slab][max_rows][ldy].  splits == 0 (balanced): only the remainder tiles have partial sums,
 // laid out [remainder tile][slab][256][BN]; the number of segments of a tile follows from the same unit arithmetic the
 // conv kernel used (grid = its CTA count); a remainder tile that one CTA covered entirely was finished there.
+// amax_out (nullable) is raised to max |y| of the rows written here, as the conv kernel does for the rows it writes.
 __global__ void tc_reduce_kernel(const float* __restrict__ partial, int splits, int grid, int BN, int nchunks,
                                  const float* __restrict__ bias, float* __restrict__ y, int ldy, int cout,
-                                 const int32_t* __restrict__ count, int max_rows, int act, float act_param) {
+                                 const int32_t* __restrict__ count, int total_px, int max_rows, int act, float act_param,
+                                 float* __restrict__ amax_out) {
   partial += kBalCounterBytes / 4;                   // the workspace starts with the balanced mode's arrival counters (kept zero)
-  const int rows = count ? min(*count, max_rows) : max_rows;
+  const int rows = min(count ? *count : total_px, max_rows);   // the conv kernel's row count
+  float out_max = 0.f;                               // max |y| this thread writes (-> amax_out)
   const long long slab_sz = static_cast<long long>(max_rows) * ldy;
   const int n_tiles = (cout + BN - 1) / BN;
   const long long tiles = static_cast<long long>((rows + TC_BM - 1) / TC_BM) * n_tiles;
@@ -900,14 +905,20 @@ __global__ void tc_reduce_kernel(const float* __restrict__ partial, int splits, 
       }
       v.x = activate(v.x, act, act_param); v.y = activate(v.y, act, act_param);
       v.z = activate(v.z, act, act_param); v.w = activate(v.w, act, act_param);
+      out_max = fmaxf(out_max, fabsf(v.x));
       if (co + 3 < cout) {
+        out_max = fmaxf(fmaxf(out_max, fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
         *reinterpret_cast<float4*>(y + o) = v;
       } else {
         y[o] = v.x;
-        if (co + 1 < cout) y[o + 1] = v.y;
-        if (co + 2 < cout) y[o + 2] = v.z;
+        if (co + 1 < cout) { y[o + 1] = v.y; out_max = fmaxf(out_max, fabsf(v.y)); }
+        if (co + 2 < cout) { y[o + 2] = v.z; out_max = fmaxf(out_max, fabsf(v.z)); }
       }
     }
+  }
+  if (amax_out) {                                    // as in the conv kernel: order independent, most warps skip the atomic
+    for (int o = 16; o > 0; o >>= 1) out_max = fmaxf(out_max, __shfl_xor_sync(0xffffffffu, out_max, o));
+    if ((threadIdx.x & 31) == 0 && out_max > __ldcg(amax_out)) atomicMax(reinterpret_cast<unsigned*>(amax_out), __float_as_uint(out_max));
   }
 }
 
@@ -1007,7 +1018,8 @@ static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStr
   const long long all_tiles = static_cast<long long>(ceil_div(d.max_rows, TC_BM)) * ceil_div(d.cout, BN);
   const long long red_grid = all_tiles < 8 * cap ? all_tiles : 8 * cap;
   tc_reduce_kernel<<<static_cast<int>(red_grid < 1 ? 1 : red_grid), 256, 0, stream>>>(partial, splits, grid, BN, nchunks, d.bias, d.y, d.ldy, d.cout,
-                                                              d.count, d.max_rows, d.act, d.act_param);
+                                                              d.count, d.N * d.H * d.W, d.max_rows,
+                                                              d.act, d.act_param, d.amax_out);
   return launched();
 }
 
