@@ -186,7 +186,8 @@ typedef struct wmd_conv_desc {
   int32_t precision;        /* tensor-core engine only.  0 = WMD_PREC_TF32X3: operands split into tf32 hi + lo.  1 = WMD_PREC_F16X3:
                                operands split into two fp16 pieces of x * 2^k (same 22 mantissa bits; k from amax0 / amax1, so
                                nothing overflows) - half the MMA instructions and twice their rate; needs amax0 (and amax1 when
-                               c1 > 0) and weights packed by wmd_pack_conv_weight_tc16_f32 */
+                               c1 > 0) and weights packed by wmd_pack_conv_weight_tc16_f32.  The Python KITTI decoders use
+                               F16X3 by default; launches without source maxima use TF32X3 */
   const float* amax0;       /* device scalars: max |x0|, max |x1| over the rows the launch can read (upper bounds are fine) */
   const float* amax1;
   float* amax_out;          /* device scalar, or NULL: atomically raised to max |y| of the rows written (zero it before the
@@ -218,8 +219,15 @@ int wmd_pack_conv_weight_tc16_f32(const float* w, void* packed, int Cout, int c0
 /* max |x| of `count` floats, atomically raised into *amax (device scalar, zero it first): for sources that no libwmd
  * kernel produced (channels_last feature maps used in place).  The layout moves below take an optional `amax` too. */
 int wmd_amax_f32(const float* x, long long count, float* amax, wmd_stream_t stream);
+/* max |x| over the rows r of x (rows x cols, contiguous) with mask[r] != 0: a channels_last map used in place whose
+ * consumer reads only the masked pixels */
+int wmd_amax_rows_masked_f32(const float* x, long long rows, int cols, const uint8_t* mask, float* amax, wmd_stream_t stream);
 int wmd_nchw_to_rows_amax_f32(const float* src, float* dst, int N, int C, long long HW, int ld, float* amax, wmd_stream_t stream);
-/* gated move: the maximum covers the 32-pixel groups that hold a marked pixel (a superset of the rows written) */
+/* plain move (every row) whose maximum covers only the pixels `mask` (N, HW) marks: the rows its consumer reads */
+int wmd_nchw_to_rows_masked_amax_f32(const float* src, float* dst, const uint8_t* mask, int N, int C, long long HW, int ld,
+                                     float* amax, wmd_stream_t stream);
+/* gated move: the maximum covers exactly the marked pixels (the rows written), as the list gather's covers the listed
+ * rows - the three moves of one map under one mask report the same maximum */
 int wmd_nchw_to_rows_gated_amax_f32(const float* src, float* dst, const uint8_t* gate, int N, int C, long long HW, int ld,
                                     float* amax, wmd_stream_t stream);
 int wmd_gather_rows_list_amax_f32(const float* src_nchw, float* rows, int ld, int C, const int32_t* pixels,

@@ -111,7 +111,10 @@ SIGNATURES = {
     "wmd_conv_tc16_weight_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "wmd_pack_conv_weight_tc16_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "wmd_amax_f32": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p]),
+    "wmd_amax_rows_masked_f32": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p]),
     "wmd_nchw_to_rows_amax_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_longlong, c_int, c_void_p, c_void_p]),
+    "wmd_nchw_to_rows_masked_amax_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_longlong, c_int, c_void_p,
+                                                 c_void_p]),
     "wmd_nchw_to_rows_gated_amax_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_longlong, c_int, c_void_p, c_void_p]),
     "wmd_gather_rows_list_amax_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                               c_int, c_void_p, c_void_p]),

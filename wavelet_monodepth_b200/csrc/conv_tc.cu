@@ -3,7 +3,7 @@
 // Same contract as conv_rows_kernel (conv.cu), different engine.  A persistent grid (at most one CTA per SM) walks
 // 128 x N output tiles (N = 128 / 64 / 32); a tile's reduction K = (c0 + c1) x taps runs in 32-channel chunks, the
 // taps of a channel chunk innermost (their source rows overlap: L2 hits).  384 threads, warp-specialised: one producer
-// warpgroup fills a TC_STAGES-deep ring of shared-memory stages, two consumer warpgroups multiply; consumer warpgroup h
+// warpgroup fills a ring of TcCfg::STAGES shared-memory stages, two consumer warpgroups multiply; consumer warpgroup h
 // owns tile rows h*64 .. h*64+63 (one wgmma M = 64 each, both share the chunk's weight tile).  Producer and consumers
 // step through the same work walk (TcWalk) and hand stages over with mbarriers (full[s]: stage filled, empty[s]: both
 // consumers are done with it), so the ring runs on across tile boundaries: the producer builds the next tile's tap table
@@ -49,11 +49,11 @@ constexpr int TC_THREADS = TC_PRODUCERS + TC_CONSUMERS;
 constexpr int TC_LAUNCH_REGS = (65536 / (TC_PRODUCERS + TC_CONSUMERS)) & ~7;
 constexpr int TC_PRODUCER_REGS = 40;
 constexpr int TC_CONSUMER_REGS = 232;
-constexpr int TC_STAGES = 4;                    // ring of chunk stages between the producer and the consumers
 constexpr int TC_A_LD = TC_BK + 4;              // raw A row pitch in floats (144 B: fragment reads hit 32 distinct banks)
 constexpr int TC_A_TILE = TC_BM * TC_A_LD * 4;  // 18 KB raw fp32
 constexpr int TC_TABLES = 2 * 9 * TC_BM * 4;    // one tap table: [source][tap][row]
-constexpr int TC_BARRIERS = 2 * TC_STAGES * 8;  // full[s], empty[s]
+constexpr int TC_SMEM_MAX = 227 * 1024;         // dynamic shared memory one CTA may use on an SM
+constexpr int TC_MAX_STAGES = 8;
 static_assert(TC_PRODUCERS * (TC_LAUNCH_REGS - TC_PRODUCER_REGS) >= TC_CONSUMERS * (TC_CONSUMER_REGS - TC_LAUNCH_REGS),
               "the consumers cannot take more registers than the producer gives back");
 
@@ -67,9 +67,17 @@ struct TcCfg {
   static constexpr int B_IMG = F16 ? B_TILE : 2 * B_TILE;
   static constexpr int ACC = BN / 2;                       // accumulator registers per thread (wgmma m64 x BN fragment)
   static constexpr int STAGE = B_IMG + TC_A_TILE;
-  static constexpr size_t SMEM = static_cast<size_t>(TC_STAGES) * STAGE + TC_TABLES + TC_BARRIERS + 1024;
+  // Ring depth: as many stages as fit beside the tap tables, the two barriers per stage and the 1 KB alignment slack, at
+  // most TC_MAX_STAGES.  The gather's latency is the same for every configuration while a smaller stage drains faster
+  // (the f16 form issues half the MMAs), so the small stages need more chunks in flight: 4 for tf32 N = 128, 6 for f16
+  // N = 128 and tf32 N = 64, 8 for the rest.
+  static constexpr int FIT = (TC_SMEM_MAX - TC_TABLES - 1024) / (STAGE + 2 * 8);
+  static constexpr int STAGES = FIT < TC_MAX_STAGES ? FIT : TC_MAX_STAGES;
+  static constexpr int BARRIERS = 2 * STAGES * 8;          // full[s], empty[s]
+  static constexpr size_t SMEM = static_cast<size_t>(STAGES) * STAGE + TC_TABLES + BARRIERS + 1024;
   static_assert(STAGE % 1024 == 0, "weight images must stay 1024-byte aligned");
-  static_assert(SMEM <= 227 * 1024, "one CTA must fit the shared memory of an SM");
+  static_assert(STAGES >= 2, "the ring needs two stages");
+  static_assert(SMEM <= TC_SMEM_MAX, "one CTA must fit the shared memory of an SM");
 };
 constexpr int kFlushChunks = 32;                // epoch length: K = 1024 per wgmma accumulation run
 static_assert(kFlushChunks % 2 == 0, "an epoch starts on register set 0");
@@ -359,6 +367,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   constexpr int B_IMG = Cfg::B_IMG;                         // bytes of one chunk's weight image
   constexpr int ACC = Cfg::ACC;
   constexpr int STAGE = Cfg::STAGE;
+  constexpr int STAGES = Cfg::STAGES;
   extern __shared__ unsigned char smem_dyn[];
   __shared__ int s_fixup;                                  // balanced mode: segments of the tile to reduce here (0 = not the last)
 
@@ -367,10 +376,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   // diverge inside a warp, and are not serialised
   const int warpgroup = __shfl_sync(0xffffffffu, tid / 128, 0);
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~static_cast<uintptr_t>(1023));
-  int32_t* tab0 = reinterpret_cast<int32_t*>(base + TC_STAGES * STAGE);   // [tap][row]: source row in x0, -1 = none
+  int32_t* tab0 = reinterpret_cast<int32_t*>(base + STAGES * STAGE);      // [tap][row]: source row in x0, -1 = none
   int32_t* tab1 = tab0 + 9 * TC_BM;                                        // ... in x1
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + TC_STAGES * STAGE + TC_TABLES);   // stage s holds its chunk
-  uint64_t* empty = full + TC_STAGES;                                                    // both consumers are done with s
+  uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * STAGE + TC_TABLES);      // stage s holds its chunk
+  uint64_t* empty = full + STAGES;                                                       // both consumers are done with s
 
   const long long HW = static_cast<long long>(d.H) * d.W;
   const int total_px = static_cast<int>(static_cast<long long>(d.N) * HW);
@@ -388,7 +397,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
 
   if (tid == 0) {
 #pragma unroll
-    for (int s = 0; s < TC_STAGES; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(full + s, TC_PRODUCERS + 1);               // every producer thread's copies + the weight image's bytes
       mbar_init(empty + s, TC_CONSUMERS / 32);             // one arrival per consumer warp
     }
@@ -405,7 +414,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     const long long rows_x0 = (aligned_rows && d.rows0 > 0) ? d.rows0 : static_cast<long long>(d.N) * Hs * Ws;
     const long long rows_x1 = static_cast<long long>(d.N) * HW;
     const unsigned char* wimg = reinterpret_cast<const unsigned char*>(wtc) + (F16 ? 128 : 0);   // f16 images follow a 128-byte header
-    uint32_t g = 0;                                        // chunks this CTA has issued: stage g % TC_STAGES, use g / TC_STAGES
+    uint32_t g = 0;                                        // chunks this CTA has issued: stage g % STAGES, use g / STAGES
     while (walk.next(it)) {
       const int m0 = static_cast<int>(it.tile / n_tiles) * TC_BM;
       const int nt = static_cast<int>(it.tile % n_tiles);
@@ -481,8 +490,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       const unsigned char* wtile = wimg + static_cast<long long>(nt) * nchunks * B_IMG;
 #pragma unroll 1
       for (int c = it.cb; c < it.ce; ++c, ++g) {
-        const int s = static_cast<int>(g % TC_STAGES);
-        if (g >= TC_STAGES) mbar_wait(empty + s, ((g / TC_STAGES) - 1) & 1);
+        const int s = static_cast<int>(g % STAGES);
+        if (g >= STAGES) mbar_wait(empty + s, ((g / STAGES) - 1) & 1);
         unsigned char* st = base + s * STAGE;
         if (tid == 0) {
           mbar_arrive_expect_tx(full + s, B_IMG);
@@ -551,11 +560,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
 #pragma unroll
   for (int j = 0; j < ACC; ++j) dacc[j] = 0.f;
 
-  // wait for stage gi % TC_STAGES to hold chunk gi, then read this thread's fragment elements into register set B
+  // wait for stage gi % STAGES to hold chunk gi, then read this thread's fragment elements into register set B
   auto load_frag = [&](auto B, uint32_t gi) {
     constexpr int b = decltype(B)::value;
-    const int s = static_cast<int>(gi % TC_STAGES);
-    mbar_wait(full + s, (gi / TC_STAGES) & 1);
+    const int s = static_cast<int>(gi % STAGES);
+    mbar_wait(full + s, (gi / STAGES) & 1);
     const float* sa = reinterpret_cast<const float*>(base + s * STAGE + B_IMG);
     if (F16) {
       // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
@@ -592,7 +601,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       for (int e = 0; e < 4; ++e) { reg_fence(fa[b][ks][e]); reg_fence(fb[b][ks][e]); }
   };
   auto release = [&](uint32_t gi) {                          // this warp is done with the stage of chunk gi
-    if (lane == 0) mbar_arrive(empty + gi % TC_STAGES);
+    if (lane == 0) mbar_arrive(empty + gi % STAGES);
   };
 
   uint32_t g = 0;                                          // chunks this CTA has consumed
@@ -613,7 +622,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     auto step = [&](auto B, int i) {
       constexpr int b = decltype(B)::value;
       const uint32_t gi = g + i;
-      const uint64_t b0 = wgmma_desc_sw128(smem_u32(base + (gi % TC_STAGES) * STAGE));
+      const uint64_t b0 = wgmma_desc_sw128(smem_u32(base + (gi % STAGES) * STAGE));
       const uint32_t keep = (i % kFlushChunks) != 0;
       wgmma_fence();
 #pragma unroll
@@ -931,6 +940,28 @@ __global__ void absmax_kernel(const float* __restrict__ x, long long count, floa
   if ((threadIdx.x & 31) == 0 && m > __ldcg(out)) atomicMax(reinterpret_cast<unsigned*>(out), __float_as_uint(m));
 }
 
+// max |x| over the rows r of x (rows x cols, contiguous) with mask[r] != 0.  A warp takes 32 rows at a time: one
+// coalesced read of their mask bytes, then the marked rows only, the lanes along each row (unmarked rows cost no traffic).
+__global__ void absmax_rows_masked_kernel(const float* __restrict__ x, long long rows, int cols,
+                                          const uint8_t* __restrict__ mask, float* __restrict__ out) {
+  float m = 0.f;
+  const int lane = threadIdx.x & 31;
+  const long long groups = (rows + 31) / 32;
+  const long long warps = static_cast<long long>(gridDim.x) * (blockDim.x >> 5);
+  for (long long gi = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; gi < groups; gi += warps) {
+    const long long r0 = gi * 32;
+    unsigned marked = __ballot_sync(0xffffffffu, r0 + lane < rows && mask[r0 + lane] != 0);
+    while (marked) {
+      const int b = __ffs(marked) - 1;
+      marked &= marked - 1;
+      const float* row = x + (r0 + b) * cols;
+      for (int c = lane; c < cols; c += 32) m = fmaxf(m, fabsf(__ldg(row + c)));
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0 && m > __ldcg(out)) atomicMax(reinterpret_cast<unsigned*>(out), __float_as_uint(m));
+}
+
 // header word 0 holds max |w| when this runs; it is replaced by 1 / s_w by the last block... no: by a second tiny kernel
 // (finish_header) so that every pack thread reads the same maximum.
 __global__ void pack_weight_tc16_kernel(const float* __restrict__ w, unsigned char* __restrict__ out, int Cout, int c0, int c1,
@@ -1093,6 +1124,16 @@ extern "C" int wmd_amax_f32(const float* x, long long count, float* amax, wmd_st
   WMD_REQUIRE(x && amax, WMD_ERR_ARG);
   if (count <= 0) return WMD_OK;
   absmax_kernel<<<stride_grid(count, 256, 16), 256, 0, as_stream(stream)>>>(x, count, amax);
+  return launched();
+}
+
+extern "C" int wmd_amax_rows_masked_f32(const float* x, long long rows, int cols, const uint8_t* mask, float* amax,
+                                        wmd_stream_t stream) {
+  using namespace wmd;
+  WMD_REQUIRE(x && mask && amax, WMD_ERR_ARG);
+  WMD_REQUIRE(rows >= 0 && cols > 0, WMD_ERR_SHAPE);
+  if (rows == 0) return WMD_OK;
+  absmax_rows_masked_kernel<<<stride_grid(rows, 256, 16), 256, 0, as_stream(stream)>>>(x, rows, cols, mask, amax);
   return launched();
 }
 

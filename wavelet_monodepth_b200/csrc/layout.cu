@@ -27,6 +27,8 @@ constexpr int kListLC = 128, kListLP = 32;       // gather_rows_list
 // map only under its upsample mask - sparse_upsample, KITTI/layers.py:500).  Reads are skipped per 32-pixel group
 // (one 128-byte request) with no marked pixel, writes per unmarked pixel (one 128-byte line), and a tile with no
 // marked pixel returns after one 128-byte look at the gate; unmarked rows of dst are left untouched.
+// Not GATED, `gate` may still be given: it then only restricts amax, every row is moved.  Either way amax covers exactly
+// the marked pixels, so a plain, a gated and a list-based move of the same map under the same mask report the same max.
 template <bool GATED, int kLC, int kLP>
 __global__ void __launch_bounds__(256) nchw_to_rows_kernel(const float* __restrict__ src, float* __restrict__ dst,
                                                            const uint8_t* __restrict__ gate, int C, long long HW,
@@ -38,7 +40,8 @@ __global__ void __launch_bounds__(256) nchw_to_rows_kernel(const float* __restri
   const long long p0 = static_cast<long long>(blockIdx.x) * kLP;
   const int c0 = blockIdx.y * kLC;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (GATED) {
+  const bool masked = gate != nullptr;
+  if (masked) {
     if (warp < kLP / 32) {
       const long long p = p0 + 32 * warp + lane;
       const bool on = p < HW && gate[static_cast<long long>(n) * HW + p] != 0;
@@ -46,6 +49,8 @@ __global__ void __launch_bounds__(256) nchw_to_rows_kernel(const float* __restri
       if (lane == 0) marked[warp] = m;
     }
     __syncthreads();
+  }
+  if (GATED) {
     unsigned any = 0u;
 #pragma unroll
     for (int j = 0; j < kLP / 32; ++j) any |= marked[j];
@@ -76,10 +81,10 @@ __global__ void __launch_bounds__(256) nchw_to_rows_kernel(const float* __restri
 #pragma unroll
     for (int j = 0; j < kLP / 32; ++j) {
       tile[warp + 8 * i][lane + 32 * j] = v[i][j];
-      vmax = fmaxf(vmax, fabsf(v[i][j]));
+      if (!masked || ((marked[j] >> lane) & 1u)) vmax = fmaxf(vmax, fabsf(v[i][j]));
     }
   }
-  if (amax) {                                    // max |x| of the map, for the consumers' fp16 operand scaling
+  if (amax) {                                    // max |x| (of the marked pixels), for the consumers' fp16 operand scaling
     for (int o = 16; o > 0; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
     if (lane == 0 && vmax > __ldcg(amax)) atomicMax(reinterpret_cast<unsigned*>(amax), __float_as_uint(vmax));   // most warps skip the atomic
   }
@@ -384,6 +389,18 @@ extern "C" int wmd_nchw_to_rows_amax_f32(const float* src, float* dst, int N, in
   dim3 grid(ceil_div(HW, kDenseLP), ceil_div(ld, kDenseLC), N);
   WMD_REQUIRE(grid.y <= 65535, WMD_ERR_SHAPE);
   nchw_to_rows_kernel<false, kDenseLC, kDenseLP><<<grid, 256, 0, as_stream(stream)>>>(src, dst, nullptr, C, HW, ld, amax);
+  return launched();
+}
+
+extern "C" int wmd_nchw_to_rows_masked_amax_f32(const float* src, float* dst, const uint8_t* mask, int N, int C,
+                                                long long HW, int ld, float* amax, wmd_stream_t stream) {
+  using namespace wmd;
+  WMD_REQUIRE(src && dst && mask && amax, WMD_ERR_ARG);
+  WMD_REQUIRE(N >= 0 && C > 0 && HW > 0 && ld >= C && N <= 65535, WMD_ERR_SHAPE);
+  if (N == 0) return WMD_OK;
+  dim3 grid(ceil_div(HW, kDenseLP), ceil_div(ld, kDenseLC), N);
+  WMD_REQUIRE(grid.y <= 65535, WMD_ERR_SHAPE);
+  nchw_to_rows_kernel<false, kDenseLC, kDenseLP><<<grid, 256, 0, as_stream(stream)>>>(src, dst, mask, C, HW, ld, amax);
   return launched();
 }
 

@@ -298,7 +298,8 @@ class _WaveDecoderBase(nn.Module):
         if n == 0:
             return self._empty_outputs(feats, sparse_levels, with_masks)
         # max |x| of every tensor a tensor-core conv reads (device scalars, zeroed here, raised by the producers): the
-        # fp16-pair operand form scales by a power of two chosen from them (ops.default_conv_precision)
+        # fp16-pair operand form (the default, ops.default_conv_precision) scales by a power of two chosen from them.  A
+        # skip map's maximum covers exactly the pixels upconv(i,1) reads, so every layout option picks the same scale.
         track = ops.default_conv_precision() == "f16x3"
         amax = torch.zeros(24, dtype=torch.float32, device=dev) if track else None
         slot = (lambda k: amax[k:k + 1]) if track else (lambda k: None)
@@ -344,10 +345,13 @@ class _WaveDecoderBase(nn.Module):
                 skip_amax = slot(i)
             else:
                 skip_amax = slot(i)
+                # a sparse level's maximum covers S3 only, the rows upconv(i,1) reads, whether the move is gated or not
+                max_mask = masks["S3"] if (sparse and track) else None
                 if side is not None:
-                    skip_rows, skip_done = ops.nchw_to_rows(skip, stream=side, gate=skip_gate, amax=skip_amax)
+                    skip_rows, skip_done = ops.nchw_to_rows(skip, stream=side, gate=skip_gate, amax=skip_amax,
+                                                            amax_mask=max_mask)
                 else:
-                    skip_rows = ops.nchw_to_rows(skip, gate=skip_gate, amax=skip_amax)
+                    skip_rows = ops.nchw_to_rows(skip, gate=skip_gate, amax=skip_amax, amax_mask=max_mask)
             if with_masks:
                 for name, key in (("lowres_mask", "S1"), ("upconv0_mask", "S2"), ("upsample_mask", "S3"),
                                   ("upconv1_mask", "S4"), ("wavelet_mask", "S5")):

@@ -174,7 +174,8 @@ def sparse_conv1x1(conv_layer, xvals, nonlin):
     ochn, ichn = wt.shape[:2]
     rows, m = _cm_to_rows(xvals, ichn)
     act, ap = _act_of(nonlin)
-    out = ops.conv_rows(rows, ichn, ops.pack_weight(wt), bias.detach(), ochn, 1, 1, max(m, 1), taps=1, act=act,
+    wp = ops.pack_weight(wt, precision="tf32x3")     # no source maxima here: tf32x3 operands, no fp16-pair image
+    out = ops.conv_rows(rows, ichn, wp, bias.detach(), ochn, 1, 1, max(m, 1), taps=1, act=act,
                         act_param=ap, max_rows=m)
     return _rows_to_cm(out, ochn, m).reshape(ochn, m), ochn, m * ichn * ochn + m * ochn
 
@@ -205,7 +206,8 @@ def sparse_conv3x3(conv_layer, xvals, xidxmap, mask, nonlin=nn.Identity(), paddi
     rows, _ = _cm_to_rows(xvals, ichn)
     _, pixels, offsets = ops.compact(_mask_u8(mask), want_idxmap=False)
     act, ap = _act_of(nonlin)
-    out = ops.conv_rows(rows, ichn, ops.pack_weight(conv.weight), conv.bias.detach(), ochn, 1, h, w, taps=9,
+    wp = ops.pack_weight(conv.weight, precision="tf32x3")     # no source maxima here: tf32x3 operands
+    out = ops.conv_rows(rows, ichn, wp, conv.bias.detach(), ochn, 1, h, w, taps=9,
                         pad=PAD_BY_NAME[padding], act=act, act_param=ap,
                         map0=xidxmap.reshape(1, h, w).to(torch.int32).contiguous(), pixels=pixels, count=offsets[1:])
     m_out = int(offsets[1])

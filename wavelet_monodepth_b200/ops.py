@@ -345,18 +345,29 @@ def rows_view(x):
 
 
 @_on_device
-def amax_rows(x, out):
+def amax_rows(x, out, mask=None):
     """out (1-element device tensor, pre-zeroed or holding a lower bound) = max(out, max |x|): for sources no libwmd kernel
-    produced (channels_last maps used in place)."""
+    produced (channels_last maps used in place).  mask: optional uint8 tensor of one byte per row of x (contiguous);
+    then only the marked rows count - the rows the consumer reads."""
     lib = _lib.load()
+    if mask is None:
+        with _prof('amax', lambda: dict(count=x.numel())):
+            rc = lib.wmd_amax_f32(_lib.ptr(x, _f32), x.numel(), _lib.ptr(out, _f32), _lib.stream_ptr())
+        _lib.check(rc, "wmd_amax_f32")
+        return out
+    mask = _dense(mask, _u8)
+    if not x.is_contiguous() or mask.numel() != x.shape[0]:
+        raise _lib.WmdError("amax_rows: contiguous rows and one mask byte per row (%d rows, %d mask bytes)"
+                            % (x.shape[0], mask.numel()))
     with _prof('amax', lambda: dict(count=x.numel())):
-        rc = lib.wmd_amax_f32(_lib.ptr(x, _f32), x.numel(), _lib.ptr(out, _f32), _lib.stream_ptr())
-    _lib.check(rc, "wmd_amax_f32")
+        rc = lib.wmd_amax_rows_masked_f32(_lib.ptr(x, _f32), x.shape[0], x.shape[1], _lib.ptr(mask), _lib.ptr(out, _f32),
+                                          _lib.stream_ptr())
+    _lib.check(rc, "wmd_amax_rows_masked_f32")
     return out
 
 
 @_on_device
-def nchw_to_rows(x, ld=None, stream=None, gate=None, amax=None):
+def nchw_to_rows(x, ld=None, stream=None, gate=None, amax=None, amax_mask=None):
     """(N,C,H,W) -> rows (N*H*W, ld) pixel-major.  Zero-copy when x is channels_last and C % 4 == 0.
 
     gate: optional uint8 (N,1,H,W) / (N,H,W) mask of the pixels whose rows will be read later: only those rows are
@@ -365,7 +376,10 @@ def nchw_to_rows(x, ld=None, stream=None, gate=None, amax=None):
     host memory (zero-copy over PCIe) - the host->device transfer of a skip map shrinks with the mask density.
     stream: optional side stream to run the transpose on (it first waits for the current stream, so `x` / `gate` may
     have been produced there).  Then returns (rows, event): the consumer stream must wait for `event` (None when no
-    kernel was needed).  The output is allocated on the current stream, whose later work is what reads it."""
+    kernel was needed).  The output is allocated on the current stream, whose later work is what reads it.
+    amax: optional 1-element device tensor raised to max |x| over the pixels the consumer reads: the gate's, else those
+    of amax_mask (same form as gate; it restricts only the maximum, every row is still produced), else the whole map.
+    So a sparse level's skip map reports one maximum whichever way it is moved (plain, gated, list gather, in place)."""
     lib = _lib.load()
     n, c, h, w = x.shape
     ld = pad4(c) if ld is None else ld
@@ -378,22 +392,30 @@ def nchw_to_rows(x, ld=None, stream=None, gate=None, amax=None):
         dev = gate.device
     else:
         dev = x.device
+    # the pixels the maximum covers: the gate's, else amax_mask's, else all
+    max_mask = gate if gate is not None else amax_mask
+    if max_mask is not None:
+        max_mask = _dense(max_mask, _u8)
+        if max_mask.numel() != n * h * w:
+            raise _lib.WmdError("nchw_to_rows: mask of %d pixels for a %dx%dx%d map" % (max_mask.numel(), n, h, w))
+        if gate is not None:
+            gate = max_mask
+    if not on_host:
         if x.dtype == _f32 and ld == c and x.permute(0, 2, 3, 1).is_contiguous() and x.data_ptr() % 16 == 0:
             rows = x.permute(0, 2, 3, 1).reshape(n * h * w, c)
             if amax is not None:
-                amax_rows(rows, amax)
+                amax_rows(rows, amax, mask=max_mask)
             return (rows, None) if stream is not None else rows
         x = _dense(x)
-    if gate is not None:
-        gate = _dense(gate, _u8)
-        if gate.numel() != n * h * w:
-            raise _lib.WmdError("nchw_to_rows: gate of %d pixels for a %dx%dx%d map" % (gate.numel(), n, h, w))
     rows = torch.empty((n * h * w, ld), dtype=_f32, device=dev)
 
     def launch():
         marked = _pm_count(gate)
         with _prof('nchw_to_rows', lambda: dict(n=n, c=c, hw=h * w, ld=ld, marked=marked, host=on_host)):
-            if gate is None and amax is not None:
+            if gate is None and amax is not None and max_mask is not None:
+                rc = lib.wmd_nchw_to_rows_masked_amax_f32(_lib.ptr(x), _lib.ptr(rows), _lib.ptr(max_mask), n, c, h * w, ld,
+                                                          _lib.ptr(amax, _f32), _lib.stream_ptr())
+            elif gate is None and amax is not None:
                 rc = lib.wmd_nchw_to_rows_amax_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.ptr(amax, _f32), _lib.stream_ptr())
             elif gate is None:
                 rc = lib.wmd_nchw_to_rows_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.stream_ptr())
@@ -529,21 +551,22 @@ TC_MIN_COUT = 32      # tensor-core tiles are 128 x {128, 64, 32}; below that th
 
 
 def default_conv_precision():
-    """Operand form of the tensor-core engine: env WMD_CONV_PRECISION = tf32x3 (default) | f16x3.
+    """Operand form of the tensor-core engine: env WMD_CONV_PRECISION = f16x3 (default) | tf32x3.
 
     Both are fp32-faithful error-compensated splits with fp32 accumulation (22 mantissa bits per operand, three MMAs per
-    product).  f16x3 feeds fp16 pairs of power-of-two scaled operands - half the MMA instructions - and needs the max |x|
-    of each source (tracked on the device by the producers, see conv_rows amax*); launches that lack it use tf32x3.
-    Opt-in: it costs the max tracking in every producer; its speed on H100 has not been measured."""
+    product).  f16x3 feeds fp16 pairs of power-of-two scaled operands - half the MMA instructions, two thirds of the
+    shared-memory stage - and needs the max |x| of each source (tracked on the device by the producers, see conv_rows
+    amax*); launches that lack it use tf32x3 (the functional kitti_layers API, the NYU decoder, split-K with an external
+    reduction).  The KITTI decoders' step is faster in f16x3 (DESIGN.md 7); tf32x3 stays selectable for A/B runs."""
     import os
-    return os.environ.get("WMD_CONV_PRECISION", "tf32x3")
+    return os.environ.get("WMD_CONV_PRECISION", "f16x3")
 
 
 def default_conv_kind():
     """Engine used when a caller does not ask for one: env WMD_CONV_IMPL = auto | simt | tc.
 
-    auto (default): wgmma 3xTF32 for cout >= 32 (every upconv / 1x1 head stage of the decoders), fp32 FMA
-    tiles below."""
+    auto (default): wgmma tensor cores (operand form: default_conv_precision) for cout >= 32 (every upconv / 1x1 head
+    stage of the decoders), fp32 FMA tiles below."""
     import os
     return os.environ.get("WMD_CONV_IMPL", "auto")
 
