@@ -344,6 +344,37 @@ int wmd_gather_rows_list_f32(const float* src_nchw, float* rows, int ld, int C, 
 size_t wmd_head_idwt_ws_bytes(int N, int H, int W);
 int wmd_head_idwt_f32(const wmd_head_idwt_desc* d, void* ws, size_t ws_bytes, wmd_stream_t stream);
 
+/* ---------------------------------------------------------------- convolution backward (training)
+ * The backward of one dense wmd_conv_desc layer (pixels, gate and map1 NULL) y = act(bias + A W), A the gathered rows:
+ *
+ * Activation backward: dz[r, o] = dy[r, o] * act'(y[r, o]) from the saved post-activation output y (ELU: y > 0 ? 1 : y + 1;
+ * LeakyReLU: y > 0 ? 1 : act_param; sigmoid: y (1 - y); none: 1), for rows r < rows and o < cout.  db (nullable) = sum over
+ * rows of dz, summed in a fixed order (per-block partials, then block order), so the bits do not depend on timing.
+ * amax_dz (nullable) is raised to max |dz|: the fp16-pair operand form of the data-gradient launch needs it.  ws (with db):
+ * wmd_act_bwd_ws_bytes() bytes whose first 4 KiB are zero before the first use; the kernel leaves them zero.  The same
+ * buffer may serve wmd_conv_wgrad_f32 launches on the same stream. */
+size_t wmd_act_bwd_ws_bytes(int rows, int cout);
+int wmd_act_bwd_f32(const float* y, int ldy, const float* dy, int lddy, int rows, int cout, int act, float act_param,
+                    float* dz, int lddz, float* db, float* amax_dz, void* ws, size_t ws_bytes, wmd_stream_t stream);
+/* Weight gradient: dw[o][c][ky][kx] = sum_p A(p)[tap][c] dz[p][o] (torch's (Cout, Cin, kh, kw) layout, tap = 3 ky + kx),
+ * A gathered exactly as the forward gathers it from the desc's sources, map0 / shift0, pad mode and taps; d->w, bias, y
+ * and act are not read.  Tensor cores (mma.sync tf32) with the operands split into tf32 hi + lo (3 MMAs per product)
+ * and each 32-pixel chunk's MMA sum added into fp32 sums with round-to-nearest adds.  taps = 1 needs shift0 = 0.  Layers with few output tiles split the
+ * pixel reduction across CTAs; the last CTA of a tile to arrive sums the partial slabs in slab order, so results are
+ * deterministic (no float atomics).  ws: wmd_conv_wgrad_ws_bytes(d) bytes (0: none needed) whose first 4 KiB (per-tile
+ * arrival counters) are zero before the first use; the kernel leaves them zero. */
+size_t wmd_conv_wgrad_ws_bytes(const wmd_conv_desc* d);
+int wmd_conv_wgrad_f32(const wmd_conv_desc* d, const float* dz, int lddz, float* dw, void* ws, size_t ws_bytes,
+                       wmd_stream_t stream);
+/* Fold of the data gradient.  g: rows (N (H+2) (W+2), ldg) of the gradient of the padded input, i.e. the forward contract
+ * run over the grid extended by one pixel on each side with the flipped, transposed weight, zero padding and a map0 that
+ * reads dz (-1 on the ring).  Each ring value is added into the pixel the pad mode maps it to (pad_coord; zero padding
+ * drops it).  Channels [0, c0) go to dx0 rows: per pixel, or with shift0 = 1 summed over the 2x2 children into the
+ * (N, H/2, W/2) low-resolution rows (the nearest x2 upsample's adjoint); columns c0..lddx0-1 are written as zeros.
+ * Channels [c0, c0 + c1) go to dx1_nchw (N, c1, H, W).  Fixed summation order. */
+int wmd_conv_dgrad_fold_f32(const float* g, int ldg, int N, int H, int W, int pad_mode, int c0, int shift0, float* dx0,
+                            int lddx0, int c1, float* dx1_nchw, wmd_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

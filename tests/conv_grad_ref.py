@@ -1,0 +1,38 @@
+"""fp64 adjoint of the gather-GEMM convolution contract: torch autograd through tests/conv_ref.py.
+
+For the linear part z = A W + b of a dense layer (A the implicit im2col rows gathered by conv_ref.gather_rows) and a given
+pre-activation gradient dz, returns the fp64 gradients of x0, x1 (rows), W and b, and the per-element scale S of each,
+the magnitude sum of the element's terms: the same adjoint applied to |x0|, |x1|, |W| and |dz| (for dW: |A|^T |dz|).
+Work is cut into row blocks; it runs on whatever device the inputs live on.
+"""
+import torch
+
+import conv_ref
+
+_f64 = torch.float64
+
+
+def _adjoint(x0, c0, x1, c1, weight, dz, n, h, w, taps, pad, shift0, block_rows):
+    x0 = x0.detach().to(_f64).requires_grad_(True)
+    x1 = x1.detach().to(_f64).requires_grad_(True) if x1 is not None else None
+    cout = weight.shape[0]
+    wk = weight.detach().to(_f64).requires_grad_(True)
+    wm = wk.permute(2, 3, 1, 0).reshape(-1, cout)
+    rows = n * h * w
+    for r in range(0, rows, block_rows):
+        m = torch.arange(r, min(rows, r + block_rows), device=dz.device)
+        a = conv_ref.gather_rows(m, x0, c0, n, h, w, taps, pad, shift0=shift0, x1=x1, c1=c1).reshape(len(m), -1)
+        (a @ wm).backward(dz[r:r + len(m)].to(_f64))
+    return x0.grad, (x1.grad if x1 is not None else None), wk.grad
+
+
+def conv_grads(x0, c0, x1, c1, weight, dz, n, h, w, taps=9, pad=conv_ref.PAD_REFLECT, shift0=0, block_elems=1 << 24):
+    """dict name -> (fp64 gradient, S) for 'x0', 'x1' (rows; None without x1), 'w' (weight layout) and 'b'."""
+    block_rows = max(1, block_elems // max(taps * (c0 + c1), 1))
+    g = _adjoint(x0, c0, x1, c1, weight, dz, n, h, w, taps, pad, shift0, block_rows)
+    s = _adjoint(x0.abs(), c0, x1.abs() if x1 is not None else None, c1, weight.abs(), dz.abs(), n, h, w, taps, pad,
+                 shift0, block_rows)
+    dz64 = dz.to(_f64)
+    out = {"x0": (g[0], s[0]), "w": (g[2], s[2]), "b": (dz64.sum(0), dz64.abs().sum(0))}
+    out["x1"] = (g[1], s[1]) if x1 is not None else None
+    return out

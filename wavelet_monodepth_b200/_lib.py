@@ -130,6 +130,13 @@ SIGNATURES = {
     "wmd_head_idwt_f32": (c_int, [POINTER(HeadIdwtDesc), c_void_p, c_size_t, c_void_p]),
     "wmd_head_gather_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_void_p,
                                     c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "wmd_act_bwd_ws_bytes": (c_size_t, [c_int, c_int]),
+    "wmd_act_bwd_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int, c_void_p,
+                                c_void_p, c_void_p, c_size_t, c_void_p]),
+    "wmd_conv_wgrad_ws_bytes": (c_size_t, [POINTER(ConvDesc)]),
+    "wmd_conv_wgrad_f32": (c_int, [POINTER(ConvDesc), c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "wmd_conv_dgrad_fold_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                                        c_void_p, c_void_p]),
 }
 
 _lib = None

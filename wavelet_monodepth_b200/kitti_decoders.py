@@ -16,7 +16,9 @@ What is different underneath (H100-native, DESIGN.md):
   * the sparse decoder is BATCHED (the reference asserts batch 1, :297): thresholds, masks and active
     lists are per sample, rows of all samples are concatenated, counts stay on the device, and the only
     host sync is one read of the counts at the end for ``total_ops``;
-  * training (grad enabled) uses the differentiable path: cuDNN convs + the native IDWT with its adjoint.
+  * training (grad enabled) of the dense decoder runs every convolution forward and backward on libwmd when fp32
+    convolutions are requested (torch.backends.cudnn.allow_tf32 False, train_native.py); with TF32 allowed it takes the
+    differentiable cuDNN path.  Both train through the native IDWT with its adjoint.
 """
 import os
 from collections import OrderedDict
@@ -25,7 +27,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import opcount, ops
+from . import opcount, ops, train_native
 from .opsfuture import OpsFuture
 from ._lib import ACT_ELU, ACT_LRELU, ACT_SIGMOID, PAD_REFLECT, WmdError
 from .kitti_layers import Conv1x1, Conv3x3, ConvBlock, upsample
@@ -501,7 +503,10 @@ class DepthWaveProgressiveDecoder(_WaveDecoderBase):
         _need_cuda(input_features)
         needs_grad = torch.is_grad_enabled() and (
             any(p.requires_grad for p in self.parameters()) or any(f.requires_grad for f in input_features))
-        if needs_grad:
+        if needs_grad and train_native.fp32_convs_requested():
+            # fp32 convolutions requested: forward and backward of every convolution on libwmd
+            self.outputs = train_native.kitti_forward(self, input_features)
+        elif needs_grad:
             self.outputs = self._autograd_forward(input_features)
         else:
             self.outputs, _ = self._native_forward(input_features, 0.0, sparse_levels=(), with_masks=False)

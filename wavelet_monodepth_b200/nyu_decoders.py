@@ -8,14 +8,16 @@ output-dict keys are the reference's.  The functional ``sparse_*`` ops of NYUv2/
 are the KITTI ones minus the 1x1 branch; they are re-exported from ``kitti_layers`` (whose
 ``sparse_conv3x3`` accepts this file's ``Conv3x3`` as well).
 
-As for KITTI: inference runs natively and batched in the pixel-major row layout; grad-enabled calls of
-``DecoderWave`` take the differentiable cuDNN + native-IDWT path (NYUv2/train.py:293-327 trains through it).
+As for KITTI: inference runs natively and batched in the pixel-major row layout; grad-enabled calls of a non-depthwise
+``DecoderWave`` (NYUv2/train.py:293-327 trains through it) run every convolution forward and backward on libwmd when fp32
+convolutions are requested (``torch.backends.cudnn.allow_tf32`` False, train_native.py), else the differentiable cuDNN +
+native-IDWT path.
 """
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import opcount, ops
+from . import opcount, ops, train_native
 from .opsfuture import OpsFuture
 from ._lib import ACT_LRELU, ACT_NONE, PAD_REFLECT, PAD_REPLICATE, PAD_ZERO, WmdError
 from .kitti_decoders import _PackCache, _need_cuda, _pm
@@ -255,8 +257,11 @@ class DecoderWave(_NyuWaveBase):
         _need_cuda(x_blocks)
         needs_grad = torch.is_grad_enabled() and (
             any(p.requires_grad for p in self.parameters()) or any(f.requires_grad for f in x_blocks))
-        if needs_grad or self._depthwise:
+        if self._depthwise or (needs_grad and not train_native.fp32_convs_requested()):
             return self._autograd_forward(x_blocks)
+        if needs_grad:
+            # fp32 convolutions requested: forward and backward of every convolution on libwmd
+            return train_native.nyu_forward(self, x_blocks)
         out, _ = self._native_forward(x_blocks, 0.0, sparse=False)
         return out
 

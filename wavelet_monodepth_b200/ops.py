@@ -66,6 +66,11 @@ class _Scratch:
             buf[:4096].zero_()
         return buf.view(_f32)
 
+    def bwd(self, device, nbytes):
+        """Workspace of the convolution backward kernels (bias-gradient partials, weight-gradient slabs).  Its first 4 KiB of
+        ticket / arrival counters must be zero before the first launch (the kernels leave them zeroed): zeroed once."""
+        return self._get(self._key("bwd", device), device, nbytes, 1 << 16, True)
+
     def compact(self, device, nbytes, slot=0):
         """slot: compactions that may run concurrently need different workspaces (side streams have their own key
         anyway; the slot also separates them when the caller serialises them on one stream)."""
@@ -665,6 +670,99 @@ def conv_rows(x0, c0, wpacked, bias, cout, n, h, w, taps=9, pad=PAD_REFLECT, act
             rc = lib.wmd_conv_rows_f32(ctypes.byref(d), _lib.stream_ptr())
     _lib.check(rc, "wmd_conv_rows_%sf32" % ("tc_" if wpacked.kind == "tc" else ""))
     return out
+
+
+# --------------------------------------------------------------------------- conv backward (training)
+@_on_device
+def act_backward(y, dy, cout, act, act_param=0.0, want_bias=True, amax=None):
+    """dz = dy * act'(y) on rows, from the saved post-activation output y (wmd_act_bwd_f32).
+
+    Returns (dz rows (R, pad4(cout)), db (cout,) summed over the rows in a fixed order, or None).  amax: optional
+    1-element device tensor raised to max |dz|."""
+    lib = _lib.load()
+    y, dy = _dense(y), _dense(dy)
+    rows = y.shape[0]
+    dev = y.device
+    dz = torch.empty((rows, pad4(cout)), dtype=_f32, device=dev)
+    db = torch.empty((cout,), dtype=_f32, device=dev) if want_bias else None
+    ws = _scratch.bwd(dev, lib.wmd_act_bwd_ws_bytes(rows, cout)) if want_bias else None
+    with _prof('act_bwd', lambda: dict(rows=rows, cout=cout, act=act)):
+        rc = lib.wmd_act_bwd_f32(_lib.ptr(y), y.shape[1], _lib.ptr(dy), dy.shape[1], rows, cout, act, float(act_param),
+                                 _lib.ptr(dz), dz.shape[1], _lib.ptr(db), _lib.ptr(amax, _f32), _lib.ptr(ws),
+                                 ws.numel() if ws is not None else 0, _lib.stream_ptr())
+    _lib.check(rc, "wmd_act_bwd_f32")
+    return dz, db
+
+
+def _bwd_desc(x0, c0, cout, n, h, w, taps, pad, map0, shift0, x1, c1):
+    d = _lib.ConvDesc()
+    d.N, d.H, d.W = n, h, w
+    d.x0, d.c0, d.ld0 = _lib.ptr(x0, _f32), c0, x0.shape[1]
+    d.map0, d.shift0 = _lib.ptr(map0, _i32), shift0
+    d.x1, d.c1, d.ld1 = (_lib.ptr(x1, _f32), c1, x1.shape[1]) if x1 is not None else (None, 0, 0)
+    d.cout, d.taps, d.pad_mode = cout, taps, pad
+    return d
+
+
+@_on_device
+def conv_wgrad(x0, c0, dz, cout, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0, x1=None, c1=0):
+    """Weight gradient (cout, c0 + c1, k, k) of a dense gather-GEMM convolution (wmd_conv_wgrad_f32): the sources are
+    the forward's (x0 / map0 / shift0 rows, dense x1 rows), dz the rows of the pre-activation gradient."""
+    lib = _lib.load()
+    dz = _dense(dz)
+    k = 3 if taps == 9 else 1
+    dw = torch.empty((cout, c0 + c1, k, k), dtype=_f32, device=dz.device)
+    d = _bwd_desc(x0, c0, cout, n, h, w, taps, pad, map0, shift0, x1, c1)
+    nbytes = lib.wmd_conv_wgrad_ws_bytes(ctypes.byref(d))
+    ws = _scratch.bwd(dz.device, nbytes) if nbytes else None
+    with _prof('conv_wgrad', lambda: dict(n=n, h=h, w=w, taps=taps, c0=c0, c1=c1, cout=cout)):
+        rc = lib.wmd_conv_wgrad_f32(ctypes.byref(d), _lib.ptr(dz), dz.shape[1], _lib.ptr(dw), _lib.ptr(ws),
+                                    ws.numel() if ws is not None else 0, _lib.stream_ptr())
+    _lib.check(rc, "wmd_conv_wgrad_f32")
+    return dw
+
+
+_RING_MAPS = {}
+
+
+def ring_map(n, h, w, device):
+    """int32 (N, H+2, W+2) map of the grid extended by a one-pixel ring: the row of pixel (y-1, x-1), -1 on the ring."""
+    key = (n, h, w, str(device))
+    m = _RING_MAPS.get(key)
+    if m is None:
+        idx = torch.arange(n * h * w, dtype=_i32, device=device).reshape(n, h, w)
+        m = torch.full((n, h + 2, w + 2), -1, dtype=_i32, device=device)
+        m[:, 1:h + 1, 1:w + 1] = idx
+        _RING_MAPS[key] = m
+    return m
+
+
+@_on_device
+def conv_dgrad(dz, cout, wt_packed, c0, n, h, w, taps=9, pad=PAD_REFLECT, shift0=0, c1=0, amax=None, want_x1=True):
+    """Data gradient of a dense gather-GEMM convolution -> (dx0 rows (N*(H>>shift0)*(W>>shift0), pad4(c0)), dx1 NCHW or None).
+
+    wt_packed: pack_weight of the flipped, transposed weight W.transpose(0, 1).flip(2, 3).  1x1 layers are one forward
+    launch on dz; 3x3 layers run the forward contract over the grid extended by one pixel on each side under zero padding
+    (map0 = ring_map into the dz rows), then wmd_conv_dgrad_fold_f32 folds the ring by the pad mode, sums the 2x2 children of
+    a shift0 = 1 source and writes the source-1 columns to NCHW.  amax: max |dz| (device scalar) for the fp16-pair form."""
+    lib = _lib.load()
+    cin = c0 + c1
+    if taps == 1:
+        if shift0 or c1:
+            raise _lib.WmdError("conv_dgrad: 1x1 layers read one dense source")
+        dx = conv_rows(dz, cout, wt_packed, None, cin, n, h, w, taps=1, amax0=amax)
+        dx[:, cin:] = 0                   # pad columns: the rows are a gradient autograd may add to another one whole
+        return dx, None
+    g = conv_rows(dz, cout, wt_packed, None, cin, n, h + 2, w + 2, taps=9, pad=PAD_ZERO, map0=ring_map(n, h, w, dz.device),
+                  amax0=amax)
+    dx0 = torch.empty((n * (h >> shift0) * (w >> shift0), pad4(c0)), dtype=_f32, device=dz.device)
+    c1w = c1 if want_x1 else 0
+    dx1 = torch.empty((n, c1, h, w), dtype=_f32, device=dz.device) if c1w else None
+    with _prof('conv_dgrad_fold', lambda: dict(n=n, h=h, w=w, c0=c0, c1=c1w, shift0=shift0)):
+        rc = lib.wmd_conv_dgrad_fold_f32(_lib.ptr(g), g.shape[1], n, h, w, pad, c0, shift0, _lib.ptr(dx0), dx0.shape[1], c1w,
+                                         _lib.ptr(dx1), _lib.stream_ptr())
+    _lib.check(rc, "wmd_conv_dgrad_fold_f32")
+    return dx0, dx1
 
 
 def head_mlp_supported(c, n1):
