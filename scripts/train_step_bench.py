@@ -3,7 +3,9 @@
     python scripts/train_step_bench.py [--steps 10] [--warmup 3] [--runs 3] [--out DIR]
 
 Workloads: KITTI ResNet18 640x192 with 12 frames (the KITTI options' default batch), KITTI ResNet50 1024x320 with 8
-frames, NYU DenseNet161 640x480 with 8 frames.  Modes: native (libwmd forward and backward, selected because
+frames, NYU DenseNet161 640x480 with 8 frames, and the 224-pixel NYU decoder (DecoderWave224) on DenseNet161 and
+MobileNetV2-light features with 8 frames (NYUv2/train.py --bs).  The 224 decoder's loss leaves out ("disp", 1), its
+floor division, which torch cannot differentiate.  Modes: native (libwmd forward and backward, selected because
 allow_tf32 is False), cudnn_fp32 (the decoder's cuDNN path with allow_tf32 False) and cudnn_tf32 (context only: it
 computes a less precise result).  The three modes run alternated, --runs times each, in one process.  Also reported:
 per-kernel times of the backward kernels (torch.profiler, a separate step), the largest gradient difference between
@@ -25,6 +27,8 @@ WORKLOADS = {
     "kitti_r18_640x192_b12": ("kitti", [64, 64, 128, 256, 512], 12, 192, 640),
     "kitti_r50_1024x320_b8": ("kitti", [64, 256, 512, 1024, 2048], 8, 320, 1024),
     "nyu_d161_640x480_b8": ("nyu", [96, 96, 192, 384, 2208], 8, 480, 640),
+    "nyu224_d161_b8": ("nyu224", [96, 96, 192, 384, 2208], 8, 224, 224),
+    "nyu224_mnv2light_b8": ("nyu224", [32, 24, 32, 64, 160], 8, 224, 224),
 }
 MODES = ("native", "cudnn_fp32", "cudnn_tf32")
 KERNELS = ("act_bwd_kernel", "conv_wgrad_kernel", "fold_src0_kernel", "fold_src1_kernel")
@@ -41,7 +45,7 @@ def build(kind, ch, n, h, w):
         mod = kd.DepthWaveProgressiveDecoder(np.array(ch))
         shapes = synth.kitti_feature_shapes(n, h, w, ch)
     else:
-        mod = nd.DecoderWave(enc_features=ch, decoder_width=0.5)
+        mod = (nd.DecoderWave224 if kind == "nyu224" else nd.DecoderWave)(enc_features=ch, decoder_width=0.5)
         shapes = synth.nyu_feature_shapes(n, h, w, ch)
     synth.load_random(mod, seed=1)
     feats = [f.cuda().requires_grad_(True) for f in synth.blocky_features(shapes, seed=2)]
@@ -54,7 +58,7 @@ def step(mod, feats, mode):
     for f in feats:
         f.grad = None
     out = mod._autograd_forward(feats) if mode == "cudnn_fp32" else mod(feats)
-    disp = [v for k, v in out.items() if k[0] == "disp"]
+    disp = [v for k, v in out.items() if k[0] == "disp" and not (k[1] == 1 and isinstance(mod, nd.DecoderWave224))]
     sum(d.mean() for d in disp).backward()
 
 

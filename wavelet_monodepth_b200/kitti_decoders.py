@@ -205,7 +205,8 @@ class _WaveDecoderBase(nn.Module):
 
     def _upconv(self, i, j):
         conv = self.convs[("upconv", i, j)].conv.conv
-        c1 = int(self.num_ch_enc[i - 1]) if j == 1 else 0          # upconv(i,1) reads the skip map as gather source 1
+        # upconv(i,1) reads the skip map as gather source 1; without skips it reads only the upsampled upconv(i,0)
+        c1 = int(self.num_ch_enc[i - 1]) if (j == 1 and self.use_skips) else 0
         kind = ops.default_conv_kind()
         return self._packs.get(("upconv", i, j, kind), [conv.weight], lambda: ops.pack_weight(conv.weight, c1)), conv.bias.detach()
 
@@ -320,9 +321,10 @@ class _WaveDecoderBase(nn.Module):
         for i in range(4, 0, -1):
             c = int(self.num_ch_dec[i])
             sparse = i in sparse_levels
-            skip = feats[i - 1]
-            cs = skip.shape[1]
-            if tuple(skip.shape[2:]) != (2 * h, 2 * w):
+            # without skips the maps feats[0..3] are never read: no layout move, gate, compaction or maximum for them
+            skip = feats[i - 1] if self.use_skips else None
+            cs = skip.shape[1] if self.use_skips else 0
+            if self.use_skips and tuple(skip.shape[2:]) != (2 * h, 2 * w):
                 raise WmdError("skip feature %d has shape %s, expected spatial %s" % (i - 1, tuple(skip.shape), (2 * h, 2 * w)))
             masks = None
             if with_masks:
@@ -331,29 +333,29 @@ class _WaveDecoderBase(nn.Module):
                 else:
                     thresh = next_thresh if next_thresh is not None else ops.range_thresh(yl, thresh_ratio)
                     masks = ops.level_masks(yh, thresh)
-            skip_gate = masks["S3"] if (sparse and self.gated_layout) else None
-            skip_done = None
-            map3 = None
-            if sparse and self.compact_skip and (i in self.compact_skip_levels or not skip.is_cuda) and \
-                    ops.rows_view(skip) is None:                         # channels_last maps are used in place instead
-                # S3's compaction and the gather of exactly its rows, on a side stream next to gate_map / compact(S2) / upconv(i,0)
-                s3 = _side_stream(dev, 3) if self.overlap_compaction else None
-                if s3 is not None:
-                    (map3, pix3, off3), _ = ops.compact(masks["S3"], stream=s3, ws_slot=3)
-                    skip_rows, skip_done = ops.gather_rows_list(skip, pix3, off3[n:], stream=s3, amax=slot(i))
+            skip_rows = skip_amax = skip_done = map3 = None
+            if self.use_skips:
+                skip_gate = masks["S3"] if (sparse and self.gated_layout) else None
+                if sparse and self.compact_skip and (i in self.compact_skip_levels or not skip.is_cuda) and \
+                        ops.rows_view(skip) is None:                         # channels_last maps are used in place instead
+                    # S3's compaction and the gather of exactly its rows, on a side stream next to gate_map / compact(S2) / upconv(i,0)
+                    s3 = _side_stream(dev, 3) if self.overlap_compaction else None
+                    if s3 is not None:
+                        (map3, pix3, off3), _ = ops.compact(masks["S3"], stream=s3, ws_slot=3)
+                        skip_rows, skip_done = ops.gather_rows_list(skip, pix3, off3[n:], stream=s3, amax=slot(i))
+                    else:
+                        map3, pix3, off3 = ops.compact(masks["S3"], ws_slot=3)
+                        skip_rows = ops.gather_rows_list(skip, pix3, off3[n:], amax=slot(i))
+                    skip_amax = slot(i)
                 else:
-                    map3, pix3, off3 = ops.compact(masks["S3"], ws_slot=3)
-                    skip_rows = ops.gather_rows_list(skip, pix3, off3[n:], amax=slot(i))
-                skip_amax = slot(i)
-            else:
-                skip_amax = slot(i)
-                # a sparse level's maximum covers S3 only, the rows upconv(i,1) reads, whether the move is gated or not
-                max_mask = masks["S3"] if (sparse and track) else None
-                if side is not None:
-                    skip_rows, skip_done = ops.nchw_to_rows(skip, stream=side, gate=skip_gate, amax=skip_amax,
-                                                            amax_mask=max_mask)
-                else:
-                    skip_rows = ops.nchw_to_rows(skip, gate=skip_gate, amax=skip_amax, amax_mask=max_mask)
+                    skip_amax = slot(i)
+                    # a sparse level's maximum covers S3 only, the rows upconv(i,1) reads, whether the move is gated or not
+                    max_mask = masks["S3"] if (sparse and track) else None
+                    if side is not None:
+                        skip_rows, skip_done = ops.nchw_to_rows(skip, stream=side, gate=skip_gate, amax=skip_amax,
+                                                                amax_mask=max_mask)
+                    else:
+                        skip_rows = ops.nchw_to_rows(skip, gate=skip_gate, amax=skip_amax, amax_mask=max_mask)
             if with_masks:
                 for name, key in (("lowres_mask", "S1"), ("upconv0_mask", "S2"), ("upsample_mask", "S3"),
                                   ("upconv1_mask", "S4"), ("wavelet_mask", "S5")):

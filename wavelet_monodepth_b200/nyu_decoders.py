@@ -1,17 +1,18 @@
 """NYUv2 DenseDepth-style wavelet decoders with the reference's contract, on libwmd.
 
 Mirrors NYUv2/networks/layers.py:11-79 (``Conv3x3``, ``upsample``, ``UpSampleBlock``, ``depthwise``,
-``pointwise``) and NYUv2/networks/decoders/densedepth_decoder.py:92-148 (``DecoderWave``), :224-409
-(``SparseDecoderWave``).  State-dict names (``conv2.conv.weight``, ``up1.convA.conv.weight``,
+``pointwise``) and NYUv2/networks/decoders/densedepth_decoder.py:92-148 (``DecoderWave``), :151-221
+(``DecoderWave224``), :224-409 (``SparseDecoderWave``).  The three share one native level engine, driven by a per-class
+level table (``_NyuWaveBase._LEVELS``).  State-dict names (``conv2.conv.weight``, ``up1.convA.conv.weight``,
 ``wave1_ll.conv.weight`` ..., ``iwt.*`` / ``iwt_LL.*`` buffers), constructor and forward signatures and the
 output-dict keys are the reference's.  The functional ``sparse_*`` ops of NYUv2/networks/layers.py:82-223
 are the KITTI ones minus the 1x1 branch; they are re-exported from ``kitti_layers`` (whose
 ``sparse_conv3x3`` accepts this file's ``Conv3x3`` as well).
 
 As for KITTI: inference runs natively and batched in the pixel-major row layout; grad-enabled calls of a non-depthwise
-``DecoderWave`` (NYUv2/train.py:293-327 trains through it) run every convolution forward and backward on libwmd when fp32
-convolutions are requested (``torch.backends.cudnn.allow_tf32`` False, train_native.py), else the differentiable cuDNN +
-native-IDWT path.
+``DecoderWave`` or ``DecoderWave224`` (NYUv2/train.py:293-327 trains through them) run every convolution forward and
+backward on libwmd when fp32 convolutions are requested (``torch.backends.cudnn.allow_tf32`` False, train_native.py),
+else the differentiable cuDNN + native-IDWT path.
 """
 import torch
 import torch.nn as nn
@@ -83,6 +84,14 @@ class UpSampleBlock(nn.Sequential):
 
 
 class _NyuWaveBase(nn.Module):
+    # Level table of the native engine and of the native training forward (train_native.nyu_forward).
+    # _LL_HEAD: (LL scale, k) - LL = scale * wave1_ll(up1 output), and ("disp", k) is the raw LL head (k None: no such
+    # output).  _LEVELS: one (j, s, disp) per IDWT level, coarse to fine: the level reads up<j>'s output (up1 for j = 1,
+    # shared with the LL head), its details are 2**s * wave<j>, and ("disp", s) is "div" ll / 2**s, "floor" ll // 2 or
+    # "last" ll itself (with depth_epilogue's ("depth", s)).  Sparse decoders run the levels j > 1 on active lists.
+    _LL_HEAD = (2 ** 3, 3)                                        # densedepth_decoder.py:122-123
+    _LEVELS = ((1, 2, "div"), (2, 1, "div"), (3, 0, "last"))     # densedepth_decoder.py:124-146
+
     def _build(self, enc_features, decoder_width, dw_waveconv=False, dw_upconv=False):
         features = int(enc_features[-1] * decoder_width)
         self.features = features
@@ -96,12 +105,11 @@ class _NyuWaveBase(nn.Module):
                                  padding=padding, is_depthwise=dw_upconv)
         self.wave1_ll = Conv3x3(features // 2, 1, padding="replicate")
         self.wave1 = Conv3x3(features // 2, 3, padding=wave_pad, is_depthwise=dw_waveconv)
-        self.up2 = UpSampleBlock(skip_input=features // 2 + enc_features[-3], output_features=features // 4,
-                                 padding=padding, is_depthwise=dw_upconv)
-        self.wave2 = Conv3x3(features // 4, 3, padding=wave_pad, is_depthwise=dw_waveconv)
-        self.up3 = UpSampleBlock(skip_input=features // 4 + enc_features[-4], output_features=features // 8,
-                                 padding=padding, is_depthwise=dw_upconv)
-        self.wave3 = Conv3x3(features // 8, 3, padding=wave_pad, is_depthwise=dw_waveconv)
+        for j in range(2, len(self._LEVELS) + 1):                 # up2, wave2, up3, wave3 [, up4, wave4]
+            setattr(self, "up%d" % j, UpSampleBlock(skip_input=features // 2 ** (j - 1) + enc_features[-1 - j],
+                                                    output_features=features // 2 ** j, padding=padding,
+                                                    is_depthwise=dw_upconv))
+            setattr(self, "wave%d" % j, Conv3x3(features // 2 ** j, 3, padding=wave_pad, is_depthwise=dw_waveconv))
         self._depthwise = bool(dw_waveconv or dw_upconv)
         # optional consumer epilogue of ("disp", 0), off by default: (div, lo, hi) adds ("depth", 0) =
         # clamp(("disp", 0) / div, lo, hi) - NYUv2/utils.py:219,229 uses (100, 0.4, 10) - fused into the last IDWT
@@ -128,9 +136,23 @@ class _NyuWaveBase(nn.Module):
         conv = layer.conv
         return self._packs.get(("head", name), [conv.weight], lambda: ops.pack_head_weight(conv.weight)), conv.bias.detach()
 
+    def _forward(self, x_blocks):
+        """Dense decoders: the cuDNN module graph for depthwise variants and for training with TF32 allowed, the native
+        training forward for training with fp32 convolutions, the native engine otherwise (no_grad / inference)."""
+        _need_cuda(x_blocks)
+        needs_grad = torch.is_grad_enabled() and (
+            any(p.requires_grad for p in self.parameters()) or any(f.requires_grad for f in x_blocks))
+        if self._depthwise or (needs_grad and not train_native.fp32_convs_requested()):
+            return self._autograd_forward(x_blocks)
+        if needs_grad:
+            # fp32 convolutions requested: forward and backward of every convolution on libwmd
+            return train_native.nyu_forward(self, x_blocks)
+        out, _ = self._native_forward(x_blocks, 0.0, sparse=False)
+        return out
+
     @torch.no_grad()
     def _native_forward(self, blocks, thresh_ratio, sparse):
-        """conv2/up1/wave1 dense, then the up2/wave2 and up3/wave3 levels dense or on active lists.
+        """conv2/up1 and the first level dense, then the levels of _LEVELS dense or on active lists.
 
         Returns (outputs, counts): counts = int32 device tensor (2, 2, N+1), row offsets of S4 / S5 of the two sparse
         blocks (None on the dense path)."""
@@ -158,65 +180,72 @@ class _NyuWaveBase(nn.Module):
         d1 = ops.conv_rows(d0, f, wp, b, f // 2, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_LRELU, act_param=0.2,
                            shift0=1, x1=ops.nchw_to_rows(skip), c1=skip.shape[1])
         h, w = 2 * h, 2 * w
+        ll_scale, ll_disp = self._LL_HEAD
         wl, bl = self._head("wave1_ll", self.wave1_ll)
         raw = ops.head_conv3x3(d1, f // 2, 0, wl, bl, n, h, w, 1, scale=1.0, act=ACT_NONE, pad=PAD_REPLICATE)
-        ll = raw * float(2 ** 3)             # exact power-of-two scaling of a (N,1,H/16,W/16) map
-        out[("disp", 3)] = raw               # == ll / 2**3 (densedepth_decoder.py:123)
-        wh, bh = self._head("wave1", self.wave1)
-        hcoef = ops.head_conv3x3(d1, f // 2, 0, wh, bh, n, h, w, 3, scale=float(2 ** 2), act=ACT_NONE, pad=PAD_ZERO)
-        if sparse:
-            # the reference builds this one as ones_like(h[:, 0]) with h already (N,1,3,H,W): a 3-channel map
-            # (densedepth_decoder.py:301-303); kept as is
-            out[("wavelet_mask", 2)] = torch.ones((n, 3, h, w), dtype=torch.float32, device=xb.device)
-        out[("wavelets", 2, "LL")] = ll
-        for k, band in enumerate(("LH", "HL", "HH")):
-            out[("wavelets", 2, band)] = hcoef[:, k:k + 1]
-        ll, disp = ops.idwt_haar(ll, hcoef.unsqueeze(1), disp_scale=1.0 / 2 ** 2, clamp01=False)
-        out[("disp", 2)] = disp
+        ll = raw * float(ll_scale)           # exact power-of-two scaling of a (N,1,H/16,W/16) map
+        if ll_disp is not None:
+            out[("disp", ll_disp)] = raw     # == ll / ll_scale (densedepth_decoder.py:123)
 
-        x_rows, x_c, prev_map = d1, f // 2, None
-        for s, (up, wave, scale) in enumerate(((self.up2, self.wave2, 2.0), (self.up3, self.wave3, 1.0))):
-            name = "up%d" % (s + 2)
-            skip = blocks[-3 - s]
-            cs = skip.shape[1]
-            cout = up.convA.conv.weight.shape[0]
-            wp, b = self._gemm(name, up.convA, cs)
-            wh, bh = self._head("wave%d" % (s + 2), wave)
-            if tuple(skip.shape[2:]) != (2 * h, 2 * w):
-                raise WmdError("skip block has shape %s, expected spatial %s" % (tuple(skip.shape), (2 * h, 2 * w)))
-            if sparse:
-                thresh = ops.range_thresh(ll, thresh_ratio)
-                masks = ops.level_masks(hcoef, thresh, want=("S2", "S3", "S4", "S5"))
-                gmap = ops.gate_map(masks["S2"], prev_map)
-                map4, pix4, off4 = ops.compact(masks["S4"])
-                _, pix5, off5 = ops.compact(masks["S5"], want_idxmap=False)
-                counts.append((off4, off5))
-                out[("wavelet_mask", 1 - s)] = masks["S5"].to(torch.float32)
-                xa = ops.conv_rows(x_rows, x_c, wp, b, cout, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_LRELU,
-                                   act_param=0.2, map0=gmap, shift0=1, x1=ops.nchw_to_rows(skip), c1=cs,
-                                   gate=masks["S3"], pixels=pix4, count=off4[n:],
-                                   m_in0=_pm(lambda: (gmap >= 0).sum()), m_in1=_pm(lambda: masks["S3"].sum()))
-                hcoef = ops.head_conv3x3(xa, cout, 0, wh, bh, n, 2 * h, 2 * w, 3, scale=scale, act=ACT_NONE,
-                                         pad=PAD_ZERO, idxmap=map4, pixels=pix5, count=off5[n:])
-                prev_map = map4
+        x_rows, x_c, prev_map, hcoef = d1, f // 2, None, None
+        for j, s, disp_form in self._LEVELS:
+            scale = float(2 ** s)
+            wave = getattr(self, "wave%d" % j)
+            if j == 1:
+                # the first level's details come from up1's output, like the LL head
+                wh, bh = self._head("wave1", wave)
+                hcoef = ops.head_conv3x3(d1, f // 2, 0, wh, bh, n, h, w, 3, scale=scale, act=ACT_NONE, pad=PAD_ZERO)
+                if sparse:
+                    # the reference builds this one as ones_like(h[:, 0]) with h already (N,1,3,H,W): a 3-channel map
+                    # (densedepth_decoder.py:301-303); kept as is
+                    out[("wavelet_mask", s)] = torch.ones((n, 3, h, w), dtype=torch.float32, device=xb.device)
+                out[("wavelets", s, "LL")] = ll
             else:
-                xa = ops.conv_rows(x_rows, x_c, wp, b, cout, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_LRELU,
-                                   act_param=0.2, shift0=1, x1=ops.nchw_to_rows(skip), c1=cs)
-                hcoef = ops.head_conv3x3(xa, cout, 0, wh, bh, n, 2 * h, 2 * w, 3, scale=scale, act=ACT_NONE,
-                                         pad=PAD_ZERO)
+                name = "up%d" % j
+                up = getattr(self, name)
+                skip = blocks[-1 - j]
+                cs = skip.shape[1]
+                cout = up.convA.conv.weight.shape[0]
+                wp, b = self._gemm(name, up.convA, cs)
+                wh, bh = self._head("wave%d" % j, wave)
+                if tuple(skip.shape[2:]) != (2 * h, 2 * w):
+                    raise WmdError("skip block has shape %s, expected spatial %s" % (tuple(skip.shape), (2 * h, 2 * w)))
+                if sparse:
+                    thresh = ops.range_thresh(ll, thresh_ratio)
+                    masks = ops.level_masks(hcoef, thresh, want=("S2", "S3", "S4", "S5"))
+                    gmap = ops.gate_map(masks["S2"], prev_map)
+                    map4, pix4, off4 = ops.compact(masks["S4"])
+                    _, pix5, off5 = ops.compact(masks["S5"], want_idxmap=False)
+                    counts.append((off4, off5))
+                    out[("wavelet_mask", s)] = masks["S5"].to(torch.float32)
+                    xa = ops.conv_rows(x_rows, x_c, wp, b, cout, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_LRELU,
+                                       act_param=0.2, map0=gmap, shift0=1, x1=ops.nchw_to_rows(skip), c1=cs,
+                                       gate=masks["S3"], pixels=pix4, count=off4[n:],
+                                       m_in0=_pm(lambda: (gmap >= 0).sum()), m_in1=_pm(lambda: masks["S3"].sum()))
+                    hcoef = ops.head_conv3x3(xa, cout, 0, wh, bh, n, 2 * h, 2 * w, 3, scale=scale, act=ACT_NONE,
+                                             pad=PAD_ZERO, idxmap=map4, pixels=pix5, count=off5[n:])
+                    prev_map = map4
+                else:
+                    xa = ops.conv_rows(x_rows, x_c, wp, b, cout, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_LRELU,
+                                       act_param=0.2, shift0=1, x1=ops.nchw_to_rows(skip), c1=cs)
+                    hcoef = ops.head_conv3x3(xa, cout, 0, wh, bh, n, 2 * h, 2 * w, 3, scale=scale, act=ACT_NONE,
+                                             pad=PAD_ZERO)
+                x_rows, x_c = xa, cout
+                h, w = 2 * h, 2 * w
             for k, band in enumerate(("LH", "HL", "HH")):
-                out[("wavelets", 1 - s, band)] = hcoef[:, k:k + 1]
-            if s == 0:
-                ll, disp = ops.idwt_haar(ll, hcoef.unsqueeze(1), disp_scale=0.5, clamp01=False)
-                out[("disp", 1)] = disp
+                out[("wavelets", s, band)] = hcoef[:, k:k + 1]
+            if disp_form == "div":
+                ll, disp = ops.idwt_haar(ll, hcoef.unsqueeze(1), disp_scale=1.0 / 2 ** s, clamp01=False)
+                out[("disp", s)] = disp
+            elif disp_form == "floor":
+                ll = ops.idwt_haar(ll, hcoef.unsqueeze(1))
+                out[("disp", s)] = ll // 2           # torch's floor division, as the reference computes it
             elif self.depth_epilogue is not None:
                 ll, depth = ops.idwt_haar(ll, hcoef.unsqueeze(1), epilogue=("div_clamp",) + tuple(self.depth_epilogue))
-                out[("disp", 0)], out[("depth", 0)] = ll, depth
+                out[("disp", s)], out[("depth", s)] = ll, depth
             else:
                 ll = ops.idwt_haar(ll, hcoef.unsqueeze(1))
-                out[("disp", 0)] = ll
-            x_rows, x_c = xa, cout
-            h, w = 2 * h, 2 * w
+                out[("disp", s)] = ll
         return out, (torch.stack([torch.stack(c) for c in counts]) if counts else None)
 
 
@@ -254,16 +283,7 @@ class DecoderWave(_NyuWaveBase):
         return outputs
 
     def forward(self, x_blocks):
-        _need_cuda(x_blocks)
-        needs_grad = torch.is_grad_enabled() and (
-            any(p.requires_grad for p in self.parameters()) or any(f.requires_grad for f in x_blocks))
-        if self._depthwise or (needs_grad and not train_native.fp32_convs_requested()):
-            return self._autograd_forward(x_blocks)
-        if needs_grad:
-            # fp32 convolutions requested: forward and backward of every convolution on libwmd
-            return train_native.nyu_forward(self, x_blocks)
-        out, _ = self._native_forward(x_blocks, 0.0, sparse=False)
-        return out
+        return self._forward(x_blocks)
 
 
 class SparseDecoderWave(_NyuWaveBase):
@@ -315,8 +335,7 @@ class SparseDecoderWave(_NyuWaveBase):
 
 # ------------------------------------------------------------------------------------------------------------------
 # API surface outside the hot path (SURVEY 8b lists them as constructible from NYUv2/model.py:47-64): the DenseDepth
-# baseline decoders and the 224-pixel wavelet variant.  They run on the differentiable cuDNN path (+ the native IDWT
-# through its autograd function); no native gather-GEMM engine is built for them.
+# baseline decoders.  They run on the differentiable cuDNN path; no native gather-GEMM engine is built for them.
 # ------------------------------------------------------------------------------------------------------------------
 class _BaselineDecoder(nn.Module):
     """conv2 -> four UpSampleBlocks -> [x2 + conv5 + LeakyReLU(0.2)] -> conv3; zero padding everywhere."""
@@ -368,31 +387,30 @@ class Decoder224(_BaselineDecoder):
         self._build(enc_features, decoder_width, is_depthwise, extra_stage=True)
 
 
-class DecoderWave224(nn.Module):
-    """Four-level wavelet decoder for 224-pixel inputs.  [densedepth_decoder.py:151-221]
+class DecoderWave224(_NyuWaveBase):
+    """Four-level wavelet decoder for 224-pixel inputs (NYUv2/train.py --use_224).  [densedepth_decoder.py:151-221]
 
-    Same state-dict names as the reference (conv2, up1..up4, wave1_ll, wave1..wave4, iwt / iwt_LL buffers).  Keeps the
-    reference's quirk of FLOOR-dividing ``("disp", 1)`` (:212, SURVEY A.5)."""
+    Same state-dict names and order as the reference (conv2, up1..up4, wave1_ll, wave1..wave4, iwt / iwt_LL buffers, the
+    unused sigmoid).  Runs like ``DecoderWave``: the native engine at inference, the native training forward when fp32
+    convolutions are requested, the cuDNN module graph for depthwise variants and for training with TF32 allowed.  Like
+    every NYU engine launch, the tensor-core convolutions take the tf32x3 operand form: the engine does not track its
+    sources' maxima, which the fp16-pair form needs.  ``depth_epilogue`` works as in ``DecoderWave``: with the reference's
+    224 evaluation (NYUv2/utils.py:215-229, no resize) it is ``(100, 0.4, 10)``.
+
+    Keeps the reference's quirks (:181-221): ``("wavelets", 3, "LL")`` is 16 * wave1_ll with details scaled 8, 4, 2, 1;
+    ``("disp", 3)`` is taken after the first IDWT; ``("disp", 1)`` is FLOOR-divided (:212, SURVEY A.5) - by torch on the
+    level's LL, so that it equals the reference's given the same LL; the native training step gives it a zero gradient
+    (train_native._FloorHalfFn); nothing is clamped."""
+
+    _LL_HEAD = (2 ** 4, None)
+    _LEVELS = ((1, 3, "div"), (2, 2, "div"), (3, 1, "floor"), (4, 0, "last"))
 
     def __init__(self, enc_features=[96, 96, 192, 384, 2208], decoder_width=0.5, dw_waveconv=False, dw_upconv=False):
         super().__init__()
-        f = int(enc_features[-1] * decoder_width)
-        self.iwt = IDWT(wave="haar", mode="zero")
-        self.iwt_LL = IDWT(wave="haar", mode="zero")
-        self.conv2 = Conv3x3(enc_features[-1], f, padding="replicate")
-        self.up1 = UpSampleBlock(skip_input=f + enc_features[-2], output_features=f // 2, padding="reflection",
-                                 is_depthwise=dw_upconv)
-        self.wave1_ll = Conv3x3(f // 2, 1, padding="replicate")
-        self.wave1 = Conv3x3(f // 2, 3, padding="zero", is_depthwise=dw_waveconv)
-        for k in range(2, 5):
-            setattr(self, "up%d" % k, UpSampleBlock(skip_input=f // 2 ** (k - 1) + enc_features[-1 - k],
-                                                    output_features=f // 2 ** k, padding="reflection",
-                                                    is_depthwise=dw_upconv))
-            setattr(self, "wave%d" % k, Conv3x3(f // 2 ** k, 3, padding="zero", is_depthwise=dw_waveconv))
+        self._build(enc_features, decoder_width, dw_waveconv, dw_upconv)
         self.sigmoid = nn.Sigmoid()
 
-    def forward(self, x_blocks):
-        _need_cuda(x_blocks)
+    def _autograd_forward(self, x_blocks):
         out = {}
         x = self.up1(self.conv2(x_blocks[-1]), x_blocks[-2])
         ll = (2 ** 4) * self.wave1_ll(x)
@@ -407,3 +425,6 @@ class DecoderWave224(nn.Module):
             ll = self.iwt((ll, [hcoef]))
             out[("disp", s)] = ll // 2 if s == 1 else ll / (2 ** s)
         return out
+
+    def forward(self, x_blocks):
+        return self._forward(x_blocks)

@@ -84,6 +84,23 @@ class _ConvRowsFn(torch.autograd.Function):
         return dx0 if need_x0 else None, dx1, dw, db, None
 
 
+class _FloorHalfFn(torch.autograd.Function):
+    """ll // 2 (torch's floor division) with a zero gradient: DecoderWave224's ("disp", 1) (densedepth_decoder.py:212).
+
+    A floor is flat wherever it is differentiable, so a loss on that output trains nothing; the native step keeps it that
+    way rather than giving it the gradient of ll / 2.  (Recent torch has no derivative for floor division at all: the
+    cuDNN path's backward raises when ("disp", 1) is in the loss.)"""
+
+    @staticmethod
+    def forward(ctx, ll):
+        return ll // 2
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        return torch.zeros_like(g)
+
+
 def _amax(dev):
     return torch.zeros(1, dtype=torch.float32, device=dev)
 
@@ -156,7 +173,10 @@ def kitti_forward(dec, feats):
 
 
 def nyu_forward(dec, blocks):
-    """DecoderWave's outputs (the reference's keys) with every convolution on libwmd, differentiable."""
+    """DecoderWave's / DecoderWave224's outputs (the reference's keys) with every convolution on libwmd, differentiable.
+
+    Follows the decoder's level table (nyu_decoders._NyuWaveBase._LEVELS).  A "floor" level's ("disp", s) is ll // 2
+    with a zero gradient (_FloorHalfFn)."""
     out = {}
     n, _, h, w = (int(v) for v in blocks[-1].shape)
     x, x_amax = to_rows(blocks[-1])
@@ -165,22 +185,27 @@ def nyu_forward(dec, blocks):
     c = dec.up1.convA.conv
     d, d_amax = conv(d, d_amax, blocks[-2], c.weight, c.bias, n, 2 * h, 2 * w, act=ACT_LRELU, act_param=0.2, shift0=1)
     h, w = 2 * h, 2 * w
+    ll_scale, ll_disp = dec._LL_HEAD
     c = dec.wave1_ll.conv
-    ll = 2 ** 3 * to_nchw(conv(d, d_amax, None, c.weight, c.bias, n, h, w, pad=PAD_REPLICATE)[0], n, 1, h, w)
-    out[("disp", 3)] = ll / 2 ** 3
-    out[("wavelets", 2, "LL")] = ll
-    for s, (up, wave, scale) in enumerate(((None, dec.wave1, 2), (dec.up2, dec.wave2, 1), (dec.up3, dec.wave3, 0))):
-        if up is not None:
-            c = up.convA.conv
-            d, d_amax = conv(d, d_amax, blocks[-2 - s], c.weight, c.bias, n, 2 * h, 2 * w, act=ACT_LRELU, act_param=0.2,
+    ll = ll_scale * to_nchw(conv(d, d_amax, None, c.weight, c.bias, n, h, w, pad=PAD_REPLICATE)[0], n, 1, h, w)
+    if ll_disp is not None:
+        out[("disp", ll_disp)] = ll / ll_scale
+    out[("wavelets", dec._LEVELS[0][1], "LL")] = ll
+    for j, s, disp_form in dec._LEVELS:
+        if j > 1:
+            c = getattr(dec, "up%d" % j).convA.conv
+            d, d_amax = conv(d, d_amax, blocks[-1 - j], c.weight, c.bias, n, 2 * h, 2 * w, act=ACT_LRELU, act_param=0.2,
                              shift0=1)
             h, w = 2 * h, 2 * w
-        c = wave.conv
+        c = getattr(dec, "wave%d" % j).conv
         hc = to_nchw(conv(d, d_amax, None, c.weight, c.bias, n, h, w, pad=PAD_ZERO)[0], n, 3, h, w).unsqueeze(1)
-        if scale:
-            hc = 2 ** scale * hc
+        if s:
+            hc = 2 ** s * hc
         for k, band in enumerate(("LH", "HL", "HH")):
-            out[("wavelets", scale, band)] = hc[:, :, k]
+            out[("wavelets", s, band)] = hc[:, :, k]
         ll = dec.iwt((ll, [hc]))
-        out[("disp", scale)] = ll / 2 ** scale if scale else ll
+        if disp_form == "floor":
+            out[("disp", s)] = _FloorHalfFn.apply(ll)
+        else:
+            out[("disp", s)] = ll / 2 ** s if s else ll
     return out
