@@ -247,10 +247,6 @@ int wmd_conv_rows_tc_f32(const wmd_conv_desc* d, wmd_stream_t stream);
  * layer (4 KiB of counters + SMs x 8 x 128 x 128 floats).  The first 4 KiB of `ws` (any splits) must be ZERO before the
  * first launch that uses the buffer; every launch leaves them zero. */
 size_t wmd_conv_tc_splitk_ws_bytes(int max_rows, int ldy, int splits);
-/* Shared-tap gather setting (one gather per (channel chunk, dy) feeding the three dx taps).  The sm_90a engine gathers
- * every tap's rows itself, so the setting does not change what runs or its bits; it is kept for the C ABI.  on < 0 only
- * queries.  Returns the previous setting.  Process-wide. */
-int wmd_conv_tc_set_shared_taps(int on);
 /* The tensor-core engine runs one persistent CTA per SM, and such a CTA holds most of the SM's shared memory: no other kernel -
  * an NCCL collective of the previous step in particular - can run beside it.  wmd_conv_tc_set_reserved_sms(n) makes the
  * persistent grid n CTAs smaller so that n SMs stay free (multi-GPU serving: the all-gather of step k then really runs

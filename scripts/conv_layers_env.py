@@ -1,4 +1,4 @@
-"""Per-layer CUDA-event times of one bench step under the current environment (A/B of env knobs: run it once per setting)."""
+"""Per-layer CUDA-event times of one bench step (A/B of builds: run it once per library, WMD_LIB_PATH selects it)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -17,5 +17,5 @@ for _ in range(3):
     dec(feats, bench.THRESH)
 torch.cuda.synchronize(); ops.set_profiler(None)
 tab = bench.conv_layer_table(prof.results(), 6570.9, 761.6, 3)
-print("WMD_TC_BALANCE_MIN_CHUNKS =", os.environ.get("WMD_TC_BALANCE_MIN_CHUNKS"), " sum %.1f us" % sum(l["us"] for l in tab))
+print("sum %.1f us" % sum(l["us"] for l in tab))
 print("  " + "  ".join("%s%s->%d:%.0f" % (l["taps"], l["cin"], l["cout"], l["us"]) for l in tab))

@@ -318,57 +318,50 @@ def test_cuda_graph_replay_matches_eager_and_follows_input_updates():
 
 
 def test_layout_move_options_are_bit_identical_eager_and_graphed():
-    """overlap_layout: the skip maps' NCHW->rows transposes run on a side stream (fork after the current stream,
-    join by event before first use).  gated_layout: a sparse level's skip map is transposed only under its upsample
-    mask (the only rows upconv(i,1) reads).  Neither changes what is computed: every output must equal the plain
-    in-order run bit for bit, launch by launch and inside a captured CUDA graph."""
+    """gated_layout: a sparse level's skip map is transposed only under its upsample mask (the only rows upconv(i,1)
+    reads).  That does not change what is computed: every output must equal the plain run bit for bit, launch by launch
+    and inside a captured CUDA graph."""
     from wavelet_monodepth_b200 import graphs
     mod, _, feats = _full_kitti(synth.RESNET18_CH, 3, 192, 640)
-    mod.overlap_layout = mod.gated_layout = False
-    mod.compact_skip = False                                 # these options concern the dense-row layout of the skip maps
+    mod.gated_layout = False
+    mod.compact_skip = False                                 # gated_layout concerns the dense-row layout of the skip maps
     for thr in (0.05, 0.2, 0.4, 0.6, 0.8):                   # first threshold at which the gate really removes rows
         want = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in mod(feats, thr).items()}
         dens = float(want[("upsample_mask", 0)].float().mean())
         if 0.0 < dens < 0.9:
             break
     assert 0.0 < dens < 0.9, dens
-    try:
-        for overlap, gated in ((True, False), (False, True), (True, True)):
-            mod.overlap_layout, mod.gated_layout = overlap, gated
-            mod.overlap_compaction = overlap                       # compactions on parallel streams: same kernels, same data
-            for _ in range(3):                               # repeated: allocator reuse across the two streams
-                got = mod(feats, thr)
-                torch.cuda.synchronize()
-                for k, v in want.items():
-                    assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (overlap, gated, key_str(k))
-            g = graphs.GraphedSparseDecoder(mod, feats, thr)
-            for _ in range(2):
-                got = g.replay()
-                for k, v in want.items():
-                    assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (overlap, gated, key_str(k))
-            del g
-        # gated move reading the two finest skip maps in place from pinned host memory (zero-copy over PCIe)
-        on_host = [feats[0].cpu().pin_memory(), feats[1].cpu().pin_memory()] + list(feats[2:])
-        for overlap in (False, True):
-            mod.overlap_layout, mod.gated_layout = overlap, True
-            got = mod(on_host, thr)
+    for gated in (False, True):
+        mod.gated_layout = gated
+        for _ in range(3):                                   # repeated: allocator reuse across the side streams
+            got = mod(feats, thr)
             torch.cuda.synchronize()
             for k, v in want.items():
-                assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), ("host", overlap, key_str(k))
-        g = graphs.GraphedSparseDecoder(mod, on_host, thr)
-        got = g.replay()
-        for k, v in want.items():
-            assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), ("host graph", key_str(k))
+                assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (gated, key_str(k))
+        g = graphs.GraphedSparseDecoder(mod, feats, thr)
+        for _ in range(2):
+            got = g.replay()
+            for k, v in want.items():
+                assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (gated, key_str(k))
         del g
-        with pytest.raises(kd.WmdError):                       # pageable host memory is refused
-            mod([feats[0].cpu()] + list(feats[1:]), thr)
-        with pytest.raises(kd.WmdError):                       # a dense level's skip map must be on the device
-            mod(list(feats[:3]) + [feats[3].cpu().pin_memory(), feats[4]], thr)
-        mod.gated_layout = False
-        with pytest.raises(kd.WmdError):                       # without the gated move nothing reads host memory
-            mod(on_host, thr)
-    finally:
-        mod.overlap_layout = mod.gated_layout = mod.overlap_compaction = False
+    # gated move reading the two finest skip maps in place from pinned host memory (zero-copy over PCIe)
+    on_host = [feats[0].cpu().pin_memory(), feats[1].cpu().pin_memory()] + list(feats[2:])
+    got = mod(on_host, thr)
+    torch.cuda.synchronize()
+    for k, v in want.items():
+        assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), ("host", key_str(k))
+    g = graphs.GraphedSparseDecoder(mod, on_host, thr)
+    got = g.replay()
+    for k, v in want.items():
+        assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), ("host graph", key_str(k))
+    del g
+    with pytest.raises(kd.WmdError):                         # pageable host memory is refused
+        mod([feats[0].cpu()] + list(feats[1:]), thr)
+    with pytest.raises(kd.WmdError):                         # a dense level's skip map must be on the device
+        mod(list(feats[:3]) + [feats[3].cpu().pin_memory(), feats[4]], thr)
+    mod.gated_layout = False
+    with pytest.raises(kd.WmdError):                         # without the gated move nothing reads host memory
+        mod(on_host, thr)
 
 
 def test_fused_head_stages_match_the_two_launch_path():
@@ -396,25 +389,6 @@ def test_fused_head_stages_match_the_two_launch_path():
 def _lib_launches():
     from wavelet_monodepth_b200 import _lib
     return _lib.launch_count()
-
-
-def test_factored_ll_head_matches_the_direct_head_kernel():
-    """factored_ll: level 4 computes the LL head's 3x3 stage as nine more tap-product columns of the +/- heads' GEMM and
-    a 9-float gather-sum, instead of the warp-per-pixel head kernel.  Same arithmetic up to summation order."""
-    mod, _, feats = _full_kitti(synth.RESNET18_CH, 3, 192, 640)
-    mod.factored_ll = False
-    want = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in mod(feats, 0.05).items()}
-    mod.factored_ll = True
-    try:
-        got = mod(feats, 0.05)
-        torch.cuda.synchronize()
-    finally:
-        mod.factored_ll = False
-    assert rel_err(got[("wavelets", 3, "LL")], want[("wavelets", 3, "LL")]) <= 1e-5
-    for s in range(4):
-        assert rel_err(got[("disp", s)], want[("disp", s)]) <= 1e-5, s
-        flips = float((got[("wavelet_mask", s)] != want[("wavelet_mask", s)]).float().mean())
-        assert flips <= 1e-4, (s, flips)
 
 
 # ------------------------------------------------------------------------------------------ host-side behaviour added in round 2
@@ -528,24 +502,25 @@ def test_npy_coefficient_dumps_as_test_simple_writes_them(tmp_path):
     assert rel_err(np.load(tmp_path / "x_disp.npy"), want["disp_0"]) <= REL_TOL
 
 
-def test_fused_level_tail_is_bit_identical_to_the_three_kernel_chain_and_epilogue_matches_disp_to_depth():
-    """fused_tail: head gather-sum -> yh -> IDWT -> disp -> next threshold in one kernel (wmd_head_idwt_f32) must equal the
-    head_gather + idwt_haar + range_thresh chain bit for bit (same summation order), on sparse, masked-dense and dense
-    levels, TMA-staged (W % 16 == 0) and plain staging; depth_range adds disp_to_depth(("disp", 0)) (KITTI/layers.py:16-25)."""
+def test_fused_level_tail_is_bit_identical_to_the_three_kernel_chain_and_epilogue_matches_disp_to_depth(monkeypatch):
+    """The fused level tail: head gather-sum -> yh -> IDWT -> disp -> next threshold in one kernel (wmd_head_idwt_f32) must
+    equal the head_gather + idwt_haar + range_thresh chain bit for bit (same summation order), on sparse, masked-dense and
+    dense levels, TMA-staged (W % 16 == 0) and plain staging; depth_range adds disp_to_depth(("disp", 0))
+    (KITTI/layers.py:16-25)."""
     for ch, hw in ((synth.RESNET18_CH, (192, 640)), (synth.RESNET18_CH, (128, 256))):      # widths 40.. (plain) / 16.. (TMA)
         mod, dense, feats = _full_kitti(ch, 3, *hw)
         for scales in ([1, 2, 3], [1]):
-            mod.fused_tail = False
-            want = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in mod(feats, 0.05, scales).items()}
-            mod.fused_tail = True
+            with monkeypatch.context() as m:
+                m.setattr(kd, "_fused_tail_fits", lambda width: False)          # every level on the chain
+                want = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in mod(feats, 0.05, scales).items()}
             got = mod(feats, 0.05, scales)
             assert set(got) == set(want)
             for k, v in want.items():
                 assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (hw, scales, key_str(k))
-        dense.fused_tail = False
-        with torch.no_grad():
+        with torch.no_grad(), monkeypatch.context() as m:
+            m.setattr(kd, "_fused_tail_fits", lambda width: False)
             want = {k: v.clone() for k, v in dense(feats).items()}
-            dense.fused_tail = True
+        with torch.no_grad():
             got = dense(feats)
         for k, v in want.items():
             assert torch.equal(got[k], v), (hw, "dense", key_str(k))
@@ -602,13 +577,10 @@ def test_compact_skip_rows_bit_identical_to_dense_skip_rows_device_and_pinned_ho
     mod.compact_skip_levels = (1, 2, 3)
     on_host = [f.cpu().pin_memory() for f in feats[:3]] + list(feats[3:])
     for inputs in (feats, on_host):
-        for overlap in (True, False):
-            mod.overlap_compaction = overlap
-            got = mod(inputs, 0.05)
-            torch.cuda.synchronize()
-            for k, v in want.items():
-                assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (inputs is on_host, overlap, key_str(k))
-        mod.overlap_compaction = True
+        got = mod(inputs, 0.05)
+        torch.cuda.synchronize()
+        for k, v in want.items():
+            assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (inputs is on_host, key_str(k))
         g = graphs.GraphedSparseDecoder(mod, inputs, 0.05)
         got = g.replay()
         for k, v in want.items():
@@ -619,10 +591,9 @@ def test_compact_skip_rows_bit_identical_to_dense_skip_rows_device_and_pinned_ho
 
 
 def test_f16x3_operand_form_meets_the_same_parity_bars(monkeypatch):
-    """WMD_CONV_PRECISION=f16x3 (opt-in): fp16-pair operands with per-tensor power-of-two scaling - the tiny sparse golden
-    (reference outputs) and the batched-vs-per-sample oracle comparison hold at the tolerance of the default form, masks
-    and total_ops exact; every tensor-core launch that has its sources' maxima really runs the f16 form."""
-    monkeypatch.setenv("WMD_CONV_PRECISION", "f16x3")
+    """f16x3: fp16-pair operands with per-tensor power-of-two scaling - the tiny sparse golden (reference outputs) and the
+    batched-vs-per-sample oracle comparison hold at the tolerance of the default form, masks and total_ops exact; every
+    tensor-core launch that has its sources' maxima really runs the f16 form."""
     seen = []
     real = ops.conv_rows
 

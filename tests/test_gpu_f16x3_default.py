@@ -3,7 +3,7 @@
 - Every layout move of a sparse level's skip map reports the max |x| of exactly the pixels upconv(i,1) reads (the level's
   upsample mask S3), whether it is plain, gated, list-based or a channels_last view used in place.  The operand scale is a
   power of two taken from that maximum, so the layout options pick the same scale and give the same bits.
-- With no environment set, the flagship decoder (ResNet50 pyramid, 1024x320) runs every tensor-core launch in f16x3.
+- The flagship decoder (ResNet50 pyramid, 1024x320) runs every tensor-core launch in f16x3.
 - The shared-memory ring is 6 stages deep for f16 N = 128 tiles and 8 for N = 64 / 32.  Contract cases whose chunk counts
   per tile are not multiples of the ring depth put the tile boundaries at changing ring offsets, with several tiles per CTA
   (whole tiles) and stream-K segments (balanced); each is checked against the fp64 reference of tests/conv_ref.py.
@@ -73,9 +73,7 @@ def test_masked_row_maximum_of_a_view():
     assert float(none) == 0.0
 
 
-def test_flagship_decoder_runs_every_tensor_core_launch_in_f16x3(monkeypatch):
-    monkeypatch.delenv("WMD_CONV_PRECISION", raising=False)
-    assert ops.default_conv_precision() == "f16x3"
+def test_flagship_decoder_runs_every_tensor_core_launch_in_f16x3_without_configuration():
     mod = kd.SparseDepthWaveProgressiveDecoder(np.array(synth.RESNET50_CH))
     synth.bench_kitti_params(mod)
     mod = mod.to(DEV).eval()

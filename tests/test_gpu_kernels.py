@@ -425,12 +425,10 @@ def _blob_mask(n, h, w, p, seed, grow):
 
 @pytest.mark.parametrize("case", ["dense_two_sources", "blobs_two_sources_balanced", "blobs_one_source", "isolated_pixels_fallback",
                                   "thin_n32", "wide_n128"])
-def test_shared_tap_gather_is_bit_identical_to_per_tap_gather(case):
-    """conv_rows_tc<N, SH>: one raw-stage fill per (chunk, dy) feeding the three dx taps through the slot table must give
-    the bits of the one-gather-per-tap form (same MMAs, same order) - dense grids, clustered active lists (extras at
-    run ends), isolated pixels (extras overflow -> per-chunk fills), stream-K cuts that start mid-group, all N tiles."""
-    from wavelet_monodepth_b200 import _lib
-    lib = _lib.load()
+def test_tc_conv_gathers_give_the_same_bits_on_every_launch(case):
+    """conv_rows_tc gathers every tap's rows itself: two launches must give the same bits, and non-zero ones - dense
+    grids, clustered active lists (extras at run ends), isolated pixels (extras overflow -> per-chunk fills), stream-K
+    cuts that start mid-group, all N tiles."""
     cfg = {
         "dense_two_sources": dict(n=2, h=40, w=64, c0=64, c1=96, cout=64, p=None, grow=0, pad=PAD_REFLECT),
         "blobs_two_sources_balanced": dict(n=3, h=48, w=96, c0=256, c1=64, cout=64, p=0.02, grow=2, pad=PAD_REFLECT),
@@ -464,15 +462,9 @@ def test_shared_tap_gather_is_bit_identical_to_per_tap_gather(case):
             kw.update(map0=map0)
         assert int(offsets[n]) > 3 * 256                # several tiles
     outs = []
-    was = lib.wmd_conv_tc_set_shared_taps(-1)
-    try:
-        for sh in (0, 1):
-            lib.wmd_conv_tc_set_shared_taps(sh)
-            for _ in range(2):                           # twice: deterministic
-                outs.append(ops.conv_rows(lo_rows, c0, wp, b.to(DEV), cout, n, h, w, **kw).clone())
-            torch.cuda.synchronize()
-    finally:
-        lib.wmd_conv_tc_set_shared_taps(was)
+    for _ in range(2):                                   # twice: deterministic
+        outs.append(ops.conv_rows(lo_rows, c0, wp, b.to(DEV), cout, n, h, w, **kw).clone())
+    torch.cuda.synchronize()
     rows = int(kw["count"][0]) if "count" in kw else n * h * w
     for o in outs[1:]:
         assert torch.equal(o[:rows, :cout], outs[0][:rows, :cout])

@@ -37,22 +37,19 @@ def _worker(rank, world, port, n_global, result_dir):
         assert full.shape[0] == n_global
         # the overlapped form: three "steps" whose local output buffer is overwritten right after start() - what a
         # CUDA-graph replay does - each gathered through the double-buffered staging slots
-        # ... and the copy-engine form's class, which must fall back to the same NCCL / gloo path off an NVLink node
-        assert type(shard.make_gather(n_global)) is shard.OverlappedGather        # gloo: no peer memory
-        for og in (shard.OverlappedGather(n_global), shard.PeerGather(n_global)):
-            buf = torch.empty_like(out[("disp", 0)])
-            handles, wants = [], []
-            for k in range(5):
-                buf.copy_(out[("disp", 0)] * (k + 1))
-                handles.append(og.start(buf))
-                buf.fill_(-1.0)                            # the producer moves on before the gather is consumed
-                wants.append(full * (k + 1))
-                if k >= 1:                                 # consume step k-1 while step k is in flight
-                    got = handles[k - 1].wait()
-                    assert torch.equal(got, wants[k - 1]), ("overlapped gather", type(og).__name__, k - 1)
-            assert torch.equal(handles[4].wait(), wants[4])
-            if isinstance(og, shard.PeerGather):
-                assert og._peer is False and og.why_not
+        assert type(shard.make_gather(n_global)) is shard.OverlappedGather
+        og = shard.OverlappedGather(n_global)
+        buf = torch.empty_like(out[("disp", 0)])
+        handles, wants = [], []
+        for k in range(5):
+            buf.copy_(out[("disp", 0)] * (k + 1))
+            handles.append(og.start(buf))
+            buf.fill_(-1.0)                                # the producer moves on before the gather is consumed
+            wants.append(full * (k + 1))
+            if k >= 1:                                     # consume step k-1 while step k is in flight
+                got = handles[k - 1].wait()
+                assert torch.equal(got, wants[k - 1]), ("overlapped gather", k - 1)
+        assert torch.equal(handles[4].wait(), wants[4])
         if rank == 0:
             ref = okitti.dense_forward(sd, feats)[("disp", 0)]
             torch.save({"full": full, "ref": ref}, os.path.join(result_dir, "r0_%d.pt" % n_global))
@@ -68,11 +65,11 @@ def _run(n_global, tmp_path):
     assert float((res["full"] - res["ref"]).abs().max()) < 1e-5
 
 
-def test_even_shards(tmp_path):
+def test_even_shards_through_the_overlapped_gather(tmp_path):
     _run(2, tmp_path)
 
 
-def test_ragged_shards(tmp_path):
+def test_ragged_shards_through_the_overlapped_gather(tmp_path):
     _run(3, tmp_path)
 
 

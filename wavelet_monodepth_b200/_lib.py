@@ -118,7 +118,6 @@ SIGNATURES = {
     "wmd_nchw_to_rows_gated_amax_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_longlong, c_int, c_void_p, c_void_p]),
     "wmd_gather_rows_list_amax_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                               c_int, c_void_p, c_void_p]),
-    "wmd_conv_tc_set_shared_taps": (c_int, [c_int]),
     "wmd_conv_tc_set_reserved_sms": (c_int, [c_int]),
     "wmd_conv_tc_weight_floats": (c_size_t, [c_int, c_int, c_int, c_int]),
     "wmd_pack_conv_weight_tc_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

@@ -1025,7 +1025,6 @@ __global__ void finish_header_tc16_kernel(unsigned char* out) {
 static int tc_tile_n(int cout) { return cout >= 96 ? 128 : (cout >= 48 ? 64 : 32); }
 
 static int g_reserved_sms = 0;     // SMs the persistent grid leaves free (for a collective's kernel on multi-GPU runs)
-static int g_shared_taps = 1;      // kept for the C ABI: every tap gathers its own rows in this engine
 
 template <int BN, bool F16>
 static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStream_t stream) {
@@ -1061,12 +1060,6 @@ extern "C" int wmd_conv_tc_tile_n(int cout) { return wmd::tc_tile_n(cout); }
 extern "C" int wmd_conv_tc_set_reserved_sms(int n) {
   const int was = wmd::g_reserved_sms;
   if (n >= 0) wmd::g_reserved_sms = n;
-  return was;
-}
-
-extern "C" int wmd_conv_tc_set_shared_taps(int on) {
-  const int was = wmd::g_shared_taps;
-  if (on >= 0) wmd::g_shared_taps = on ? 1 : 0;
   return was;
 }
 

@@ -20,7 +20,6 @@ What is different underneath (H100-native, DESIGN.md):
     convolutions are requested (torch.backends.cudnn.allow_tf32 False, train_native.py); with TF32 allowed it takes the
     differentiable cuDNN path.  Both train through the native IDWT with its adjoint.
 """
-import os
 from collections import OrderedDict
 
 import numpy as np
@@ -73,13 +72,20 @@ def _pm(fn):
 _SIDE_STREAMS = {}
 
 
-def _side_stream(device, which=0):
-    """Side streams per device (0: layout moves, 1-2: compactions), created lazily and reused: CUDA graphs fork/join
-    through them."""
+def _side_stream(device, which):
+    """Side streams per device (1-2: compactions of S4 / S5, 3: S3's compaction and skip-row gather), created lazily and
+    reused: CUDA graphs fork/join through them."""
     key = (device.type, device.index if device.index is not None else torch.cuda.current_device(), which)
     if key not in _SIDE_STREAMS:
         _SIDE_STREAMS[key] = torch.cuda.Stream(device=device)
     return _SIDE_STREAMS[key]
+
+
+def _fused_tail_fits(width):
+    """Whether a level's tail runs as one kernel (wmd_head_idwt_f32: head gather-sum -> yh -> IDWT -> disp -> next level's
+    threshold, bit-identical to the head_gather + idwt_haar + range_thresh chain).  The kernel needs the width of the
+    level's coefficient maps to be a multiple of 4; other widths (level 4 of small frames) take the chain."""
+    return width % 4 == 0
 
 
 def _need_cuda(feats, host_ok=()):
@@ -165,28 +171,19 @@ class _WaveDecoderBase(nn.Module):
         # align_corners=False) for s = 1..3 - what KITTI/trainer.py:338-339 computes from every scale - produced
         # straight from the coefficients by the fused IDWT+bilinear kernel
         self.full_res_size = None
-        # run the skip maps' layout transposes on a side stream (WMD_OVERLAP_LAYOUT=0/1 sets the default)
-        self.overlap_layout = os.environ.get("WMD_OVERLAP_LAYOUT", "0") == "1"
-        # transpose a sparse level's skip map only under its upsample mask (WMD_GATED_LAYOUT=0/1 sets the default).  On since
-        # the gated move issues all its loads before using any (72 us against 175 before and ~110 for the whole level-3 map)
-        self.gated_layout = os.environ.get("WMD_GATED_LAYOUT", "1") == "1"
-        # run the two 1x1 head stages of the fine levels as one fused kernel (WMD_FUSED_HEADS=0/1 sets the default)
-        self.fused_heads = os.environ.get("WMD_FUSED_HEADS", "1") == "1"
-        # level 4: the LL head's 3x3 stage rides in the tap-product GEMM of the +/- heads (WMD_FACTORED_LL=0/1)
-        self.factored_ll = os.environ.get("WMD_FACTORED_LL", "1") == "1"
-        # compactions of the level's three active sets on parallel streams (WMD_OVERLAP_COMPACTION=0/1)
-        self.overlap_compaction = os.environ.get("WMD_OVERLAP_COMPACTION", "1") == "1"
+        # transpose a sparse level's skip map only under its upsample mask.  On since the gated move issues all its loads
+        # before using any (72 us against 175 before and ~110 for the whole level-3 map)
+        self.gated_layout = True
+        # run the two 1x1 head stages of the fine levels as one fused kernel
+        self.fused_heads = True
         # sparse levels keep their skip map COMPACT: only the rows of the upsample mask S3 are moved out of the NCHW map
         # (list-based gather-transpose: bytes scale with the mask density, 16-50 % on the bench) and upconv(i,1) reaches them
-        # through S3's index map (wmd_conv_desc.map1).  The skip map may then be a pinned HOST tensor.  WMD_COMPACT_SKIP=0/1
-        self.compact_skip = os.environ.get("WMD_COMPACT_SKIP", "1") == "1"
+        # through S3's index map (wmd_conv_desc.map1).  The skip map may then be a pinned HOST tensor.
+        self.compact_skip = True
         # ... at the levels where it pays on a device-resident map: the list-based gather moves fewer useful bytes per second
         # than the whole-map transpose (scripts/probe_gather.py), so it wins only at low mask density - levels 2 and 1
         # (16-28 % on the bench), not level 3 (50 %).  A pinned-host skip map always takes it.
-        self.compact_skip_levels = tuple(int(v) for v in os.environ.get("WMD_COMPACT_SKIP_LEVELS", "1,2").split(",") if v)
-        # tail of every level as one kernel: head gather-sum -> yh -> IDWT -> disp -> next level's threshold
-        # (wmd_head_idwt_f32; WMD_FUSED_TAIL=0/1).  Bit-identical to the head_gather + idwt_haar + range_thresh chain.
-        self.fused_tail = os.environ.get("WMD_FUSED_TAIL", "1") == "1"
+        self.compact_skip_levels = (1, 2)
         # optional consumer epilogue of ("disp", 0), off by default: (min_depth, max_depth) adds ("scaled_disp", 0) and
         # ("depth", 0) = disp_to_depth(("disp", 0), min_depth, max_depth) (KITTI/layers.py:16-25; evaluate_depth.py:193,
         # test_simple.py:151), produced by the last level's fused tail
@@ -207,15 +204,14 @@ class _WaveDecoderBase(nn.Module):
         conv = self.convs[("upconv", i, j)].conv.conv
         # upconv(i,1) reads the skip map as gather source 1; without skips it reads only the upsampled upconv(i,0)
         c1 = int(self.num_ch_enc[i - 1]) if (j == 1 and self.use_skips) else 0
-        kind = ops.default_conv_kind()
-        return self._packs.get(("upconv", i, j, kind), [conv.weight], lambda: ops.pack_weight(conv.weight, c1)), conv.bias.detach()
+        return self._packs.get(("upconv", i, j), [conv.weight], lambda: ops.pack_weight(conv.weight, c1)), conv.bias.detach()
 
     def _head_1x1(self, i):
         """Concatenated 1x1 stages of the level's heads: [LL (i==4) | + | -] -> (packed (C, ld), bias, offsets)."""
         names = ([0] if i == 4 else []) + [1, -1]
         convs = [self.convs[("waveconv", i, j)][0].conv for j in names]
         wts = [c.weight for c in convs]
-        packed = self._packs.get(("head1x1", i, ops.default_conv_kind()), wts,
+        packed = self._packs.get(("head1x1", i), wts,
                                  lambda: ops.pack_weight(torch.cat([w.detach() for w in wts], 0)))
         bias = self._packs.get(("head1x1b", i), [c.bias for c in convs],
                                lambda: torch.cat([c.bias.detach() for c in convs], 0).contiguous())
@@ -228,19 +224,18 @@ class _WaveDecoderBase(nn.Module):
     def _head_taps(self, i, offs, ctot):
         """Factored +/- 3x3 stage: packed (54, ctot) tap-product weight and the 6 biases [+ | -].
 
-        With factored_ll, level 4 appends the LL head's nine tap filters as columns 54..62 (same 64-wide GEMM tile)."""
+        Level 4 appends the LL head's nine tap filters as columns 54..62 (same 64-wide GEMM tile)."""
         cp, cn = self.convs[("waveconv", i, 1)][2].conv, self.convs[("waveconv", i, -1)][2].conv
-        kind = ops.default_conv_kind()
-        if i == 4 and self.factored_ll:
+        if i == 4:
             cl = self.convs[("waveconv", i, 0)][2].conv
-            wz = self._packs.get(("headtaps+ll", i, kind), [cp.weight, cn.weight, cl.weight],
+            wz = self._packs.get(("headtaps+ll", i), [cp.weight, cn.weight, cl.weight],
                                  lambda: ops.pack_weight(torch.cat([
                                      ops.head_tap_weight([cp.weight, cn.weight], [offs[1], offs[-1]], ctot),
                                      ops.head_tap_weight([cl.weight], [offs[0]], ctot)], 0)))
             bz = self._packs.get(("headtapsb", i), [cp.bias, cn.bias],
                                  lambda: torch.cat([cp.bias.detach(), cn.bias.detach()]).contiguous())
             return wz, bz
-        wz = self._packs.get(("headtaps", i, kind), [cp.weight, cn.weight],
+        wz = self._packs.get(("headtaps", i), [cp.weight, cn.weight],
                              lambda: ops.pack_weight(ops.head_tap_weight([cp.weight, cn.weight], [offs[1], offs[-1]], ctot)))
         bz = self._packs.get(("headtapsb", i), [cp.bias, cn.bias],
                              lambda: torch.cat([cp.bias.detach(), cn.bias.detach()]).contiguous())
@@ -257,10 +252,6 @@ class _WaveDecoderBase(nn.Module):
                                lambda: ops.pack_head_mlp(torch.cat([c1p.weight.detach(), c1n.weight.detach()], 0),
                                                          torch.cat([c1p.bias.detach(), c1n.bias.detach()], 0),
                                                          ops.head_tap_weight([c3p.weight, c3n.weight], [0, c], 2 * c)))
-
-    def _head_3x3(self, i, j):
-        conv = self.convs[("waveconv", i, j)][2].conv
-        return self._packs.get(("head3x3", i, j), [conv.weight], lambda: ops.pack_head_weight(conv.weight)), conv.bias.detach()
 
     # ---- native engine ------------------------------------------------------------------------
     @torch.no_grad()
@@ -301,19 +292,14 @@ class _WaveDecoderBase(nn.Module):
         if n == 0:
             return self._empty_outputs(feats, sparse_levels, with_masks)
         # max |x| of every tensor a tensor-core conv reads (device scalars, zeroed here, raised by the producers): the
-        # fp16-pair operand form (the default, ops.default_conv_precision) scales by a power of two chosen from them.  A
-        # skip map's maximum covers exactly the pixels upconv(i,1) reads, so every layout option picks the same scale.
-        track = ops.default_conv_precision() == "f16x3"
-        amax = torch.zeros(24, dtype=torch.float32, device=dev) if track else None
-        slot = (lambda k: amax[k:k + 1]) if track else (lambda k: None)
+        # fp16-pair operand form scales by a power of two chosen from them.  A skip map's maximum covers exactly the
+        # pixels upconv(i,1) reads, so every layout option picks the same scale.
+        amax = torch.zeros(24, dtype=torch.float32, device=dev)
+
+        def slot(k):
+            return amax[k:k + 1]
         x_rows, x_c, prev_map = ops.nchw_to_rows(feats[4], amax=slot(0)), feats[4].shape[1], None
         x_amax = slot(0)
-        # layout moves of the skip maps (NCHW -> pixel-major rows), two options on top of the plain in-order transpose:
-        #  gated_layout   a sparse level reads its skip map only under the upsample mask S3 (sparse_upsample:
-        #                 skip[mask], layers.py:500), so only those rows are produced - the move scales with density;
-        #  overlap_layout the move runs on a side stream next to the level's upconv(i,0), which does not need it
-        #                 (HBM-bound transposes fill the tails of the tensor-bound convolution), joined by an event.
-        side = _side_stream(dev) if self.overlap_layout else None
         h, w = feats[4].shape[2:]
         yl = yh = None
         counts = {}
@@ -321,6 +307,7 @@ class _WaveDecoderBase(nn.Module):
         for i in range(4, 0, -1):
             c = int(self.num_ch_dec[i])
             sparse = i in sparse_levels
+            one_kernel_tail = _fused_tail_fits(2 * w)
             # without skips the maps feats[0..3] are never read: no layout move, gate, compaction or maximum for them
             skip = feats[i - 1] if self.use_skips else None
             cs = skip.shape[1] if self.use_skips else 0
@@ -335,27 +322,20 @@ class _WaveDecoderBase(nn.Module):
                     masks = ops.level_masks(yh, thresh)
             skip_rows = skip_amax = skip_done = map3 = None
             if self.use_skips:
-                skip_gate = masks["S3"] if (sparse and self.gated_layout) else None
+                skip_amax = slot(i)
                 if sparse and self.compact_skip and (i in self.compact_skip_levels or not skip.is_cuda) and \
                         ops.rows_view(skip) is None:                         # channels_last maps are used in place instead
                     # S3's compaction and the gather of exactly its rows, on a side stream next to gate_map / compact(S2) / upconv(i,0)
-                    s3 = _side_stream(dev, 3) if self.overlap_compaction else None
-                    if s3 is not None:
-                        (map3, pix3, off3), _ = ops.compact(masks["S3"], stream=s3, ws_slot=3)
-                        skip_rows, skip_done = ops.gather_rows_list(skip, pix3, off3[n:], stream=s3, amax=slot(i))
-                    else:
-                        map3, pix3, off3 = ops.compact(masks["S3"], ws_slot=3)
-                        skip_rows = ops.gather_rows_list(skip, pix3, off3[n:], amax=slot(i))
-                    skip_amax = slot(i)
+                    s3 = _side_stream(dev, 3)
+                    (map3, pix3, off3), _ = ops.compact(masks["S3"], stream=s3, ws_slot=3)
+                    skip_rows, skip_done = ops.gather_rows_list(skip, pix3, off3[n:], stream=s3, amax=skip_amax)
                 else:
-                    skip_amax = slot(i)
-                    # a sparse level's maximum covers S3 only, the rows upconv(i,1) reads, whether the move is gated or not
-                    max_mask = masks["S3"] if (sparse and track) else None
-                    if side is not None:
-                        skip_rows, skip_done = ops.nchw_to_rows(skip, stream=side, gate=skip_gate, amax=skip_amax,
-                                                                amax_mask=max_mask)
-                    else:
-                        skip_rows = ops.nchw_to_rows(skip, gate=skip_gate, amax=skip_amax, amax_mask=max_mask)
+                    # layout move of the skip map (NCHW -> pixel-major rows).  gated_layout: a sparse level reads its skip
+                    # map only under the upsample mask S3 (sparse_upsample: skip[mask], layers.py:500), so only those rows
+                    # are produced - the move scales with density.  A sparse level's maximum covers S3 only, the rows
+                    # upconv(i,1) reads, whether the move is gated or not
+                    skip_gate = masks["S3"] if (sparse and self.gated_layout) else None
+                    skip_rows = ops.nchw_to_rows(skip, gate=skip_gate, amax=skip_amax, amax_mask=masks["S3"] if sparse else None)
             if with_masks:
                 for name, key in (("lowres_mask", "S1"), ("upconv0_mask", "S2"), ("upsample_mask", "S3"),
                                   ("upconv1_mask", "S4"), ("wavelet_mask", "S5")):
@@ -368,27 +348,21 @@ class _WaveDecoderBase(nn.Module):
             if sparse:
                 if yl is None:
                     raise WmdError("a sparse level needs a previous dense level (depth_decoder.py:344)")
-                ev4 = ev5 = None
-                if self.overlap_compaction:
-                    # the three compactions are independent: S4 / S5 go to two side streams (own workspaces) and are
-                    # joined where their lists are first read (upconv(i,1) / the head scatter)
-                    (map4, pix4, off4), ev4 = ops.compact(masks["S4"], stream=_side_stream(dev, 1), ws_slot=1)
-                    (_, pix5, off5), ev5 = ops.compact(masks["S5"], want_idxmap=False, want_pixels=not self.fused_tail,
-                                                       stream=_side_stream(dev, 2), ws_slot=2)   # fused tail: the count only
+                # the three compactions are independent: S4 / S5 go to two side streams (own workspaces) and are joined
+                # where their lists are first read (upconv(i,1) / the head scatter)
+                (map4, pix4, off4), ev4 = ops.compact(masks["S4"], stream=_side_stream(dev, 1), ws_slot=1)
+                (_, pix5, off5), ev5 = ops.compact(masks["S5"], want_idxmap=False, want_pixels=not one_kernel_tail,
+                                                   stream=_side_stream(dev, 2), ws_slot=2)   # fused tail: the count only
                 gmap = ops.gate_map(masks["S1"], prev_map)
                 map2, pix2, off2 = ops.compact(masks["S2"])
-                if not self.overlap_compaction:
-                    map4, pix4, off4 = ops.compact(masks["S4"])
-                    _, pix5, off5 = ops.compact(masks["S5"], want_idxmap=False, want_pixels=not self.fused_tail)
                 counts[i] = (off2, off4, off5)
                 xa = ops.conv_rows(x_rows, x_c, wp0, b0, c, n, h, w, pad=PAD_REFLECT, act=ACT_ELU, map0=gmap,
                                    pixels=pix2, count=off2[n:], m_in0=_pm(lambda: (gmap >= 0).sum()),
                                    amax0=x_amax, amax_out=slot(4 + i))
                 if skip_done is not None:
                     torch.cuda.current_stream(dev).wait_event(skip_done)
-                if ev4 is not None:
-                    torch.cuda.current_stream(dev).wait_event(ev4)
-                    torch.cuda.current_stream(dev).wait_event(ev5)
+                torch.cuda.current_stream(dev).wait_event(ev4)
+                torch.cuda.current_stream(dev).wait_event(ev5)
                 xb = ops.conv_rows(xa, c, wp1, b1, c, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_ELU, map0=map2,
                                    shift0=1, x1=skip_rows, c1=cs, map1=map3, gate=masks["S3"], pixels=pix4, count=off4[n:],
                                    m_in0=off2[n:], m_in1=_pm(lambda: masks["S3"].sum()),
@@ -401,8 +375,6 @@ class _WaveDecoderBase(nn.Module):
             else:
                 xa = ops.conv_rows(x_rows, x_c, wp0, b0, c, n, h, w, pad=PAD_REFLECT, act=ACT_ELU, map0=prev_map,
                                    amax0=x_amax, amax_out=slot(4 + i))
-                if skip_done is not None:
-                    torch.cuda.current_stream(dev).wait_event(skip_done)
                 xb = ops.conv_rows(xa, c, wp1, b1, c, n, 2 * h, 2 * w, pad=PAD_REFLECT, act=ACT_ELU, shift0=1,
                                    x1=skip_rows, c1=cs, amax0=slot(4 + i), amax1=skip_amax, amax_out=slot(8 + i))
                 if mlp is None:
@@ -414,12 +386,8 @@ class _WaveDecoderBase(nn.Module):
                     _, pix5, off5 = ops.compact(masks["S5"], want_idxmap=False)
                     head_kw = dict(pixels=pix5, count=off5[n:])
                 prev_map = None
-            ll_in_gemm = i == 4 and self.factored_ll
-            if i == 4 and not ll_in_gemm:
-                wl, bl = self._head_3x3(i, 0)
-                yl = ops.head_conv3x3(t, c // 4, offs[0], wl, bl, n, 2 * h, 2 * w, 1, scale=float(2 ** i),
-                                      act=ACT_SIGMOID, pad=PAD_REFLECT)
-            # +/- heads, factored: per-row tap products on the GEMM engine, then a 9 x 6 float gather-sum per pixel
+            # +/- heads, factored: per-row tap products on the GEMM engine, then a 9 x 6 float gather-sum per pixel.  Level 4's
+            # LL head rides in the same GEMM as nine more tap-product columns (54..62), then a 9-float gather-sum
             wz, bz = self._head_taps(i, offs, c1x1)
             if mlp is not None:
                 z = ops.head_mlp(xb, c, mlp, c1x1, 0.1, count=off4[n:] if sparse else None, max_rows=n * 4 * h * w)
@@ -427,13 +395,13 @@ class _WaveDecoderBase(nn.Module):
                 z = ops.conv_rows(t, c1x1, wz, None, 54, n, 2 * h, 2 * w, taps=1, pixels=pix4, count=off4[n:], m_in0=off4[n:],
                                   amax0=slot(12 + i))
             else:
-                z = ops.conv_rows(t, c1x1, wz, None, 63 if ll_in_gemm else 54, n, 2 * h, 2 * w, taps=1, amax0=slot(12 + i))
-            if ll_in_gemm:
+                z = ops.conv_rows(t, c1x1, wz, None, 63 if i == 4 else 54, n, 2 * h, 2 * w, taps=1, amax0=slot(12 + i))
+            if i == 4:
                 yl = ops.head_gather(z, 1, self.convs[("waveconv", i, 0)][2].conv.bias.detach(), n, 2 * h, 2 * w, 1,
                                      scale=float(2 ** i), act=ACT_SIGMOID, pad=PAD_REFLECT, col0=54)
             next_thresh = None
             epi = ("disp_to_depth",) + tuple(self.depth_range) if (self.depth_range is not None and i == 1) else None
-            if self.fused_tail and (2 * w) % 4 == 0:
+            if one_kernel_tail:
                 tail = ops.head_idwt(z, bz, yl, float(2 ** (i - 1)), 1.0 / 2 ** (i - 1), idxmap=head_kw.get("idxmap"),
                                      mask=masks["S5"] if head_kw else None, pad=PAD_REFLECT, clamp01=True,
                                      thresh_ratio=thresh_ratio if (with_masks and i > 1) else None, epilogue=epi)
@@ -443,7 +411,8 @@ class _WaveDecoderBase(nn.Module):
                     out[("scaled_disp", 0)], out[("depth", 0)] = tail["scaled_disp"], tail["depth"]
             else:
                 if epi is not None:
-                    raise WmdError("depth_range needs the fused tail (fused_tail = True, even width)")
+                    raise WmdError("depth_range needs the fused level tail, which takes coefficient maps whose width is a "
+                                   "multiple of 4 (got %d)" % (2 * w))
                 yh = ops.head_gather(z, 6, bz, n, 2 * h, 2 * w, 3, scale=float(2 ** (i - 1)), act=ACT_SIGMOID, dual=True,
                                      pad=PAD_REFLECT, **head_kw)
                 yl_next, disp = ops.idwt_haar(yl, yh.unsqueeze(1), disp_scale=1.0 / 2 ** (i - 1), clamp01=True)

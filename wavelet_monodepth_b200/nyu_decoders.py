@@ -129,7 +129,7 @@ class _NyuWaveBase(nn.Module):
     def _gemm(self, name, layer, c1=0):
         conv = layer.conv
         # the NYU decoder does not track its sources' maxima, so it runs the tf32x3 operand form: no fp16-pair image
-        return self._packs.get(("gemm", name, ops.default_conv_kind()), [conv.weight],
+        return self._packs.get(("gemm", name), [conv.weight],
                                lambda: ops.pack_weight(conv.weight, c1, precision="tf32x3")), conv.bias.detach()
 
     def _head(self, name, layer):

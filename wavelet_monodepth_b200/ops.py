@@ -372,16 +372,13 @@ def amax_rows(x, out, mask=None):
 
 
 @_on_device
-def nchw_to_rows(x, ld=None, stream=None, gate=None, amax=None, amax_mask=None):
+def nchw_to_rows(x, ld=None, gate=None, amax=None, amax_mask=None):
     """(N,C,H,W) -> rows (N*H*W, ld) pixel-major.  Zero-copy when x is channels_last and C % 4 == 0.
 
     gate: optional uint8 (N,1,H,W) / (N,H,W) mask of the pixels whose rows will be read later: only those rows are
     produced (wmd_nchw_to_rows_gated_f32); the other rows of the result are uninitialised memory.
     With a gate, x may also be a PINNED HOST tensor: the kernel then reads the marked parts of the map straight out of
     host memory (zero-copy over PCIe) - the host->device transfer of a skip map shrinks with the mask density.
-    stream: optional side stream to run the transpose on (it first waits for the current stream, so `x` / `gate` may
-    have been produced there).  Then returns (rows, event): the consumer stream must wait for `event` (None when no
-    kernel was needed).  The output is allocated on the current stream, whose later work is what reads it.
     amax: optional 1-element device tensor raised to max |x| over the pixels the consumer reads: the gate's, else those
     of amax_mask (same form as gate; it restricts only the maximum, every row is still produced), else the whole map.
     So a sparse level's skip map reports one maximum whichever way it is moved (plain, gated, list gather, in place)."""
@@ -410,37 +407,26 @@ def nchw_to_rows(x, ld=None, stream=None, gate=None, amax=None, amax_mask=None):
             rows = x.permute(0, 2, 3, 1).reshape(n * h * w, c)
             if amax is not None:
                 amax_rows(rows, amax, mask=max_mask)
-            return (rows, None) if stream is not None else rows
+            return rows
         x = _dense(x)
     rows = torch.empty((n * h * w, ld), dtype=_f32, device=dev)
-
-    def launch():
-        marked = _pm_count(gate)
-        with _prof('nchw_to_rows', lambda: dict(n=n, c=c, hw=h * w, ld=ld, marked=marked, host=on_host)):
-            if gate is None and amax is not None and max_mask is not None:
-                rc = lib.wmd_nchw_to_rows_masked_amax_f32(_lib.ptr(x), _lib.ptr(rows), _lib.ptr(max_mask), n, c, h * w, ld,
-                                                          _lib.ptr(amax, _f32), _lib.stream_ptr())
-            elif gate is None and amax is not None:
-                rc = lib.wmd_nchw_to_rows_amax_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.ptr(amax, _f32), _lib.stream_ptr())
-            elif gate is None:
-                rc = lib.wmd_nchw_to_rows_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.stream_ptr())
-            elif amax is not None:
-                rc = lib.wmd_nchw_to_rows_gated_amax_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
-                                                         _lib.ptr(amax, _f32), _lib.stream_ptr())
-            else:
-                rc = lib.wmd_nchw_to_rows_gated_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
-                                                    _lib.stream_ptr())
-        _lib.check(rc, "wmd_nchw_to_rows_f32")
-
-    if stream is None:
-        launch()
-        return rows
-    stream.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(stream):
-        launch()
-        done = torch.cuda.Event()
-        done.record(stream)
-    return rows, done
+    marked = _pm_count(gate)
+    with _prof('nchw_to_rows', lambda: dict(n=n, c=c, hw=h * w, ld=ld, marked=marked, host=on_host)):
+        if gate is None and amax is not None and max_mask is not None:
+            rc = lib.wmd_nchw_to_rows_masked_amax_f32(_lib.ptr(x), _lib.ptr(rows), _lib.ptr(max_mask), n, c, h * w, ld,
+                                                      _lib.ptr(amax, _f32), _lib.stream_ptr())
+        elif gate is None and amax is not None:
+            rc = lib.wmd_nchw_to_rows_amax_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.ptr(amax, _f32), _lib.stream_ptr())
+        elif gate is None:
+            rc = lib.wmd_nchw_to_rows_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.stream_ptr())
+        elif amax is not None:
+            rc = lib.wmd_nchw_to_rows_gated_amax_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
+                                                     _lib.ptr(amax, _f32), _lib.stream_ptr())
+        else:
+            rc = lib.wmd_nchw_to_rows_gated_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
+                                                _lib.stream_ptr())
+    _lib.check(rc, "wmd_nchw_to_rows_f32")
+    return rows
 
 
 def _pm_count(gate):
@@ -482,7 +468,9 @@ def gather_rows_list(x, pixels, count, ld=None, stream=None, amax=None):
 
     x: (N,C,H,W) CUDA tensor or PINNED HOST tensor (read in place over PCIe: only the listed pixels cross the bus).
     pixels / count: list + device count from `compact`.  Returns rows (N*H*W capacity, ld); rows past *count are
-    uninitialised.  stream: as in nchw_to_rows (side stream; returns (rows, event))."""
+    uninitialised.  stream: optional side stream to run the gather on (it first waits for the current stream, which
+    produced `pixels` / `count`).  Then returns (rows, event): the consumer stream must wait for `event`.  The output is
+    allocated on the current stream, whose later work is what reads it."""
     lib = _lib.load()
     n, c, h, w = x.shape
     ld = pad4(c) if ld is None else ld
@@ -527,7 +515,7 @@ def scatter_rows(rows, c, pixels, count, n, h, w, max_rows=None, out=None):
     return out
 
 
-def tc_splits(max_rows, cout, nchunks, device, ldy=None):
+def tc_splits(nchunks):
     """Scheduling mode of the tensor-core (wgmma) engine for one launch: 1 = whole tiles, 0 = balanced (data-parallel + stream-K).
 
     At most one CTA per SM runs equal (128-row x N-channel) tiles, so with few tiles per SM the last round is mostly idle
@@ -539,7 +527,7 @@ def tc_splits(max_rows, cout, nchunks, device, ldy=None):
     return 0 if nchunks >= TC_BALANCE_MIN_CHUNKS else 1
 
 
-TC_BALANCE_MIN_CHUNKS = int(__import__("os").environ.get("WMD_TC_BALANCE_MIN_CHUNKS", "80"))
+TC_BALANCE_MIN_CHUNKS = 80
 
 
 class PackedW:
@@ -555,36 +543,23 @@ TC_MIN_K = 128        # shallower reductions (1x1 heads of the fine levels) do n
 TC_MIN_COUT = 32      # tensor-core tiles are 128 x {128, 64, 32}; below that the FMA tiles / head kernel take over
 
 
-def default_conv_precision():
-    """Operand form of the tensor-core engine: env WMD_CONV_PRECISION = f16x3 (default) | tf32x3.
-
-    Both are fp32-faithful error-compensated splits with fp32 accumulation (22 mantissa bits per operand, three MMAs per
-    product).  f16x3 feeds fp16 pairs of power-of-two scaled operands - half the MMA instructions, two thirds of the
-    shared-memory stage - and needs the max |x| of each source (tracked on the device by the producers, see conv_rows
-    amax*); launches that lack it use tf32x3 (the functional kitti_layers API, the NYU decoder, split-K with an external
-    reduction).  The KITTI decoders' step is faster in f16x3 (DESIGN.md 7); tf32x3 stays selectable for A/B runs."""
-    import os
-    return os.environ.get("WMD_CONV_PRECISION", "f16x3")
-
-
-def default_conv_kind():
-    """Engine used when a caller does not ask for one: env WMD_CONV_IMPL = auto | simt | tc.
-
-    auto (default): wgmma tensor cores (operand form: default_conv_precision) for cout >= 32 (every upconv / 1x1 head
-    stage of the decoders), fp32 FMA tiles below."""
-    import os
-    return os.environ.get("WMD_CONV_IMPL", "auto")
-
-
 @_on_device
-def pack_weight(weight, c1=0, kind=None, precision=None):
+def pack_weight(weight, c1=0, kind=None, precision="f16x3"):
     """(Cout,Cin,k,k) conv weight -> PackedW.  c1 = trailing input channels that come from gather source 1.
-    precision ('tc' only): 'f16x3' also builds the fp16-pair image (default: default_conv_precision()).
+
+    kind: 'simt' | 'tc' | 'auto' (None): wgmma tensor cores for cout >= 32 (every upconv / 1x1 head stage of the
+    decoders), fp32 FMA tiles below.
+    precision ('tc' only): 'f16x3' also builds the fp16-pair image, 'tf32x3' does not.  Both operand forms are
+    fp32-faithful error-compensated splits with fp32 accumulation (22 mantissa bits per operand, three MMAs per product).
+    f16x3 feeds fp16 pairs of power-of-two scaled operands - half the MMA instructions, two thirds of the shared-memory
+    stage - and needs the max |x| of each source (tracked on the device by the producers, see conv_rows amax*); launches
+    that lack it run tf32x3 (the functional kitti_layers API, the NYU decoder, split-K with an external reduction).
+    The KITTI decoders' step is faster in f16x3 (DESIGN.md 7), hence the default.
 
     simt: [k*k][Cin][ldw] rows (ldw = pad4(Cout)).  tc: per (n-tile, 32-channel chunk) swizzled smem images
     [tf32 hi | tf32 lo] (chunk boundaries follow the two gather sources, hence c1 matters)."""
     lib = _lib.load()
-    kind = kind or default_conv_kind()
+    kind = kind or "auto"
     wt = _dense(weight.detach())
     cout, cin = wt.shape[0], wt.shape[1]
     taps = wt.shape[2] * wt.shape[3]
@@ -597,7 +572,7 @@ def pack_weight(weight, c1=0, kind=None, precision=None):
         rc = lib.wmd_pack_conv_weight_tc_f32(_lib.ptr(wt), _lib.ptr(packed), cout, c0, c1, taps, _lib.stream_ptr())
         _lib.check(rc, "wmd_pack_conv_weight_tc_f32")
         packed16 = None
-        if (precision or default_conv_precision()) == "f16x3":
+        if precision == "f16x3":
             packed16 = torch.empty((lib.wmd_conv_tc16_weight_bytes(cout, c0, c1, taps),), dtype=_u8, device=wt.device)
             rc = lib.wmd_pack_conv_weight_tc16_f32(_lib.ptr(wt), _lib.ptr(packed16), cout, c0, c1, taps, _lib.stream_ptr())
             _lib.check(rc, "wmd_pack_conv_weight_tc16_f32")
@@ -648,7 +623,7 @@ def conv_rows(x0, c0, wpacked, bias, cout, n, h, w, taps=9, pad=PAD_REFLECT, act
     # amax_out (optional): device scalar raised to max |y|, for the consumers of this layer
     # (the split-K form with an external reduction keeps the tf32 operands: its reduction kernel adds unscaled slabs)
     if wpacked.kind == "tc" and splits is None:
-        splits = tc_splits(max_rows, cout, taps * (-(-c0 // 32) + -(-c1 // 32)), dev, out.shape[1])
+        splits = tc_splits(taps * (-(-c0 // 32) + -(-c1 // 32)))
     use16 = (wpacked.kind == "tc" and wpacked.data16 is not None and amax0 is not None and
              (x1 is None or amax1 is not None) and splits in (0, 1))
     d.precision = _lib.PREC_F16X3 if use16 else _lib.PREC_TF32X3
