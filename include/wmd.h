@@ -340,6 +340,22 @@ int wmd_gather_rows_list_f32(const float* src_nchw, float* rows, int ld, int C, 
 size_t wmd_head_idwt_ws_bytes(int N, int H, int W);
 int wmd_head_idwt_f32(const wmd_head_idwt_desc* d, void* ws, size_t ws_bytes, wmd_stream_t stream);
 
+/* ---------------------------------------------------------------- full-resolution tail of the baseline decoder
+ * ("disp", 0) of monodepth2's DepthDecoder (KITTI/networks/decoders/depth_decoder.py:55-67 at i = 0) in one launch:
+ *   u    = ELU(b1 + conv3x3(up2(x); W1))        upconv(0,1): nearest x2, ZERO padding, 16 -> 16 channels
+ *   disp = sigmoid(b2 + conv3x3(u; W2))         dispconv(0): REFLECT padding (KITTI/layers.py:149), 16 -> cout
+ * x: rows (N*H*W, ld) at half resolution H x W (upconv(0,0)'s output as wmd_conv_rows_f32 writes it: ld >= 16,
+ * ld % 4 == 0, 16-byte aligned); disp: (N, cout, 2H, 2W) NCHW, cout = 1..4; nothing else is written.  u never reaches
+ * memory.  The 16 -> 16 stage runs on tensor cores with the 3xTF32 split (fp32-faithful, fp32 accumulation), the
+ * dispconv in fp32 FMAs.  N = 0 launches nothing.
+ * The weights are packed once by wmd_pack_disp_tail16_f32: w1 (16,16,3,3), b1 (16) or NULL, w2 (cout,16,3,3), b2 (cout)
+ * or NULL -> packed, WMD_DISP_TAIL16_PACKED_FLOATS floats, 16-byte aligned. */
+enum { WMD_DISP_TAIL16_PACKED_FLOATS = 5332 };
+int wmd_pack_disp_tail16_f32(const float* w1, const float* b1, const float* w2, const float* b2, int cout, float* packed,
+                             wmd_stream_t stream);
+int wmd_disp_tail16_f32(const float* x, int ld, const float* packed, int cout, float* disp, int N, int H, int W,
+                        wmd_stream_t stream);
+
 /* ---------------------------------------------------------------- convolution backward (training)
  * The backward of one dense wmd_conv_desc layer (pixels, gate and map1 NULL) y = act(bias + A W), A the gathered rows:
  *

@@ -136,7 +136,10 @@ SIGNATURES = {
     "wmd_conv_wgrad_f32": (c_int, [POINTER(ConvDesc), c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "wmd_conv_dgrad_fold_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
                                         c_void_p, c_void_p]),
+    "wmd_pack_disp_tail16_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "wmd_disp_tail16_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
+DISP_TAIL16_PACKED_FLOATS = 5332          # WMD_DISP_TAIL16_PACKED_FLOATS
 
 _lib = None
 

@@ -1,7 +1,7 @@
 """KITTI depth decoders with the reference's constructor / forward / state-dict contract, on libwmd.
 
 Mirrors KITTI/networks/decoders/depth_decoder.py:
-  * ``DepthDecoder``                       (:18-69)   baseline, API surface only (cuDNN convs)
+  * ``DepthDecoder``                       (:18-69)   monodepth2 baseline decoder
   * ``DepthWaveProgressiveDecoder``        (:72-168)  dense wavelet decoder
   * ``SparseDepthWaveProgressiveDecoder``  (:171-428) threshold-gated sparse decoder
 
@@ -18,7 +18,10 @@ What is different underneath (H100-native, DESIGN.md):
     host sync is one read of the counts at the end for ``total_ops``;
   * training (grad enabled) of the dense decoder runs every convolution forward and backward on libwmd when fp32
     convolutions are requested (torch.backends.cudnn.allow_tf32 False, train_native.py); with TF32 allowed it takes the
-    differentiable cuDNN path.  Both train through the native IDWT with its adjoint.
+    differentiable cuDNN path.  Both train through the native IDWT with its adjoint;
+  * the baseline ``DepthDecoder`` runs the same way: natively at inference (its full-resolution level 0 as one fused
+    kernel, wmd_disp_tail16_f32), natively in training with fp32 convolutions, the cuDNN module graph with TF32 allowed
+    and whenever ``num_output_channels > 4``.
 """
 from collections import OrderedDict
 
@@ -28,7 +31,7 @@ import torch.nn as nn
 
 from . import opcount, ops, train_native
 from .opsfuture import OpsFuture
-from ._lib import ACT_ELU, ACT_LRELU, ACT_SIGMOID, PAD_REFLECT, WmdError
+from ._lib import ACT_ELU, ACT_LRELU, ACT_SIGMOID, PAD_REFLECT, PAD_ZERO, WmdError
 from .kitti_layers import Conv1x1, Conv3x3, ConvBlock, upsample
 from .wavelets import IDWT
 
@@ -98,8 +101,40 @@ def _need_cuda(feats, host_ok=()):
                            "CPU fallback (got a feature map on %s)" % f.device)
 
 
-class DepthDecoder(nn.Module):
-    """monodepth2 baseline decoder (sigmoid disparity at 4 scales).  [depth_decoder.py:18-69]"""
+class _PackedModule(nn.Module):
+    """A decoder that keeps packed copies of its weights for the native engine (see _PackCache)."""
+
+    def _init_packs(self):
+        self._packs = _PackCache()
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packs())
+
+    def invalidate_packs(self):
+        """Drop the packed copies of the weights (they are rebuilt on the next native forward).  Needed only after a
+        weight update the version counters cannot see, e.g. ``p.data.copy_(...)``."""
+        self._packs.invalidate()
+
+    def _apply(self, fn, *args, **kwargs):
+        if hasattr(self, "_packs"):
+            self._packs.invalidate()
+        return super()._apply(fn, *args, **kwargs)
+
+
+def _needs_grad(module, feats):
+    return torch.is_grad_enabled() and (
+        any(p.requires_grad for p in module.parameters()) or any(f.requires_grad for f in feats))
+
+
+class DepthDecoder(_PackedModule):
+    """monodepth2 baseline decoder (sigmoid disparity at 4 scales).  [depth_decoder.py:18-69]
+
+    Same module structure, state dict and outputs as the reference.  Selects its path like the dense wavelet decoder:
+    ``no_grad`` calls run the native engine, grad-enabled calls with fp32 convolutions requested
+    (``torch.backends.cudnn.allow_tf32`` False) run ``train_native.kitti_baseline_forward``, and training with TF32
+    allowed - or any call with ``num_output_channels > 4`` - runs the cuDNN module graph.  The native engine follows
+    the reference's padding: zeros in the ELU ConvBlocks, reflection in the dispconvs (KITTI/layers.py:123,149).
+    Levels finer than the finest requested scale feed no output and are not run."""
+
+    NATIVE_MAX_OUTPUT_CHANNELS = 4         # the dispconv kernels (head_conv3x3, the fused tail) take 1..4 channels
 
     def __init__(self, num_ch_enc, scales=range(4), num_output_channels=1, use_skips=True):
         super().__init__()
@@ -121,8 +156,21 @@ class DepthDecoder(nn.Module):
             self.convs[("dispconv", s)] = Conv3x3(self.num_ch_dec[s], self.num_output_channels)
         self.decoder = nn.ModuleList(list(self.convs.values()))
         self.sigmoid = nn.Sigmoid()
+        self._init_packs()
 
     def forward(self, input_features):
+        needs_grad = _needs_grad(self, input_features)
+        if self.num_output_channels > self.NATIVE_MAX_OUTPUT_CHANNELS or \
+                (needs_grad and not train_native.fp32_convs_requested()):
+            self.outputs = self._autograd_forward(input_features)
+        elif needs_grad:
+            _need_cuda(input_features)
+            self.outputs = train_native.kitti_baseline_forward(self, input_features)
+        else:
+            self.outputs = self._native_forward(input_features)
+        return self.outputs
+
+    def _autograd_forward(self, input_features):
         self.outputs = {}
         x = input_features[-1]
         for i in range(4, -1, -1):
@@ -135,8 +183,76 @@ class DepthDecoder(nn.Module):
                 self.outputs[("disp", i)] = self.sigmoid(self.convs[("dispconv", i)](x))
         return self.outputs
 
+    # ---- native engine ------------------------------------------------------------------------
+    def _upconv(self, i, j):
+        conv = self.convs[("upconv", i, j)].conv.conv
+        c1 = int(self.num_ch_enc[i - 1]) if (j == 1 and self.use_skips and i > 0) else 0
+        return self._packs.get(("upconv", i, j), [conv.weight], lambda: ops.pack_weight(conv.weight, c1)), conv.bias.detach()
 
-class _WaveDecoderBase(nn.Module):
+    def _dispconv(self, s):
+        conv = self.convs[("dispconv", s)].conv
+        return self._packs.get(("dispconv", s), [conv.weight], lambda: ops.pack_head_weight(conv.weight)), conv.bias.detach()
+
+    def _tail(self):
+        """Packed weights of the fused level-0 tail: upconv(0,1) and dispconv(0)."""
+        c1, cd = self.convs[("upconv", 0, 1)].conv.conv, self.convs[("dispconv", 0)].conv
+        return self._packs.get(("tail",), [c1.weight, c1.bias, cd.weight, cd.bias],
+                               lambda: ops.pack_disp_tail16(c1.weight, c1.bias, cd.weight, cd.bias))
+
+    @torch.no_grad()
+    def _native_forward(self, feats):
+        dev = next(f.device for f in feats if f.is_cuda) if any(f.is_cuda for f in feats) else None
+        if dev is not None and dev.index is not None and dev.index != torch.cuda.current_device():
+            with torch.cuda.device(dev):       # libwmd launches on the current device: make the tensors' device current
+                return self._native_forward_on_device(feats)
+        return self._native_forward_on_device(feats)
+
+    def _native_forward_on_device(self, feats):
+        """upconv(i,0) / upconv(i,1) on the gather-GEMM engine, dispconv(s) on head_conv3x3, ("disp", 0) on the fused
+        tail.  Operands in the fp16-pair form with tracked maxima, as in the wavelet engine."""
+        _need_cuda(feats)
+        n = int(feats[-1].shape[0])
+        dev = feats[-1].device
+        h, w = (int(v) for v in feats[4].shape[2:])
+        finest = min(self.scales)
+        cout = int(self.num_output_channels)
+        out = {}
+        if n == 0:
+            for s in self.scales:
+                out[("disp", s)] = torch.zeros((0, cout, h << (5 - s), w << (5 - s)), dtype=torch.float32, device=dev)
+            return out
+        amax = torch.zeros(16, dtype=torch.float32, device=dev)
+
+        def slot(k):
+            return amax[k:k + 1]
+        x_rows, x_c, x_amax = ops.nchw_to_rows(feats[4], amax=slot(0)), int(feats[4].shape[1]), slot(0)
+        for i in range(4, finest - 1, -1):
+            c = int(self.num_ch_dec[i])
+            k = 1 + 3 * (4 - i)
+            wp0, b0 = self._upconv(i, 0)
+            xa = ops.conv_rows(x_rows, x_c, wp0, b0, c, n, h, w, pad=PAD_ZERO, act=ACT_ELU, amax0=x_amax, amax_out=slot(k))
+            if i == 0:
+                # upconv(0,1) -> dispconv(0) -> sigmoid in one kernel: the full-resolution 16-channel map stays on chip
+                out[("disp", 0)] = ops.disp_tail16(xa, self._tail(), cout, n, h, w)
+                break
+            skip_rows, cs = None, 0
+            if self.use_skips:
+                skip = feats[i - 1]
+                if tuple(skip.shape[2:]) != (2 * h, 2 * w):
+                    raise WmdError("skip feature %d has shape %s, expected spatial %s" % (i - 1, tuple(skip.shape), (2 * h, 2 * w)))
+                skip_rows, cs = ops.nchw_to_rows(skip, amax=slot(k + 1)), int(skip.shape[1])
+            wp1, b1 = self._upconv(i, 1)
+            xb = ops.conv_rows(xa, c, wp1, b1, c, n, 2 * h, 2 * w, pad=PAD_ZERO, act=ACT_ELU, shift0=1, x1=skip_rows, c1=cs,
+                               amax0=slot(k), amax1=slot(k + 1) if skip_rows is not None else None, amax_out=slot(k + 2))
+            h, w = 2 * h, 2 * w
+            if i in self.scales:
+                wd, bd = self._dispconv(i)
+                out[("disp", i)] = ops.head_conv3x3(xb, c, 0, wd, bd, n, h, w, cout, act=ACT_SIGMOID, pad=PAD_REFLECT)
+            x_rows, x_c, x_amax = xb, c, slot(k + 2)
+        return out
+
+
+class _WaveDecoderBase(_PackedModule):
     """Shared module structure + native level engine of the two wavelet decoders."""
 
     def _build(self, num_ch_enc, scales, num_output_channels, use_skips):
@@ -164,8 +280,7 @@ class _WaveDecoderBase(nn.Module):
                                                             Conv3x3(c, 3, use_refl=True))
         self.decoder = nn.ModuleList(list(self.convs.values()))
         self.sigmoid = nn.Sigmoid()
-        self._packs = _PackCache()
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packs())
+        self._init_packs()
         # optional fused consumer epilogue (not part of the reference's decoder, off by default): when set to (H, W),
         # inference also returns ("disp_full", s) = F.interpolate(("disp", s), (H, W), mode="bilinear",
         # align_corners=False) for s = 1..3 - what KITTI/trainer.py:338-339 computes from every scale - produced
@@ -190,16 +305,6 @@ class _WaveDecoderBase(nn.Module):
         self.depth_range = None
 
     # ---- packed parameters ------------------------------------------------------------------
-    def invalidate_packs(self):
-        """Drop the packed copies of the weights (they are rebuilt on the next native forward).  Needed only after a
-        weight update the version counters cannot see, e.g. ``p.data.copy_(...)``."""
-        self._packs.invalidate()
-
-    def _apply(self, fn, *args, **kwargs):
-        if hasattr(self, "_packs"):
-            self._packs.invalidate()
-        return super()._apply(fn, *args, **kwargs)
-
     def _upconv(self, i, j):
         conv = self.convs[("upconv", i, j)].conv.conv
         # upconv(i,1) reads the skip map as gather source 1; without skips it reads only the upsampled upconv(i,0)

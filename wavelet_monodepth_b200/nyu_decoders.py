@@ -12,7 +12,8 @@ are the KITTI ones minus the 1x1 branch; they are re-exported from ``kitti_layer
 As for KITTI: inference runs natively and batched in the pixel-major row layout; grad-enabled calls of a non-depthwise
 ``DecoderWave`` or ``DecoderWave224`` (NYUv2/train.py:293-327 trains through them) run every convolution forward and
 backward on libwmd when fp32 convolutions are requested (``torch.backends.cudnn.allow_tf32`` False, train_native.py),
-else the differentiable cuDNN + native-IDWT path.
+else the differentiable cuDNN + native-IDWT path.  The DenseDepth baselines ``Decoder`` and ``Decoder224``
+(densedepth_decoder.py:15-89) select their path the same way; their depthwise variants keep the cuDNN module graph.
 """
 import torch
 import torch.nn as nn
@@ -21,7 +22,7 @@ import torch.nn.functional as F
 from . import opcount, ops, train_native
 from .opsfuture import OpsFuture
 from ._lib import ACT_LRELU, ACT_NONE, PAD_REFLECT, PAD_REPLICATE, PAD_ZERO, WmdError
-from .kitti_decoders import _PackCache, _need_cuda, _pm
+from .kitti_decoders import _PackedModule, _need_cuda, _needs_grad, _pm
 from .kitti_layers import (make_result, mask2idxmap, mask2yx, sparse_conv3x3, sparse_select,  # noqa: F401
                            sparse_upsample)
 from .wavelets import IDWT
@@ -83,7 +84,21 @@ class UpSampleBlock(nn.Sequential):
         return self.leakyreluA(self.convA(torch.cat([self.upsample(x), concat_with], dim=1)))
 
 
-class _NyuWaveBase(nn.Module):
+class _NyuPacks(_PackedModule):
+    """Packed weights of the NYU engines.  The NYU decoders do not track their sources' maxima, so their tensor-core
+    convolutions run the tf32x3 operand form: no fp16-pair image."""
+
+    def _gemm(self, name, layer, c1=0):
+        conv = layer.conv
+        return self._packs.get(("gemm", name), [conv.weight],
+                               lambda: ops.pack_weight(conv.weight, c1, precision="tf32x3")), conv.bias.detach()
+
+    def _head(self, name, layer):
+        conv = layer.conv
+        return self._packs.get(("head", name), [conv.weight], lambda: ops.pack_head_weight(conv.weight)), conv.bias.detach()
+
+
+class _NyuWaveBase(_NyuPacks):
     # Level table of the native engine and of the native training forward (train_native.nyu_forward).
     # _LL_HEAD: (LL scale, k) - LL = scale * wave1_ll(up1 output), and ("disp", k) is the raw LL head (k None: no such
     # output).  _LEVELS: one (j, s, disp) per IDWT level, coarse to fine: the level reads up<j>'s output (up1 for j = 1,
@@ -114,27 +129,7 @@ class _NyuWaveBase(nn.Module):
         # optional consumer epilogue of ("disp", 0), off by default: (div, lo, hi) adds ("depth", 0) =
         # clamp(("disp", 0) / div, lo, hi) - NYUv2/utils.py:219,229 uses (100, 0.4, 10) - fused into the last IDWT
         self.depth_epilogue = None
-        self._packs = _PackCache()
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packs())
-
-    def invalidate_packs(self):
-        """Drop the packed weight copies (see kitti_decoders._PackCache)."""
-        self._packs.invalidate()
-
-    def _apply(self, fn, *args, **kwargs):
-        if hasattr(self, "_packs"):
-            self._packs.invalidate()
-        return super()._apply(fn, *args, **kwargs)
-
-    def _gemm(self, name, layer, c1=0):
-        conv = layer.conv
-        # the NYU decoder does not track its sources' maxima, so it runs the tf32x3 operand form: no fp16-pair image
-        return self._packs.get(("gemm", name), [conv.weight],
-                               lambda: ops.pack_weight(conv.weight, c1, precision="tf32x3")), conv.bias.detach()
-
-    def _head(self, name, layer):
-        conv = layer.conv
-        return self._packs.get(("head", name), [conv.weight], lambda: ops.pack_head_weight(conv.weight)), conv.bias.detach()
+        self._init_packs()
 
     def _forward(self, x_blocks):
         """Dense decoders: the cuDNN module graph for depthwise variants and for training with TF32 allowed, the native
@@ -334,11 +329,15 @@ class SparseDecoderWave(_NyuWaveBase):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# API surface outside the hot path (SURVEY 8b lists them as constructible from NYUv2/model.py:47-64): the DenseDepth
-# baseline decoders.  They run on the differentiable cuDNN path; no native gather-GEMM engine is built for them.
+# The DenseDepth baseline decoders (NYUv2/model.py:47-64 builds them without --use_wavelets).
 # ------------------------------------------------------------------------------------------------------------------
-class _BaselineDecoder(nn.Module):
-    """conv2 -> four UpSampleBlocks -> [x2 + conv5 + LeakyReLU(0.2)] -> conv3; zero padding everywhere."""
+class _BaselineDecoder(_NyuPacks):
+    """conv2 -> four UpSampleBlocks -> [x2 + conv5 + LeakyReLU(0.2)] -> conv3; zero padding everywhere.
+
+    ``no_grad`` calls run the native engine: conv2, up1..up4 and conv5 on the gather-GEMM engine (tf32x3 operands),
+    conv3 on head_conv3x3.  Grad-enabled calls with fp32 convolutions requested (``torch.backends.cudnn.allow_tf32``
+    False) run ``train_native.nyu_baseline_forward``.  Training with TF32 allowed and the depthwise variants run the cuDNN
+    module graph."""
 
     def _build(self, enc_features, decoder_width, is_depthwise, extra_stage):
         f = int(enc_features[-1] * decoder_width)
@@ -358,11 +357,59 @@ class _BaselineDecoder(nn.Module):
         if extra_stage:
             self.upsample = nn.Upsample(scale_factor=2, mode="nearest")
         self._extra_stage = extra_stage
+        self._depthwise = bool(is_depthwise)
+        self._init_packs()
 
     def forward(self, features):
         blocks = tuple(features)
         if len(blocks) != 5:
             raise ValueError("expected the five encoder blocks, fine to coarse")
+        needs_grad = _needs_grad(self, blocks)
+        if self._depthwise or (needs_grad and not train_native.fp32_convs_requested()):
+            return self._autograd_forward(blocks)
+        _need_cuda(blocks)
+        if needs_grad:
+            return train_native.nyu_baseline_forward(self, blocks)
+        return self._native_forward(blocks)
+
+    @torch.no_grad()
+    def _native_forward(self, blocks):
+        dev = blocks[-1].device
+        if dev.index is not None and dev.index != torch.cuda.current_device():
+            with torch.cuda.device(dev):       # libwmd launches on the current device
+                return self._native_forward_on_device(blocks)
+        return self._native_forward_on_device(blocks)
+
+    def _native_forward_on_device(self, blocks):
+        xb = blocks[4]
+        n, c, h, w = (int(v) for v in xb.shape)
+        up = 32 if self._extra_stage else 16
+        if n == 0:
+            return {("disp", 0): torch.zeros((0, 1, up * h, up * w), dtype=torch.float32, device=xb.device)}
+        wp, b = self._gemm("conv2", self.conv2)
+        f = int(self.conv2.conv.weight.shape[0])
+        d = ops.conv_rows(ops.nchw_to_rows(xb), c, wp, b, f, n, h, w, pad=PAD_ZERO, act=ACT_NONE)
+        c = f
+        for k in range(1, 5):
+            skip = blocks[4 - k]
+            if tuple(skip.shape[2:]) != (2 * h, 2 * w):
+                raise WmdError("skip block has shape %s, expected spatial %s" % (tuple(skip.shape), (2 * h, 2 * w)))
+            conv = getattr(self, "up%d" % k).convA
+            cout = int(conv.conv.weight.shape[0])
+            wp, b = self._gemm("up%d" % k, conv, int(skip.shape[1]))
+            d = ops.conv_rows(d, c, wp, b, cout, n, 2 * h, 2 * w, pad=PAD_ZERO, act=ACT_LRELU, act_param=0.2, shift0=1,
+                              x1=ops.nchw_to_rows(skip), c1=int(skip.shape[1]))
+            c, h, w = cout, 2 * h, 2 * w
+        if self._extra_stage:
+            cout = int(self.conv5[0].conv.weight.shape[0])
+            wp, b = self._gemm("conv5", self.conv5[0])
+            d = ops.conv_rows(d, c, wp, b, cout, n, 2 * h, 2 * w, pad=PAD_ZERO, act=ACT_LRELU, act_param=0.2, shift0=1)
+            c, h, w = cout, 2 * h, 2 * w
+        w3 = self._packs.get(("head", "conv3"), [self.conv3.weight], lambda: ops.pack_head_weight(self.conv3.weight))
+        return {("disp", 0): ops.head_conv3x3(d, c, 0, w3, self.conv3.bias.detach(), n, h, w, 1, act=ACT_NONE,
+                                              pad=PAD_ZERO)}
+
+    def _autograd_forward(self, blocks):
         x = self.conv2(blocks[4])
         for k in range(1, 5):
             x = getattr(self, "up%d" % k)(x, blocks[4 - k])

@@ -763,6 +763,41 @@ def pack_head_mlp(w1, b1, wz):
 
 
 @_on_device
+def pack_disp_tail16(w1, b1, w2, b2):
+    """upconv(0,1)'s (16, 16, 3, 3) weight and bias, dispconv(0)'s (cout <= 4, 16, 3, 3) weight and bias -> the packed
+    image of disp_tail16 (wmd_pack_disp_tail16_f32)."""
+    lib = _lib.load()
+    w1, w2 = _dense(w1.detach()), _dense(w2.detach())
+    cout = int(w2.shape[0])
+    if tuple(w1.shape) != (16, 16, 3, 3) or tuple(w2.shape[1:]) != (16, 3, 3) or not 1 <= cout <= 4:
+        raise _lib.WmdError("pack_disp_tail16: needs W1 (16, 16, 3, 3) and W2 (1..4, 16, 3, 3), got %s and %s"
+                            % (tuple(w1.shape), tuple(w2.shape)))
+    packed = torch.empty((_lib.DISP_TAIL16_PACKED_FLOATS,), dtype=_f32, device=w1.device)
+    b1 = _dense(b1.detach()) if b1 is not None else None
+    b2 = _dense(b2.detach()) if b2 is not None else None
+    rc = lib.wmd_pack_disp_tail16_f32(_lib.ptr(w1), _lib.ptr(b1), _lib.ptr(w2), _lib.ptr(b2), cout, _lib.ptr(packed),
+                                      _lib.stream_ptr())
+    _lib.check(rc, "wmd_pack_disp_tail16_f32")
+    return packed
+
+
+@_on_device
+def disp_tail16(x, packed, cout, n, h, w, out=None):
+    """("disp", 0) of the baseline KITTI decoder from upconv(0,0)'s rows x (N*h*w, ld >= 16) at half resolution:
+    sigmoid(dispconv(0)(ELU(upconv(0,1)(up2(x))))) -> (N, cout, 2h, 2w); see wmd_disp_tail16_f32."""
+    lib = _lib.load()
+    if out is None:
+        out = torch.empty((n, cout, 2 * h, 2 * w), dtype=_f32, device=x.device)
+    if n == 0:
+        return out
+    with _prof('disp_tail16', lambda: dict(n=n, h=h, w=w, cout=cout)):
+        rc = lib.wmd_disp_tail16_f32(_lib.ptr(x, _f32), x.shape[1], _lib.ptr(packed, _f32), cout, _lib.ptr(out, _f32), n, h, w,
+                                     _lib.stream_ptr())
+    _lib.check(rc, "wmd_disp_tail16_f32")
+    return out
+
+
+@_on_device
 def head_mlp(x, c, packed, n1, slope=0.1, count=None, max_rows=None, nz=54):
     """z (max_rows, 56) = Wz . lrelu(W1 . x + b1) on pixel-major rows x (R, ld >= c); see wmd_head_mlp_f32."""
     lib = _lib.load()

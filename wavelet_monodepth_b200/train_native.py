@@ -1,4 +1,5 @@
-"""Native training step of the dense wavelet decoders: every convolution runs forward and backward on libwmd.
+"""Native training step of the dense wavelet decoders and the baseline decoders: every convolution runs forward and
+backward on libwmd.
 
 Selected by the decoders for a grad-enabled call when ``torch.backends.cudnn.allow_tf32`` is False, which is how a PyTorch
 user asks for fp32 convolutions; with TF32 allowed they keep the cuDNN path.  Each decoder convolution is one
@@ -6,7 +7,8 @@ user asks for fp32 convolutions; with TF32 allowed they keep the cuDNN path.  Ea
 form), its backward the activation backward with the bias gradient, the tensor-core weight gradient and the data gradient
 (the forward engine over the ring-extended grid plus the fold).  The glue stays torch autograd: NCHW <-> rows moves (the
 reverse move is the adjoint), the power-of-two scalings and the sigma difference, the native IDWT, the clamp.  The fused
-inference kernels (head_mlp, head_idwt) are not used: they do not keep the intermediates a backward needs.
+inference kernels (head_mlp, head_idwt, the baseline's disp_tail16) are not used: they do not keep the intermediates a
+backward needs.
 """
 import torch
 import torch.nn.functional as F
@@ -209,3 +211,46 @@ def nyu_forward(dec, blocks):
         else:
             out[("disp", s)] = ll / 2 ** s if s else ll
     return out
+
+
+def kitti_baseline_forward(dec, feats):
+    """DepthDecoder's outputs with every convolution on libwmd, differentiable: ELU ConvBlocks with zero padding,
+    reflection-padded dispconvs with the sigmoid in their epilogue.  Levels finer than the finest requested scale are
+    not run (no output depends on them)."""
+    out = {}
+    n = int(feats[-1].shape[0])
+    h, w = (int(v) for v in feats[4].shape[2:])
+    x, x_amax = to_rows(feats[4])
+    cout = int(dec.num_output_channels)
+    for i in range(4, min(dec.scales) - 1, -1):
+        conv0 = dec.convs[("upconv", i, 0)].conv.conv
+        conv1 = dec.convs[("upconv", i, 1)].conv.conv
+        xa, a_amax = conv(x, x_amax, None, conv0.weight, conv0.bias, n, h, w, pad=PAD_ZERO, act=ACT_ELU)
+        skip = feats[i - 1] if (dec.use_skips and i > 0) else None
+        x, x_amax = conv(xa, a_amax, skip, conv1.weight, conv1.bias, n, 2 * h, 2 * w, pad=PAD_ZERO, act=ACT_ELU, shift0=1)
+        h, w = 2 * h, 2 * w
+        if i in dec.scales:
+            d = dec.convs[("dispconv", i)].conv
+            z, _ = conv(x, x_amax, None, d.weight, d.bias, n, h, w, pad=PAD_REFLECT, act=ACT_SIGMOID)
+            out[("disp", i)] = to_nchw(z, n, cout, h, w)
+    return out
+
+
+def nyu_baseline_forward(dec, blocks):
+    """Decoder's / Decoder224's ("disp", 0) with every convolution on libwmd, differentiable (zero padding throughout)."""
+    n, _, h, w = (int(v) for v in blocks[4].shape)
+    x, x_amax = to_rows(blocks[4])
+    c = dec.conv2.conv
+    x, x_amax = conv(x, x_amax, None, c.weight, c.bias, n, h, w, pad=PAD_ZERO)
+    for k in range(1, 5):
+        c = getattr(dec, "up%d" % k).convA.conv
+        x, x_amax = conv(x, x_amax, blocks[4 - k], c.weight, c.bias, n, 2 * h, 2 * w, pad=PAD_ZERO, act=ACT_LRELU,
+                         act_param=0.2, shift0=1)
+        h, w = 2 * h, 2 * w
+    if dec._extra_stage:
+        c = dec.conv5[0].conv
+        x, x_amax = conv(x, x_amax, None, c.weight, c.bias, n, 2 * h, 2 * w, pad=PAD_ZERO, act=ACT_LRELU, act_param=0.2,
+                         shift0=1)
+        h, w = 2 * h, 2 * w
+    z, _ = conv(x, x_amax, None, dec.conv3.weight, dec.conv3.bias, n, h, w, pad=PAD_ZERO)
+    return {("disp", 0): to_nchw(z, n, 1, h, w)}
