@@ -208,7 +208,11 @@ int wmd_conv_rows_f32(const wmd_conv_desc* d, wmd_stream_t stream);
  *                                            shared-memory images [tf32 hi | tf32 lo] of N x 32, K-major, 128-byte swizzled
  * Accumulation runs in epochs of K = 1024 in the wgmma accumulators, each added into fp32 registers with
  * round-to-nearest adds, because the tensor core's own fp32 accumulation does not round to nearest (a one-signed bias of
- * ~1.6e-8 * K of S in tf32x3, ~8.5e-9 * K in f16x3, measured on H100: it stays that of one epoch, not of the whole K). */
+ * ~1.6e-8 * K of S in tf32x3, ~8.5e-9 * K in f16x3, measured on H100: it stays that of one epoch, not of the whole K).
+ * Dense 3x3 launches (no pixels, map0, map1 or gate; splits 0 or 1) whose per-tile source windows fit 288 rows (output
+ * width W <= 79 with a full-resolution source; W <= 192 when the only source is x0 with shift0 = 1) run in a second
+ * kernel, conv_rows_tc_kernel_window, that loads each source's window of rows once per 32-channel chunk instead of once
+ * per tap; the results are bit-identical to the gather kernel's. */
 enum { WMD_PREC_TF32X3 = 0, WMD_PREC_F16X3 = 1 };
 int wmd_conv_tc_tile_n(int cout);
 /* Weights for precision = WMD_PREC_F16X3: 128-byte header (float 0: 1 / s_w) + per (n-tile, 32-channel chunk) one N x 128 B

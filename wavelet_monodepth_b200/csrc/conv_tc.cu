@@ -79,6 +79,51 @@ struct TcCfg {
   static_assert(STAGES >= 2, "the ring needs two stages");
   static_assert(SMEM <= TC_SMEM_MAX, "one CTA must fit the shared memory of an SM");
 };
+// Window mode (conv_rows_tc_kernel_window): a dense 3x3 layer (no pixel list, no index maps, no gate) reads, for one tile
+// and one source, a CONTIGUOUS range of source rows, and every tap's rows lie inside it.  So the producer loads that
+// range's 32-channel slices once per channel chunk into a window slot, and the consumers read tap `t` of tile row r at
+// window row tab[t][r] (a window-relative uint16 table that travels with the slot); the nine taps stop fetching (and
+// storing) the same rows nine times.  Window of a 128-row tile starting at output row m0, for an output width W (pad
+// modes keep every tap within one row / column of its pixel, inside the image):
+//   shift 0 (x1, and x0 at full resolution): the tap rows of output row m lie in [m - W - 1, m + W + 1], so the window
+//     is [m0 - W - 1, m0 + 127 + W + 1]: 128 + 2 (W + 1) rows;
+//   shift 1 (x0 at half resolution, Ws = W / 2, H even): output row Y (global, n H + y) reads source rows
+//     ((Y - 1) >> 1) .. ((Y + 1) >> 1), any column.  A tile spans output rows Y0 .. Y0 + D with D <= (W + 126) / W
+//     (128 pixels from any column), so the window is the whole source rows ((Y0 - 1) >> 1) .. ((Y0 + D + 1) >> 1): at
+//     most ((D + 1) >> 1) + 2 rows of Ws (the count for Y0 even; Y0 odd gives (D >> 1) + 2), starting at
+//     ((Y0 - 1) >> 1) Ws.
+// Slots hold TC_WIN_ROWS rows plus one row of zeros (padded taps and dead rows point at it); a launch whose window is
+// larger keeps the gather path.
+constexpr int TC_WIN_ROWS = 288;                                   // shift 0: W <= 79
+constexpr int TC_WIN_DATA = (TC_WIN_ROWS + 1) * TC_A_LD * 4;       // rows + the zero row, 144-byte pitch
+constexpr int TC_WIN_TAB = 9 * TC_BM * 2;                          // [tap][row] uint16 window rows
+constexpr int TC_WIN_SLOT = TC_WIN_DATA + TC_WIN_TAB;
+static_assert(TC_WIN_DATA % 16 == 0 && TC_WIN_SLOT % 16 == 0, "window rows take 16-byte cp.async");
+__host__ __device__ __forceinline__ int win_rows(int W, int shift) {
+  if (shift == 0) return TC_BM + 2 * (W + 1);
+  const int D = (W + TC_BM - 2) / W;
+  return (((D + 1) >> 1) + 2) * (W >> 1);
+}
+__host__ __device__ __forceinline__ int win_base(int m0, int W, int shift) {
+  if (shift == 0) return m0 - (W + 1);
+  const int Y0 = m0 / W;
+  return (Y0 > 0 ? (Y0 - 1) >> 1 : -1) * (W >> 1);
+}
+
+// Window mode: a ring of weight-only stages beside two window slots, the producer's tap tables, the barriers (full[s],
+// empty[s] of the ring, then full / empty of the two slots) and the alignment slack: 4 stages for tf32 N = 128, 8 for
+// the rest.
+template <int BN, bool F16>
+struct TcWinCfg {
+  static constexpr int B_IMG = TcCfg<BN, F16>::B_IMG;
+  static constexpr int FIXED = 2 * TC_WIN_SLOT + TC_TABLES + 4 * 8 + 1024;
+  static constexpr int FIT = (TC_SMEM_MAX - FIXED) / (B_IMG + 2 * 8);
+  static constexpr int STAGES = FIT < TC_MAX_STAGES ? FIT : TC_MAX_STAGES;
+  static constexpr size_t SMEM = static_cast<size_t>(STAGES) * B_IMG + FIXED + 2 * STAGES * 8;
+  static_assert(STAGES >= 2, "the ring needs two stages");
+  static_assert(SMEM <= TC_SMEM_MAX, "one CTA must fit the shared memory of an SM");
+};
+
 constexpr int kFlushChunks = 32;                // epoch length: K = 1024 per wgmma accumulation run
 static_assert(kFlushChunks % 2 == 0, "an epoch starts on register set 0");
 constexpr int32_t kNoRow = -1;                  // tap-table entry of an inactive / padded source: the gather writes zeros
@@ -359,15 +404,17 @@ struct TcWalk {
 template <int V>
 struct Ic { static constexpr int value = V; };   // a compile-time register-set index
 
-template <int BN, bool F16>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_conv_desc d, const float* __restrict__ wtc,
-                                                                     const int splits, float* __restrict__ partial) {
+// WIN: window mode (dense 3x3 layers, see TC_WIN_ROWS): stages hold weights only, A comes from the window slots.
+template <int BN, bool F16, bool WIN>
+__device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const float* __restrict__ wtc, const int splits,
+                                                  float* __restrict__ partial) {
   using Cfg = TcCfg<BN, F16>;
   constexpr int TC_B_TILE = Cfg::B_TILE;
   constexpr int B_IMG = Cfg::B_IMG;                         // bytes of one chunk's weight image
   constexpr int ACC = Cfg::ACC;
-  constexpr int STAGE = Cfg::STAGE;
-  constexpr int STAGES = Cfg::STAGES;
+  constexpr int STAGE = WIN ? B_IMG : Cfg::STAGE;
+  constexpr int STAGES = WIN ? TcWinCfg<BN, F16>::STAGES : Cfg::STAGES;
+  constexpr int SLOTS = WIN ? 2 * TC_WIN_SLOT : 0;
   extern __shared__ unsigned char smem_dyn[];
   __shared__ int s_fixup;                                  // balanced mode: segments of the tile to reduce here (0 = not the last)
 
@@ -376,10 +423,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   // diverge inside a warp, and are not serialised
   const int warpgroup = __shfl_sync(0xffffffffu, tid / 128, 0);
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~static_cast<uintptr_t>(1023));
-  int32_t* tab0 = reinterpret_cast<int32_t*>(base + STAGES * STAGE);      // [tap][row]: source row in x0, -1 = none
+  unsigned char* wslot = base + STAGES * STAGE;                            // window slots j = 0, 1: rows, then the table
+  int32_t* tab0 = reinterpret_cast<int32_t*>(base + STAGES * STAGE + SLOTS);   // [tap][row]: source row in x0, -1 = none
   int32_t* tab1 = tab0 + 9 * TC_BM;                                        // ... in x1
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * STAGE + TC_TABLES);      // stage s holds its chunk
+  uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * STAGE + SLOTS + TC_TABLES);   // stage s holds its chunk
   uint64_t* empty = full + STAGES;                                                       // both consumers are done with s
+  uint64_t* wfull = empty + STAGES;                        // window mode: slot j holds its channel chunk's rows and table
+  uint64_t* wempty = wfull + 2;                            // ... every consumer warp has read slot j for the last time
 
   const long long HW = static_cast<long long>(d.H) * d.W;
   const int total_px = static_cast<int>(static_cast<long long>(d.N) * HW);
@@ -398,10 +448,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
   if (tid == 0) {
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full + s, TC_PRODUCERS + 1);               // every producer thread's copies + the weight image's bytes
+      mbar_init(full + s, WIN ? 1 : TC_PRODUCERS + 1);     // every producer thread's copies (gather) + the weight image's bytes
       mbar_init(empty + s, TC_CONSUMERS / 32);             // one arrival per consumer warp
     }
+    if (WIN) {
+      for (int j = 0; j < 2; ++j) {
+        // two arrivals per producer thread: its copies (noinc) and a plain arrive that releases its table stores
+        mbar_init(wfull + j, 2 * TC_PRODUCERS);
+        mbar_init(wempty + j, TC_CONSUMERS / 32);
+      }
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  if (WIN && tid < 2 * TC_A_LD) {                          // the zero row of each slot, never overwritten
+    const int j = tid / TC_A_LD;
+    reinterpret_cast<float*>(wslot + j * TC_WIN_SLOT)[TC_WIN_ROWS * TC_A_LD + tid % TC_A_LD] = 0.f;
   }
   __syncthreads();
 
@@ -415,6 +476,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     const long long rows_x1 = static_cast<long long>(d.N) * HW;
     const unsigned char* wimg = reinterpret_cast<const unsigned char*>(wtc) + (F16 ? 128 : 0);   // f16 images follow a 128-byte header
     uint32_t g = 0;                                        // chunks this CTA has issued: stage g % STAGES, use g / STAGES
+    uint32_t wi = 0;                                       // window mode: windows issued: slot wi & 1, use wi >> 1
     while (walk.next(it)) {
       const int m0 = static_cast<int>(it.tile / n_tiles) * TC_BM;
       const int nt = static_cast<int>(it.tile % n_tiles);
@@ -497,13 +559,47 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
           mbar_arrive_expect_tx(full + s, B_IMG);
           bulk_copy_g2s(st, wtile + static_cast<long long>(c) * B_IMG, B_IMG, full + s);
         }
-        const int rr = c / d.taps;
-        const int tap = c - rr * d.taps;
+        const int taps = WIN ? 9 : d.taps;
+        const int rr = c / taps;
+        const int tap = c - rr * taps;
         const bool src1 = rr >= nch0;
         const int col = (src1 ? rr - nch0 : rr) * TC_BK;
         const float* x = src1 ? d.x1 : d.x0;
         const long long ld = src1 ? d.ld1 : d.ld0;
         const int csrc = src1 ? d.c1 : d.c0;
+        if constexpr (WIN) {
+          // A channel chunk's first step in this segment (a stream-K segment may start at any tap) loads its window
+          // into the next slot: the table made window-relative, then the rows, zero filled as the gather does.
+          if (c != it.cb && tap != 0) continue;
+          const int j = static_cast<int>(wi & 1);
+          if (wi >= 2) mbar_wait(wempty + j, ((wi >> 1) - 1) & 1);
+          float* sw = reinterpret_cast<float*>(wslot + j * TC_WIN_SLOT);
+          uint16_t* wt = reinterpret_cast<uint16_t*>(wslot + j * TC_WIN_SLOT + TC_WIN_DATA);
+          const int shift = src1 ? 0 : d.shift0;
+          const int wb = win_base(m0, d.W, shift), wn = win_rows(d.W, shift);
+          const long long nrows = src1 ? rows_x1 : rows_x0;
+          const int32_t* tab = src1 ? tab1 : tab0;
+#pragma unroll
+          for (int t = 0; t < 9; ++t) {
+            const int32_t a = tab[t * TC_BM + tid];
+            const int o = a - wb;
+            wt[t * TC_BM + tid] = static_cast<uint16_t>(a != kNoRow && o >= 0 && o < wn ? o : TC_WIN_ROWS);
+          }
+#pragma unroll 1
+          for (int pc = tid; pc < wn * 8; pc += TC_PRODUCERS) {
+            const int r = pc >> 3, q = pc & 7;
+            const long long srow = static_cast<long long>(wb) + r;
+            const int cc = col + 4 * q;
+            const int bytes = (srow >= 0 && srow < nrows) ? min(16, max(0, (csrc - cc) * 4)) : 0;
+            cp_async16(sw + r * TC_A_LD + 4 * q, bytes ? x + srow * ld + cc : x, bytes);
+          }
+          // cp.async's arrival tracks only its copies; the plain arrive (release) publishes this thread's table stores
+          // to the consumers' wait (acquire)
+          cp_async_mbar_arrive(wfull + j);
+          mbar_arrive(wfull + j);
+          ++wi;
+          continue;
+        }
         const int32_t* tab = (src1 ? tab1 : tab0) + tap * TC_BM;
         float* sa = reinterpret_cast<float*>(st + B_IMG);
 #pragma unroll
@@ -560,12 +656,30 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
 #pragma unroll
   for (int j = 0; j < ACC; ++j) dacc[j] = 0.f;
 
-  // wait for stage gi % STAGES to hold chunk gi, then read this thread's fragment elements into register set B
-  auto load_frag = [&](auto B, uint32_t gi) {
+  // Window mode: chunk c of a segment that starts at chunk cb reads window number wc + c / 9 - cb / 9 (wc: windows this
+  // CTA consumed in earlier segments), slot (that number) & 1.
+  uint32_t wc = 0;
+  int seg_cb = 0;
+  auto win_of = [&](int i) { return wc + static_cast<uint32_t>((seg_cb + i) / 9 - seg_cb / 9); };
+
+  // wait for stage gi % STAGES to hold chunk gi (and in window mode, at the chunk's first step of the segment, for its
+  // window), then read this thread's fragment elements (chunk i of the segment) into register set B
+  auto load_frag = [&](auto B, uint32_t gi, int i) {
     constexpr int b = decltype(B)::value;
     const int s = static_cast<int>(gi % STAGES);
     mbar_wait(full + s, (gi / STAGES) & 1);
     const float* sa = reinterpret_cast<const float*>(base + s * STAGE + B_IMG);
+    int pr0 = row_a * TC_A_LD, pr1 = (row_a + 8) * TC_A_LD;   // float offsets of this thread's two fragment rows
+    if constexpr (WIN) {
+      const uint32_t wn = win_of(i);
+      const int j = static_cast<int>(wn & 1);
+      const int tap = (seg_cb + i) % 9;
+      if (i == 0 || tap == 0) mbar_wait(wfull + j, (wn >> 1) & 1);
+      sa = reinterpret_cast<const float*>(wslot + j * TC_WIN_SLOT);
+      const uint16_t* wt = reinterpret_cast<const uint16_t*>(wslot + j * TC_WIN_SLOT + TC_WIN_DATA) + tap * TC_BM;
+      pr0 = wt[row_a] * TC_A_LD;
+      pr1 = wt[row_a + 8] * TC_A_LD;
+    }
     if (F16) {
       // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
       // precision of the tf32 hi / lo pair.  Fragment of k-step ks: rows (r, r + 8) x channels 16 ks + 2 t4 + {0, 1}, + 8
@@ -573,7 +687,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       for (int ks = 0; ks < KS; ++ks) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const float2 v = *reinterpret_cast<const float2*>(sa + (row_a + (e & 1) * 8) * TC_A_LD + ks * 16 + 2 * t4 + (e >> 1) * 8);
+          const float2 v = *reinterpret_cast<const float2*>(sa + ((e & 1) ? pr1 : pr0) + ks * 16 + 2 * t4 + (e >> 1) * 8);
           const float b0f = v.x * ascale, b1f = v.y * ascale;
           const uint32_t p = pack_f16x2(b0f, b1f);
           fa[b][ks][e] = p;
@@ -586,7 +700,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       for (int ks = 0; ks < KS; ++ks) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const float v = sa[(row_a + (e & 1) * 8) * TC_A_LD + ks * 8 + t4 + (e >> 1) * 4];
+          const float v = sa[((e & 1) ? pr1 : pr0) + ks * 8 + t4 + (e >> 1) * 4];
           fa[b][ks][e] = __float_as_uint(v) & 0xFFFFE000u;
           fb[b][ks][e] = __float_as_uint(v - __uint_as_float(fa[b][ks][e]));
         }
@@ -643,15 +757,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
         }
       }
       wgmma_commit();
+      if constexpr (WIN) {
+        // chunk i's fragments are in registers (its MMAs are issued): after its channel chunk's last step in this
+        // segment, the window slot goes back to the producer
+        if ((seg_cb + i) % 9 == 8 || i + 1 == len) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(wempty + (win_of(i) & 1));
+        }
+      }
       wgmma_wait<1>();                                     // chunk i - 1 has retired
       fence_frag(Ic<1 - b>());
       if (i > 0) release(gi - 1);
-      if (i + 1 < len) load_frag(Ic<1 - b>(), gi + 1);
+      if (i + 1 < len) load_frag(Ic<1 - b>(), gi + 1, i + 1);
     };
     // Epochs of kFlushChunks chunks counted from the segment start (even: chunk i always uses register set i % 2).  The
     // accumulators are read only after an epoch's last group has retired, outside any branch, so the compiler keeps the
     // wgmma of the epoch asynchronous.
-    load_frag(Ic<0>(), g);
+    seg_cb = it.cb;
+    load_frag(Ic<0>(), g, 0);
 #pragma unroll 1
     for (int e0 = 0; e0 < len; e0 += kFlushChunks) {
       const int e1 = min(len, e0 + kFlushChunks);
@@ -670,6 +793,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
     }
     release(g + len - 1);
     g += len;
+    if (WIN) wc = win_of(len - 1) + 1;
 
     // ---- epilogue: bias, activation, pair stores.  acc[4 j + 2 h + e] = row row_a + 8 h, column 8 j + 2 t4 + e
 #pragma unroll
@@ -824,6 +948,20 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_c
       if (lane == 0 && out_max > __ldcg(d.amax_out)) atomicMax(reinterpret_cast<unsigned*>(d.amax_out), __float_as_uint(out_max));   // most warps skip the atomic
     }
   }
+}
+
+// Two kernels with their own names, so that a profile tells them apart; the window form's name extends the gather
+// form's, so a search for the tensor-core engine by name finds both.  The window form runs the dense 3x3 launches whose
+// windows fit (tc_window_fits), the gather form every other launch.  Both give the same bits.
+template <int BN, bool F16>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_conv_desc d, const float* __restrict__ wtc,
+                                                                     const int splits, float* __restrict__ partial) {
+  conv_rows_tc_body<BN, F16, false>(d, wtc, splits, partial);
+}
+template <int BN, bool F16>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel_window(const wmd_conv_desc d, const float* __restrict__ wtc,
+                                                                         const int splits, float* __restrict__ partial) {
+  conv_rows_tc_body<BN, F16, true>(d, wtc, splits, partial);
 }
 
 // w (Cout, Cin, taps) fp32 -> per (n-tile, chunk) smem image [tf32 hi: BN x 32 | tf32 lo: BN x 32], K-major,
@@ -1026,22 +1164,29 @@ static int tc_tile_n(int cout) { return cout >= 96 ? 128 : (cout >= 48 ? 64 : 32
 
 static int g_reserved_sms = 0;     // SMs the persistent grid leaves free (for a collective's kernel on multi-GPU runs)
 
-template <int BN, bool F16>
+// Window mode (TC_WIN_ROWS) takes a launch when its rows are the dense grid, its taps read no index map or gate, its
+// tiles are not split (whole tiles or balanced) and every source's window fits a slot.
+static bool tc_window_fits(const wmd_conv_desc& d, int splits) {
+  if (d.taps != 9 || d.pixels || d.map0 || d.map1 || d.gate || splits > 1 || d.W > TC_WIN_ROWS) return false;
+  return win_rows(d.W, d.shift0) <= TC_WIN_ROWS && (d.c1 == 0 || win_rows(d.W, 0) <= TC_WIN_ROWS);
+}
+
+template <int BN, bool F16, bool WIN>
 static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStream_t stream) {
-  using Cfg = TcCfg<BN, F16>;
+  const size_t smem = WIN ? TcWinCfg<BN, F16>::SMEM : TcCfg<BN, F16>::SMEM;
+  auto kernel = WIN ? conv_rows_tc_kernel_window<BN, F16> : conv_rows_tc_kernel<BN, F16>;
   static bool attr_done[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_done[dev]) {   // outside the cache: set it on every launch
-    int rc = record(cudaFuncSetAttribute(conv_rows_tc_kernel<BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(Cfg::SMEM)));
+    int rc = record(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     if (rc != WMD_OK) return rc;
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
   }
   const long long tiles = static_cast<long long>(ceil_div(d.max_rows, TC_BM)) * ceil_div(d.cout, BN) * (splits > 0 ? splits : 1);
   const long long cap = sm_count() - g_reserved_sms > 1 ? sm_count() - g_reserved_sms : 1;
   const int grid = splits == 0 ? static_cast<int>(cap) : static_cast<int>(tiles < cap ? (tiles < 1 ? 1 : tiles) : cap);
-  conv_rows_tc_kernel<BN, F16><<<grid, TC_THREADS, Cfg::SMEM, stream>>>(d, d.w, splits, partial);
+  kernel<<<grid, TC_THREADS, smem, stream>>>(d, d.w, splits, partial);
   int rc = launched();
   if (rc != WMD_OK || splits <= 1) return rc;      // whole tiles, or balanced: the kernel's own fix-up finishes cut tiles
   const int nchunks = d.taps * ((d.c0 + TC_BK - 1) / TC_BK + (d.c1 + TC_BK - 1) / TC_BK);
@@ -1185,8 +1330,10 @@ extern "C" int wmd_conv_rows_tc_splitk_f32(const wmd_conv_desc* dp, int splits, 
   if (f16) WMD_REQUIRE(d.amax0 != nullptr && (d.c1 == 0 || d.amax1 != nullptr), WMD_ERR_ARG);
   if (f16) WMD_REQUIRE(splits <= 1, WMD_ERR_UNSUPPORTED);   // tc_reduce_kernel sums unscaled slabs: tf32 operands only
   cudaStream_t st = as_stream(stream);
-#define WMD_TC_LAUNCH(BN_) \
-  return f16 ? launch_tc<BN_, true>(d, splits, partial, st) : launch_tc<BN_, false>(d, splits, partial, st)
+  const bool win = tc_window_fits(d, splits);
+#define WMD_TC_LAUNCH(BN_)                                                                                   \
+  return f16 ? (win ? launch_tc<BN_, true, true>(d, splits, partial, st) : launch_tc<BN_, true, false>(d, splits, partial, st)) \
+             : (win ? launch_tc<BN_, false, true>(d, splits, partial, st) : launch_tc<BN_, false, false>(d, splits, partial, st))
   switch (tc_tile_n(d.cout)) {
     case 128: WMD_TC_LAUNCH(128);
     case 64: WMD_TC_LAUNCH(64);
