@@ -74,7 +74,9 @@ int wmd_idwt_haar_f32(const float* ll, const float* hf, float* out, float* disp,
  * disp = [clamp01](idwt(ll,hf) * disp_scale), PyTorch F.interpolate(mode="bilinear") index arithmetic for either
  * align_corners setting.  Replaces the consumers of ("disp", s): KITTI/trainer.py:338-339 (align_corners=False),
  * NYUv2/utils.py:223-227, NYUv2/train.py:305-306 (align_corners=True).  The intermediate disp plane is not read
- * back from HBM.  Supports upsampling (and downsampling up to ~1.3x). */
+ * back from HBM.  Upsampling only, by about 1.6x per axis or more: with sy, sx = source / destination size per axis (the
+ * disp plane is 2H x 2W), a 32 x 128 output tile's source patch must fit 2048 floats, (floor(32 sy) + 4) (floor(128 sx)
+ * + 4) <= 2048; smaller factors (equal sizes, 1.5x) return WMD_ERR_UNSUPPORTED. */
 int wmd_idwt_bilinear_f32(const float* ll, const float* hf, float* full, float disp_scale, int clamp01, int full_h,
                           int full_w, int align_corners, int N, int C, int H, int W, wmd_stream_t stream);
 
@@ -287,7 +289,9 @@ int wmd_head_conv3x3_f32(const wmd_head_desc* d, wmd_stream_t stream);
  * (taps = 1, cout = 9*groups); this entry point gathers and sums the nine taps per output pixel,
  *   s_g = bias[g] + sum_tap z[map(p + tap), tap*groups + g],
  * and scatters  out[n, j, y, x] = scale * (act(s_j) - act(s_{cout+j}))  (dual, groups = 2*cout)  or  scale * act(s_j)
- * (groups = cout) into the dense NCHW tensor (zero-filled by the caller when pixels != NULL).  groups in {1,2,3,4,6,8}. */
+ * (groups = cout) into the dense NCHW tensor (zero-filled by the caller when pixels != NULL).  groups in {1,2,3,4,6,8}.
+ * z has no alignment requirement (any column offset, any ldz); 8-byte aligned z with an even ldz reads float2 pairs,
+ * with the same sums. */
 int wmd_head_gather_f32(const float* z, int ldz, int groups, const int32_t* map, const float* bias, float scale, int act,
                         int dual, int pad_mode, const int32_t* pixels, const int32_t* count, int max_rows, float* out,
                         int cout, int N, int H, int W, wmd_stream_t stream);

@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(256) dwt_haar_kernel(const float* __restrict__
 // reads are L1/L2 hits shared by the four quadrants), then every thread blends its outputs.  The disp plane itself
 // is never read back from HBM: 16*H*W coefficient bytes in, 4*Hf*Wf bytes out.
 constexpr int kBT_H = 32, kBT_W = 128;
-constexpr int kBS_MAX = 2048;   // floats of shared source patch (>= (32/f+3) * (128/f+3) for f >= 1.33)
+constexpr int kBS_MAX = 2048;   // floats of shared source patch: (32/f + 4) * (128/f + 4) fits for f >= ~1.6 per axis
 
 __device__ __forceinline__ float src_index(float scale, int dst, bool align_corners) {
   if (align_corners) return scale * static_cast<float>(dst);
@@ -222,7 +222,7 @@ extern "C" int wmd_idwt_bilinear_f32(const float* ll, const float* hf, float* fu
                                  : static_cast<float>(Hs) / static_cast<float>(full_h);
   const float sx = align_corners ? (full_w > 1 ? static_cast<float>(Ws - 1) / static_cast<float>(full_w - 1) : 0.f)
                                  : static_cast<float>(Ws) / static_cast<float>(full_w);
-  // shared patch must hold the tile's source footprint (upsampling or mild downsampling only)
+  // shared patch must hold the tile's source footprint (upsampling by ~1.6x or more only)
   const long long need = (static_cast<long long>(kBT_H * sy) + 4) * (static_cast<long long>(kBT_W * sx) + 4);
   WMD_REQUIRE(need <= kBS_MAX, WMD_ERR_UNSUPPORTED);
   dim3 grid(ceil_div(full_w, kBT_W), ceil_div(full_h, kBT_H), static_cast<unsigned>(planes));

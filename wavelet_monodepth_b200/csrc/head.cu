@@ -115,13 +115,15 @@ static int launch_head(const wmd_head_desc& d, cudaStream_t stream) {
 // GEMM (Z = T x Wz, Wz = [tap][group] columns, wmd_conv_rows_* with taps = 1), and this kernel only gathers and adds
 // 9 x G floats per output pixel (G = 6 for a +/- pair of 3-channel heads) instead of 9 x 2C: 10-80x less gather
 // traffic.  One thread per output pixel; consecutive threads take consecutive active pixels, i.e. neighbours in
-// x, so the nine Z rows they touch are mostly adjacent in memory.
-template <int G>
+// x, so the nine Z rows they touch are mostly adjacent in memory.  VEC (G even, z 8-byte aligned, ldz even: decided on
+// the host) reads each tap's G floats as float2 pairs; otherwise scalar loads.  The sums are the same either way.
+template <int G, bool VEC>
 __global__ void __launch_bounds__(256) head_gather_kernel(const float* __restrict__ z, int ldz,
                                                           const int32_t* __restrict__ map, const float* __restrict__ bias,
                                                           float scale, int act, int dual, int pad_mode,
                                                           const int32_t* __restrict__ pixels, const int32_t* __restrict__ count,
                                                           int max_rows, float* __restrict__ out, int cout, int N, int H, int W) {
+  static_assert(!VEC || G % 2 == 0, "float2 loads need an even group count");
   const long long HW = static_cast<long long>(H) * W;
   const int total_px = static_cast<int>(static_cast<long long>(N) * HW);
   int rows = pixels ? *count : total_px;
@@ -148,7 +150,7 @@ __global__ void __launch_bounds__(256) head_gather_kernel(const float* __restric
       const int row = map ? map[q] : q;
       if (row < 0) continue;
       const float* zr = z + static_cast<long long>(row) * ldz + tap * G;
-      if (G % 2 == 0 && (ldz % 2) == 0) {
+      if (VEC) {
 #pragma unroll
         for (int g = 0; g < G; g += 2) {
           const float2 v = __ldg(reinterpret_cast<const float2*>(zr + g));
@@ -191,19 +193,25 @@ extern "C" int wmd_head_gather_f32(const float* z, int ldz, int groups, const in
   if (max_rows == 0) return WMD_OK;
   const int grid = stride_grid(max_rows, 256, 8);
   cudaStream_t st = as_stream(stream);
-#define WMD_LAUNCH_GATHER(GG)                                                                                         \
-  head_gather_kernel<GG><<<grid, 256, 0, st>>>(z, ldz, map, bias, scale, act, dual, pad_mode, pixels, count, max_rows, \
-                                               out, cout, N, H, W)
+  // float2 loads need every row's tap block 8-byte aligned: z itself (callers pass z + col0) and an even ldz
+  const bool vec = (reinterpret_cast<uintptr_t>(z) & 7) == 0 && ldz % 2 == 0;
+#define WMD_LAUNCH_GATHER_V(GG, VV)                                                                                        \
+  head_gather_kernel<GG, VV><<<grid, 256, 0, st>>>(z, ldz, map, bias, scale, act, dual, pad_mode, pixels, count, max_rows, \
+                                                   out, cout, N, H, W)
+#define WMD_LAUNCH_GATHER(GG)              \
+  if (vec) WMD_LAUNCH_GATHER_V(GG, true);  \
+  else WMD_LAUNCH_GATHER_V(GG, false)
   switch (groups) {
-    case 1: WMD_LAUNCH_GATHER(1); break;
+    case 1: WMD_LAUNCH_GATHER_V(1, false); break;
     case 2: WMD_LAUNCH_GATHER(2); break;
-    case 3: WMD_LAUNCH_GATHER(3); break;
+    case 3: WMD_LAUNCH_GATHER_V(3, false); break;
     case 4: WMD_LAUNCH_GATHER(4); break;
     case 6: WMD_LAUNCH_GATHER(6); break;
     case 8: WMD_LAUNCH_GATHER(8); break;
     default: return WMD_ERR_UNSUPPORTED;
   }
 #undef WMD_LAUNCH_GATHER
+#undef WMD_LAUNCH_GATHER_V
   return launched();
 }
 
