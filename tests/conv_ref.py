@@ -17,6 +17,10 @@ PAD_ZERO, PAD_REFLECT, PAD_REPLICATE = 0, 1, 2
 ACT_NONE, ACT_ELU, ACT_LRELU, ACT_SIGMOID = 0, 1, 2, 3
 _f64 = torch.float64
 
+# err / S bars of the three engines (the error model and the measurements behind them: tests/test_gpu_conv_contract.py)
+BAR = {"tf32x3": 4e-5, "f16x3": 2.5e-5, "simt": 1.5e-5}
+ACT_ALLOW = 5e-7                  # absolute error of the kernels' expf-based ELU / sigmoid epilogues
+
 
 def _pad_coord(q, n, pad):
     """(mapped q, inside) under pad mode `pad`, as pad_coord in csrc/common.cuh."""
@@ -83,10 +87,13 @@ def gather_rows(m, x0, c0, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0
 
 
 def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NONE, act_param=0.0, map0=None, shift0=0,
-             x1=None, c1=0, map1=None, gate=None, pixels=None, count=None, max_rows=None, rows0=None, block_elems=1 << 24):
+             x1=None, c1=0, map1=None, gate=None, pixels=None, count=None, max_rows=None, rows0=None, block_elems=1 << 24,
+             read_max=False):
     """(y64, S) for rows [0, min(count, max_rows)): the arguments of ops.conv_rows, with a plain (cout, c0 + c1, k, k)
     weight and an optional bias (cout,).  count: int or 1-element tensor (with pixels); rows0 (taps == 1, map0 None
-    only): rows x0 holds, rows past it read zeros (default: x0.shape[0])."""
+    only): rows x0 holds, rows past it read zeros (default: x0.shape[0]).
+    read_max: also return the largest |value| the launch reads from source 0 and from source 1 (the maxima its fp16-pair
+    operand scales must cover): (y64, S, max0, max1)."""
     dev = x0.device
     cout = weight.shape[0]
     rows = int(count) if pixels is not None else n * h * w
@@ -101,11 +108,18 @@ def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NON
     y64 = torch.empty(rows, cout, dtype=_f64, device=dev)
     s = torch.empty(rows, cout, dtype=_f64, device=dev)
     step = max(1, block_elems // max(k, 1))
+    max0 = max1 = 0.0
     for r in range(0, rows, step):
         m = torch.arange(r, min(rows, r + step), device=dev)
-        a = gather_rows(m, x0, c0, n, h, w, taps, pad, map0, shift0, x1, c1, map1, gate, pixels, rows0).reshape(len(m), k)
+        a = gather_rows(m, x0, c0, n, h, w, taps, pad, map0, shift0, x1, c1, map1, gate, pixels, rows0)
+        if read_max:
+            max0 = max(max0, float(a[..., :c0].abs().max()) if c0 else 0.0)
+            max1 = max(max1, float(a[..., c0:].abs().max()) if c1 else 0.0)
+        a = a.reshape(len(m), k)
         y64[r:r + len(m)] = a @ wk + b
         s[r:r + len(m)] = a.abs() @ wa + b.abs()
+    if read_max:
+        return activate(y64, act, act_param), s, max0, max1
     return activate(y64, act, act_param), s
 
 

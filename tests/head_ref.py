@@ -12,10 +12,15 @@ Values are per output row (pixel p = pixels[m], or m itself, for m < min(count, 
 head_idwt_ref's dense planes.  Independent of libwmd and ops.*; runs on whatever device the inputs live on.
 """
 import torch
+import torch.nn.functional as F
 
 import conv_ref as cr
 
 _f64 = torch.float64
+
+# err / S bars of the head kernels and idwt_bilinear's bound (measurements and error model: tests/test_gpu_head_contract.py)
+BAR = {"head_conv3x3": 4e-7, "head_gather": 4.5e-7, "head_idwt": 4.5e-7, "head_mlp": 4e-6}
+BILINEAR_ULP = 2.5                # units of 2^-23 x the largest |disp| around the four neighbours
 
 
 def _rows(n, h, w, pixels, count, max_rows):
@@ -122,3 +127,24 @@ def head_mlp_ref(x, c, w1, b1, wz, slope, count, max_rows):
     s1 = xs.abs() @ w1.abs().T + b.abs()
     t = cr.activate(pre, cr.ACT_LRELU, slope)
     return t @ wz.T, (s1 + t.abs()) @ wz.abs().T
+
+
+def bilinear_ulps(got, disp, size, align_corners):
+    """Worst |got - F.interpolate(disp)| of a bilinear resize in units of 2^-23 x the largest |disp| of the 3 x 3 window
+    around each output's top-left neighbour (a bound of the four neighbours it mixes).  disp (N, C, h, w) on got's device;
+    the interpolation runs in disp's dtype."""
+    dev = got.device
+    want = F.interpolate(disp, size=size, mode="bilinear", align_corners=align_corners)
+    hs, ws = disp.shape[-2:]
+    m = F.max_pool2d(disp.abs(), 3, stride=1, padding=1)
+    ys, xs = torch.arange(size[0], device=dev, dtype=_f64), torch.arange(size[1], device=dev, dtype=_f64)
+    if align_corners:
+        fy = ys * ((hs - 1) / max(size[0] - 1, 1))
+        fx = xs * ((ws - 1) / max(size[1] - 1, 1))
+    else:
+        fy = ((ys + 0.5) * (hs / size[0]) - 0.5).clamp(min=0)
+        fx = ((xs + 0.5) * (ws / size[1]) - 0.5).clamp(min=0)
+    y0, x0 = fy.floor().long().clamp(max=hs - 1), fx.floor().long().clamp(max=ws - 1)
+    mag = m[:, :, y0][:, :, :, x0]
+    assert got.shape == want.shape
+    return float(((got.to(want.dtype) - want).abs() / (mag * 2.0 ** -23).clamp(min=1e-38)).max())

@@ -1,0 +1,695 @@
+"""Launch-checking harness: every libwmd launch a workload makes, checked against the fp64 contract of its kernel.
+
+`Harness(monkeypatch)` wraps the public entry points of wavelet_monodepth_b200.ops.  The decoders, train_native and
+wavelets call `ops.<name>` through the module, and calls inside ops (conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows)
+resolve through the module's globals, so wrapping the module attributes catches every call, nested ones included.
+
+Each call runs the original function, synchronises (compactions and list gathers run on side streams), recomputes the
+result from the call's actual inputs with the references of the kernel contract tests (conv_ref, head_ref, disp_tail_ref,
+conv_grad_ref, oracle.haar, plain torch restatements of the wmd.h comments: none of them uses ops or libwmd) and compares
+at that kernel's bar.  It also checks the preconditions a launch's contract relies on: source maxima that cover what an
+fp16-pair launch reads, exact amax outputs, index maps inside their sources, strictly increasing pixel lists, and
+count <= max_rows.  Pack calls record the plain weights behind each packed object; a pack is right when every launch
+that uses it is right.
+
+Completeness: around each outermost wrapped call the harness takes the `launch_count()` delta; at the end of a workload the
+checked deltas must add up to the whole delta, and any libwmd symbol called outside a wrapped call is named.
+"""
+import contextlib
+import inspect
+import threading
+
+import torch
+import torch.nn.functional as F
+
+from oracle import haar as ohaar
+from wavelet_monodepth_b200 import _lib, ops
+
+import conv_grad_ref
+import conv_ref as cr
+import disp_tail_ref
+import head_ref as hr
+
+_f32, _f64 = torch.float32, torch.float64
+EPS = 2.0 ** -24
+
+# ops entry points that launch kernels -> their checker (method name below); pack entry points; helpers without launches
+CHECKED = ("conv_rows", "head_mlp", "head_gather", "head_conv3x3", "head_idwt", "idwt_haar", "dwt_haar", "idwt_bilinear",
+           "disp_tail16", "range_thresh", "level_masks", "compact", "gate_map", "nchw_to_rows", "gather_rows",
+           "gather_rows_list", "rows_to_nchw", "scatter_rows", "amax_rows", "act_backward", "conv_wgrad", "conv_dgrad")
+PACKS = ("pack_weight", "pack_head_weight", "pack_head_mlp", "pack_disp_tail16")
+
+# every symbol of _lib.SIGNATURES: ("launch", ops entry point whose checker covers it) | ("pack", ops entry point) | "query"
+SYMBOLS = {
+    "wmd_version": "query", "wmd_status_string": "query", "wmd_last_cuda_error": "query", "wmd_launch_count": "query",
+    "wmd_idwt_haar_f32": ("launch", "idwt_haar"),
+    "wmd_idwt_haar_epi_f32": ("launch", "idwt_haar"),
+    "wmd_idwt_bilinear_f32": ("launch", "idwt_bilinear"),
+    "wmd_dwt_haar_f32": ("launch", "dwt_haar"),
+    "wmd_range_ws_bytes": "query",
+    "wmd_range_thresh_f32": ("launch", "range_thresh"),
+    "wmd_level_masks": ("launch", "level_masks"),
+    "wmd_compact_ws_bytes": "query",
+    "wmd_compact_mask": ("launch", "compact"),
+    "wmd_gate_map": ("launch", "gate_map"),
+    "wmd_nchw_to_rows_f32": ("launch", "nchw_to_rows"),
+    "wmd_nchw_to_rows_gated_f32": ("launch", "nchw_to_rows"),
+    "wmd_nchw_to_rows_amax_f32": ("launch", "nchw_to_rows"),
+    "wmd_nchw_to_rows_masked_amax_f32": ("launch", "nchw_to_rows"),
+    "wmd_nchw_to_rows_gated_amax_f32": ("launch", "nchw_to_rows"),
+    "wmd_rows_to_nchw_f32": ("launch", "rows_to_nchw"),
+    "wmd_gather_rows_nchw_f32": ("launch", "gather_rows"),
+    "wmd_gather_rows_list_f32": ("launch", "gather_rows_list"),
+    "wmd_gather_rows_list_amax_f32": ("launch", "gather_rows_list"),
+    "wmd_scatter_rows_nchw_f32": ("launch", "scatter_rows"),
+    "wmd_amax_f32": ("launch", "amax_rows"),
+    "wmd_amax_rows_masked_f32": ("launch", "amax_rows"),
+    "wmd_pack_conv_weight_f32": ("pack", "pack_weight"),
+    "wmd_pack_conv_weight_tc16_f32": ("pack", "pack_weight"),
+    "wmd_pack_conv_weight_tc_f32": ("pack", "pack_weight"),
+    "wmd_conv_tc_weight_floats": "query",
+    "wmd_conv_tc16_weight_bytes": "query",
+    "wmd_conv_tc_tile_n": "query",
+    "wmd_conv_tc_set_reserved_sms": "query",
+    "wmd_conv_tc_splitk_ws_bytes": "query",
+    "wmd_conv_rows_f32": ("launch", "conv_rows"),
+    "wmd_conv_rows_tc_f32": ("launch", "conv_rows"),
+    "wmd_conv_rows_tc_splitk_f32": ("launch", "conv_rows"),
+    "wmd_head_mlp_supported": "query",
+    "wmd_head_mlp_weight_floats": "query",
+    "wmd_pack_head_mlp_f32": ("pack", "pack_head_mlp"),
+    "wmd_head_mlp_f32": ("launch", "head_mlp"),
+    "wmd_head_conv3x3_f32": ("launch", "head_conv3x3"),
+    "wmd_head_gather_f32": ("launch", "head_gather"),
+    "wmd_head_idwt_ws_bytes": "query",
+    "wmd_head_idwt_f32": ("launch", "head_idwt"),
+    "wmd_pack_disp_tail16_f32": ("pack", "pack_disp_tail16"),
+    "wmd_disp_tail16_f32": ("launch", "disp_tail16"),
+    "wmd_act_bwd_ws_bytes": "query",
+    "wmd_act_bwd_f32": ("launch", "act_backward"),
+    "wmd_conv_wgrad_ws_bytes": "query",
+    "wmd_conv_wgrad_f32": ("launch", "conv_wgrad"),
+    "wmd_conv_dgrad_fold_f32": ("launch", "conv_dgrad"),
+}
+
+# bars of the checks this file adds on top of the contract tests' (units of 2^-24 of the element's scale)
+DWT_ULP = 8            # four roundings on each path of a one-level analysis bound the error by 4 x 2^-24 S; twice that
+ACT_BWD_ULP = 4        # dz = dy act'(y): at most three roundings (sigmoid: 1 - y, y (1 - y), the product with dy)
+
+REPORT = {}            # (entry, engine, mode) -> [worst err, bar, launches, largest row count]
+
+
+def _record(entry, engine, mode, err, bar, rows):
+    r = REPORT.setdefault((entry, engine, mode), [0.0, bar, 0, 0])
+    r[0] = max(r[0], err)
+    r[2] += 1
+    r[3] = max(r[3], int(rows))
+
+
+def report_lines():
+    lines = ["worst err per (entry point, engine / precision, mode): worst (bar, launches, most rows)"]
+    for k in sorted(REPORT):
+        worst, bar, count, rows = REPORT[k]
+        lines.append("  %-16s %-8s %-18s %.2e  (bar %s, %d launches, %d rows)"
+                     % (k + (worst, "exact" if bar == 0 else "%.2g" % bar, count, rows)))
+    return lines
+
+
+def _err(got, want, s, allow=0.0):
+    """max over the elements of (|got - want| - allow) / S."""
+    if got.numel() == 0:
+        return 0.0
+    return float(((got.double() - want).abs() - allow).clamp(min=0).div(s.clamp(min=1e-300)).max())
+
+
+def _i(t):
+    return int(t.reshape(-1)[0]) if torch.is_tensor(t) else int(t)
+
+
+def _nhwc(x):
+    n, c = x.shape[:2]
+    return x.permute(0, 2, 3, 1).reshape(-1, c)
+
+
+def _scalar(t):
+    return float(t.reshape(-1)[0])
+
+
+class LaunchError(AssertionError):
+    pass
+
+
+def _require(ok, what):
+    if not ok:
+        raise LaunchError(what)
+
+
+class _LibSpy:
+    """Stands in for the loaded CDLL: records the libwmd symbols called while no wrapped entry point is running."""
+
+    def __init__(self, lib, harness):
+        self._lib, self._h = lib, harness
+
+    def __getattr__(self, name):
+        fn = getattr(self._lib, name)
+        if not name.startswith("wmd_") or SYMBOLS.get(name) == "query":
+            return fn
+        h = self._h
+
+        def call(*args):
+            if h.depth == 0:
+                h.outside.append(name)
+            return fn(*args)
+        return call
+
+
+class Harness:
+    def __init__(self, monkeypatch):
+        self.packs = {}            # data_ptr of a packed image -> (packed object, plain weights)
+        self.depth = 0
+        self.main = threading.get_ident()
+        self.current = None
+        self.checked = 0
+        self.outside = []
+        self.gaps = []             # kernels launched between two checked calls of a thread other than the workload's
+        self.last_end = {}         # thread -> launch_count() when its last outermost checked call returned
+        self.calls = {}
+        lib = _lib.load()
+        monkeypatch.setattr(_lib, "_lib", _LibSpy(lib, self))
+        for name in CHECKED:
+            monkeypatch.setattr(ops, name, self._wrap(name, getattr(ops, name), getattr(self, "_check_" + name)))
+        for name in PACKS:
+            monkeypatch.setattr(ops, name, self._wrap(name, getattr(ops, name), getattr(self, "_pack_" + name)))
+
+    # ------------------------------------------------------------------------------------------ plumbing
+    def _wrap(self, name, orig, check):
+        sig = inspect.signature(orig)
+        before = getattr(self, "_before_" + name, None)
+
+        def wrapped(*args, **kwargs):
+            a = sig.bind(*args, **kwargs)
+            a.apply_defaults()
+            a = dict(a.arguments)
+            outer = self.depth == 0
+            if outer:
+                torch.cuda.synchronize()
+                c0 = _lib.launch_count()
+                tid = threading.get_ident()
+                if tid != self.main and tid in self.last_end and c0 != self.last_end[tid]:
+                    self.gaps.append((name, c0 - self.last_end[tid]))
+            pre = before(a) if before is not None else None
+            self.depth += 1
+            try:
+                res = orig(*args, **kwargs)
+            finally:
+                self.depth -= 1
+            torch.cuda.synchronize()
+            if outer:
+                c1 = _lib.launch_count()
+                self.last_end[tid] = c1
+                if tid == self.main:
+                    self.checked += c1 - c0
+            self.calls[name] = self.calls.get(name, 0) + 1
+            check(a, res, pre)
+            return res
+        return wrapped
+
+    @contextlib.contextmanager
+    def workload(self, name):
+        """Checks that every kernel launched inside the block ran inside a checked call.  launch_count() counts per host
+        thread: on the calling thread the checked deltas must add up to the whole; autograd runs the backward on its own
+        thread, whose counter must not move between two checked calls."""
+        torch.cuda.synchronize()
+        self.current, self.checked, self.outside, self.gaps, self.last_end = name, 0, [], [], {}
+        self.main = threading.get_ident()
+        c0 = _lib.launch_count()
+        yield self
+        torch.cuda.synchronize()
+        total = _lib.launch_count() - c0
+        _require(not self.outside and not self.gaps and total == self.checked,
+                 "%s: %d kernels launched, %d inside checked calls; libwmd called outside them: %s; launched between "
+                 "checked calls of the backward thread, before: %s" % (name, total, self.checked, sorted(set(self.outside)),
+                                                                        self.gaps))
+        _require(total > 0, "%s launched nothing" % name)
+
+    def _weights(self, packed):
+        key = packed.data.data_ptr() if isinstance(packed, ops.PackedW) else packed.data_ptr()
+        _require(key in self.packs, "a launch uses a packed weight no pack call of this harness produced")
+        return self.packs[key][1]
+
+    def _keep(self, packed, weights):
+        key = packed.data.data_ptr() if isinstance(packed, ops.PackedW) else packed.data_ptr()
+        self.packs[key] = (packed, weights)
+
+    # ------------------------------------------------------------------------------------------ packs
+    def _pack_pack_weight(self, a, res, pre):
+        self._keep(res, a["weight"].detach().clone())
+
+    def _pack_pack_head_weight(self, a, res, pre):
+        self._keep(res, a["weight"].detach().clone())
+
+    def _pack_pack_head_mlp(self, a, res, pre):
+        b1 = a["b1"].detach().clone() if a["b1"] is not None else None
+        self._keep(res, (a["w1"].detach().clone(), b1, a["wz"].detach().clone()))
+
+    def _pack_pack_disp_tail16(self, a, res, pre):
+        self._keep(res, tuple(t.detach().clone() if t is not None else None for t in (a["w1"], a["b1"], a["w2"], a["b2"])))
+
+    # ------------------------------------------------------------------------------------------ shared preconditions
+    def _check_list(self, entry, pixels, count, max_rows, total):
+        """count <= max_rows; the first min(count, max_rows) entries of the list strictly increasing, inside the grid."""
+        if pixels is None:
+            return total
+        cnt = _i(count)
+        _require(0 <= cnt <= max_rows, "%s: count %d outside [0, max_rows = %d]" % (entry, cnt, max_rows))
+        p = pixels.reshape(-1)[:cnt].long()
+        if cnt:
+            _require(bool((p[1:] > p[:-1]).all()), "%s: pixel list not strictly increasing" % entry)
+            _require(int(p[0]) >= 0 and int(p[-1]) < total, "%s: pixel list leaves the %d-pixel grid" % (entry, total))
+        return cnt
+
+    def _check_map(self, entry, m, rows):
+        if m is not None and m.numel():
+            _require(int(m.max()) < rows, "%s: index map entry %d past the %d rows of its source" % (entry, int(m.max()), rows))
+            _require(int(m.min()) >= -1, "%s: index map entry below -1" % entry)
+
+    def _before_amax(self, t):
+        return t.clone() if t is not None else None
+
+    def _check_amax_out(self, entry, old, new, values):
+        want = max(_scalar(old), float(values.abs().max()) if values.numel() else 0.0)
+        _require(_scalar(new) == want, "%s: amax %.9g, want exactly %.9g" % (entry, _scalar(new), want))
+
+    # ------------------------------------------------------------------------------------------ convolution
+    def _before_conv_rows(self, a):
+        return self._before_amax(a["amax_out"])
+
+    def _check_conv_rows(self, a, out, old_amax):
+        wp = a["wpacked"]
+        weight = self._weights(wp)
+        n, h, w, taps, c0, c1, cout = a["n"], a["h"], a["w"], a["taps"], a["c0"], a["c1"], a["cout"]
+        x0, x1 = a["x0"], a["x1"]
+        total = n * h * w
+        max_rows = total if a["max_rows"] is None else int(a["max_rows"])
+        splits = a["splits"]
+        if wp.kind == "tc" and splits is None:
+            nchunks = taps * (-(-c0 // 32) + -(-c1 // 32))
+            splits = 0 if nchunks >= ops.TC_BALANCE_MIN_CHUNKS else 1
+        use16 = (wp.kind == "tc" and wp.data16 is not None and a["amax0"] is not None
+                 and (x1 is None or a["amax1"] is not None) and splits in (0, 1))
+        engine = "simt" if wp.kind == "simt" else ("f16x3" if use16 else "tf32x3")
+        mode = "-" if wp.kind == "simt" else {1: "whole", 0: "balanced"}.get(splits, "split-K")
+        dense3 = taps == 9 and a["pixels"] is None and a["map0"] is None and a["map1"] is None and a["gate"] is None
+        mode += "/dense3x3" if dense3 else ("/1x1" if taps == 1 else "/gather")
+        entry = "conv_rows"
+        rows = min(self._check_list(entry, a["pixels"], a["count"], max_rows, total), max_rows)
+        rows0 = int(x0.shape[0])
+        self._check_map(entry, a["map0"], rows0)
+        if x1 is not None:
+            self._check_map(entry, a["map1"], int(x1.shape[0]))
+        y64, s, m0, m1 = cr.conv_ref(x0, c0, weight, a["bias"], n, h, w, taps=taps, pad=a["pad"], act=a["act"],
+                                     act_param=a["act_param"], map0=a["map0"], shift0=a["shift0"], x1=x1, c1=c1,
+                                     map1=a["map1"], gate=a["gate"], pixels=a["pixels"], count=a["count"],
+                                     max_rows=max_rows, rows0=rows0 if (taps == 1 and a["map0"] is None) else None,
+                                     read_max=True)
+        if use16:
+            _require(_scalar(a["amax0"]) >= m0, "conv_rows: amax0 %.9g below the largest |x0| read, %.9g"
+                     % (_scalar(a["amax0"]), m0))
+            if x1 is not None:
+                _require(_scalar(a["amax1"]) >= m1, "conv_rows: amax1 %.9g below the largest |x1| read, %.9g"
+                         % (_scalar(a["amax1"]), m1))
+        y = out[:rows, :cout]
+        if wp.kind == "tc" and a["amax_out"] is not None:
+            self._check_amax_out(entry, old_amax, a["amax_out"], y)
+        allow = 0.0 if a["act"] in (cr.ACT_NONE, cr.ACT_LRELU) else cr.ACT_ALLOW
+        err = _err(y, y64, s, allow)
+        bar = cr.BAR[engine]
+        _record(entry, engine, mode, err, bar, rows)
+        _require(err <= bar, "%s: conv_rows %s %s (n %d, %dx%d, c0 %d, c1 %d, cout %d, taps %d, %d rows): err/S %.3g > %.3g"
+                 % (self.current, engine, mode, n, h, w, c0, c1, cout, taps, rows, err, bar))
+
+    # ------------------------------------------------------------------------------------------ coefficient heads
+    def _check_head_mlp(self, a, z, pre):
+        w1, b1, wz = self._weights(a["packed"])
+        x = a["x"]
+        max_rows = x.shape[0] if a["max_rows"] is None else int(a["max_rows"])
+        count = _i(a["count"]) if a["count"] is not None else None
+        if count is not None:
+            _require(count <= max_rows, "head_mlp: count %d > max_rows %d" % (count, max_rows))
+        rows = max_rows if count is None else min(count, max_rows)
+        want, s = hr.head_mlp_ref(x, a["c"], w1, b1, wz, a["slope"], count, max_rows)
+        nz = a["nz"]
+        _require(bool((z[:rows, nz:56] == 0).all()), "head_mlp: columns nz..55 are not zero")
+        err = _err(z[:rows, :nz], want, s)
+        bar = hr.BAR["head_mlp"]
+        _record("head_mlp", "tf32x3", "-", err, bar, rows)
+        _require(err <= bar, "%s: head_mlp err/S %.3g > %.3g" % (self.current, err, bar))
+
+    def _written(self, out, pixels, rows, cout):
+        flat = out.permute(0, 2, 3, 1).reshape(-1, cout)
+        return flat[pixels.reshape(-1)[:rows].long()] if pixels is not None else flat
+
+    def _check_head_gather(self, a, out, pre):
+        z, groups, n, h, w, cout = a["z"], a["groups"], a["n"], a["h"], a["w"], a["cout"]
+        total = n * h * w
+        max_rows = total if a["max_rows"] is None else int(a["max_rows"])
+        rows = min(self._check_list("head_gather", a["pixels"], a["count"], max_rows, total), max_rows)
+        self._check_map("head_gather", a["idxmap"], z.shape[0])
+        want, s = hr.head_gather_ref(z, z.shape[1], a["col0"], groups, a["idxmap"], a["bias"], a["scale"], a["act"],
+                                     a["dual"], a["pad"], a["pixels"], a["count"], max_rows, cout, n, h, w)
+        allow = 0.0 if a["act"] == cr.ACT_NONE else cr.ACT_ALLOW * abs(a["scale"]) * (2 if a["dual"] else 1)
+        err = _err(self._written(out, a["pixels"], rows, cout), want, s, allow)
+        bar = hr.BAR["head_gather"]
+        _record("head_gather", "fp32", "list" if a["pixels"] is not None else "dense", err, bar, rows)
+        _require(err <= bar, "%s: head_gather err/S %.3g > %.3g" % (self.current, err, bar))
+
+    def _check_head_conv3x3(self, a, out, pre):
+        t, n, h, w, cout, c = a["t"], a["n"], a["h"], a["w"], a["cout"], a["c"]
+        total = n * h * w
+        max_rows = total if a["max_rows"] is None else int(a["max_rows"])
+        rows = min(self._check_list("head_conv3x3", a["pixels"], a["count"], max_rows, total), max_rows)
+        self._check_map("head_conv3x3", a["idxmap"], t.shape[0])
+        dual = a["off_b"] >= 0
+        wa = self._weights(a["wa"])
+        wb = self._weights(a["wb"]) if dual else None
+        want, s = hr.head_conv3x3_ref(t, t.shape[1], c, a["off_a"], a["off_b"], wa, a["ba"], wb, a["bb"], cout, a["scale"],
+                                      a["act"], a["pad"], a["idxmap"], a["pixels"], a["count"], max_rows, n, h, w)
+        allow = 0.0 if a["act"] == cr.ACT_NONE else cr.ACT_ALLOW * abs(a["scale"]) * (2 if dual else 1)
+        err = _err(self._written(out, a["pixels"], rows, cout), want, s, allow)
+        bar = hr.BAR["head_conv3x3"]
+        _record("head_conv3x3", "fp32", "list" if a["pixels"] is not None else "dense", err, bar, rows)
+        _require(err <= bar, "%s: head_conv3x3 (c %d, cout %d) err/S %.3g > %.3g" % (self.current, c, cout, err, bar))
+
+    def _check_head_idwt(self, a, res, pre):
+        z, yl = a["z"], a["yl"]
+        n, _, h, w = yl.shape
+        self._check_map("head_idwt", a["idxmap"], z.shape[0])
+        ref = hr.head_idwt_ref(z, a["col0"], a["idxmap"], a["mask"], a["bias"], a["scale"], a["pad"], yl, a["disp_scale"],
+                               a["clamp01"], n, h, w)
+        al = cr.ACT_ALLOW * abs(a["scale"])
+        err = max(_err(res["yh"], ref["yh"], ref["s_yh"], 2 * al), _err(res["out"], ref["out"], ref["s_out"], 3 * al),
+                  _err(res["disp"], ref["disp"], ref["s_disp"], 3 * al * abs(a["disp_scale"])))
+        if a["mask"] is not None:
+            off = (a["mask"].reshape(n, 1, h, w) == 0).expand(-1, 3, -1, -1)
+            _require(bool((res["yh"][off] == 0).all()), "head_idwt: coefficients outside the wavelet mask are not zero")
+        bar = hr.BAR["head_idwt"]
+        _record("head_idwt", "fp32", "masked" if a["mask"] is not None else "dense", err, bar, n * h * w)
+        _require(err <= bar, "%s: head_idwt err/S %.3g > %.3g" % (self.current, err, bar))
+        if a["thresh_ratio"] is not None:
+            o = res["out"].reshape(n, -1)
+            want = (o.amax(1) - o.amin(1)) * torch.tensor(a["thresh_ratio"], dtype=_f32, device=o.device)
+            _require(torch.equal(res["thresh"], want), "head_idwt: threshold is not (max - min)(out) * ratio")
+        self._check_epilogue("head_idwt", a["epilogue"], res["out"], res["disp"],
+                             [res[k] for k in ("scaled_disp", "depth") if k in res])
+
+    def _check_epilogue(self, entry, epi, out, disp, planes):
+        """The consumer epilogue planes against the torch expressions on the kernel's own reconstruction / disparity."""
+        if epi is None:
+            return
+        if epi[0] == "disp_to_depth":
+            lo, span = 1 / float(epi[2]), 1 / float(epi[1]) - 1 / float(epi[2])
+            scaled = torch.tensor(lo, dtype=_f32, device=disp.device) + torch.tensor(span, dtype=_f32, device=disp.device) * disp
+            _require(torch.equal(planes[0], scaled), "%s: scaled_disp plane" % entry)
+            if len(planes) > 1:
+                _require(torch.equal(planes[1], 1 / scaled), "%s: depth plane" % entry)
+        else:
+            v = out * (torch.tensor(1.0, dtype=_f32) / torch.tensor(float(epi[1]), dtype=_f32)).to(out.device)
+            if epi[2] is not None:
+                v = torch.clamp(v, min=float(epi[2]), max=float(epi[3]))
+            _require(torch.equal(planes[0], v), "%s: div_clamp depth plane" % entry)
+
+    # ------------------------------------------------------------------------------------------ Haar transforms
+    def _oracle_idwt(self, ll, hf):
+        """oracle.haar's synthesis in fp32 on the CPU (the order the kernel claims bit-identity with)."""
+        return ohaar.DWTInverse("haar", "zero")((ll.detach().float().cpu(), [hf.detach().float().cpu()]))
+
+    def _check_idwt_haar(self, a, res, pre):
+        ll, hf = a["ll"], a["hf"]
+        n, c, h, w = ll.shape
+        res_t = res if isinstance(res, tuple) else (res,)
+        want = self._oracle_idwt(ll, hf.reshape(n, c, 3, h, w))
+        _require(torch.equal(res_t[0].cpu(), want), "idwt_haar: reconstruction differs from oracle.haar.DWTInverse")
+        scale = torch.tensor(a["disp_scale"] if a["disp_scale"] is not None else 1.0, dtype=_f32)
+        disp = want * scale
+        if a["clamp01"]:
+            disp = disp.clamp(0.0, 1.0)
+        k = 1
+        if a["disp_scale"] is not None:
+            _require(torch.equal(res_t[1].cpu(), disp), "idwt_haar: disparity plane")
+            k = 2
+        if a["epilogue"] is not None:
+            self._check_epilogue("idwt_haar", a["epilogue"], res_t[0], disp.to(res_t[0].device), list(res_t[k:]))
+        _record("idwt_haar", "fp32", "-", 0.0, 0, n * c * h * w)
+
+    def _check_dwt_haar(self, a, res, pre):
+        """One analysis level against oracle.haar in fp64: |err| <= DWT_ULP 2^-24 S, S = 1/2 the sum of the four |x|."""
+        x = a["x"]
+        ll, hf = res
+        n, c, hh, ww = x.shape
+        x64 = x.detach().double()
+        rl, rh = ohaar.DWTForward(J=1, wave="haar", mode="zero").to(x.device).double()(x64)
+        sc = 0.5 * F.avg_pool2d(x64.abs(), 2) * 4
+        err = max(_err(ll, rl, sc), _err(hf, rh[0], sc.unsqueeze(2).expand_as(rh[0])))
+        bar = DWT_ULP * EPS
+        ol, oh = ohaar.DWTForward(J=1, wave="haar", mode="zero")(x.detach().float().cpu())
+        exact = torch.equal(ll.cpu(), ol) and torch.equal(hf.cpu(), oh[0])
+        _record("dwt_haar", "fp32", "exact" if exact else "bounded", err, bar, n * c * hh * ww // 4)
+        _require(err <= bar, "%s: dwt_haar err/S %.3g > %.3g" % (self.current, err, bar))
+
+    def _check_idwt_bilinear(self, a, full, pre):
+        ll, hf, size, ac = a["ll"], a["hf"], a["size"], bool(a["align_corners"])
+        n, c, h, w = ll.shape
+        disp = self._oracle_idwt(ll, hf.reshape(n, c, 3, h, w)) * torch.tensor(a["disp_scale"], dtype=_f32)
+        if a["clamp01"]:
+            disp = disp.clamp(0.0, 1.0)
+        disp = disp.to(full.device).double()
+        ulps = hr.bilinear_ulps(full, disp, size, ac)
+        _record("idwt_bilinear", "fp32", "ac" if ac else "-", ulps, hr.BILINEAR_ULP, full.numel())
+        _require(ulps <= hr.BILINEAR_ULP, "%s: idwt_bilinear %.3g ulp > %.3g" % (self.current, ulps, hr.BILINEAR_ULP))
+
+    # ------------------------------------------------------------------------------------------ baseline tail
+    def _check_disp_tail16(self, a, out, pre):
+        n = a["n"]
+        if n == 0:
+            return
+        w1, b1, w2, b2 = self._weights(a["packed"])
+        want, s = disp_tail_ref.disp_tail_ref(a["x"], w1, b1, w2, b2, n, a["h"], a["w"])
+        err = _err(out, want, s)
+        _record("disp_tail16", "tf32x3", "-", err, disp_tail_ref.BAR, n * a["h"] * a["w"] * 4)
+        _require(err <= disp_tail_ref.BAR, "%s: disp_tail16 err/S %.3g > %.3g" % (self.current, err, disp_tail_ref.BAR))
+
+    # ------------------------------------------------------------------------------------------ masks and compaction
+    def _check_range_thresh(self, a, res, pre):
+        x = a["x"]
+        n = x.shape[0]
+        xs = x.reshape(n, -1).float()
+        mn, mx = xs.amin(1), xs.amax(1)
+        want = (mx - mn) * torch.tensor(a["ratio"], dtype=_f32, device=x.device)
+        got = res[0] if a["return_minmax"] else res
+        _require(torch.equal(got, want), "range_thresh: not (max - min) * ratio")
+        if a["return_minmax"]:
+            _require(torch.equal(res[1], torch.stack([mn, mx], 1)), "range_thresh: minmax")
+        _record("range_thresh", "fp32", "-", 0.0, 0, n)
+
+    def _check_level_masks(self, a, res, pre):
+        if a["thresh"] is not None:
+            yh = a["yh"]
+            n, h, w = yh.shape[0], yh.shape[-2], yh.shape[-1]
+            s0 = yh.reshape(n, 3, h, w).abs().amax(1, keepdim=True) > a["thresh"].reshape(n, 1, 1, 1)
+        else:
+            n, h, w = a["n"], a["h"], a["w"]
+            s0 = torch.ones((n, 1, h, w), dtype=torch.bool, device=a["device"])
+        f = s0.float()
+        s5 = f.repeat_interleave(2, 2).repeat_interleave(2, 3)
+        want = {"S0": f, "S1": F.max_pool2d(f, 3, 1, 1), "S2": F.max_pool2d(f, 5, 1, 2),
+                "S5": s5, "S4": F.max_pool2d(s5, 3, 1, 1), "S3": F.max_pool2d(s5, 5, 1, 2)}
+        for k, m in res.items():
+            _require(torch.equal(m, want[k].to(torch.uint8)), "level_masks: %s" % k)
+        _record("level_masks", "-", "-", 0.0, 0, n * h * w)
+
+    def _check_compact(self, a, res, pre):
+        if a["stream"] is not None:
+            res = res[0]
+        idxmap, pixels, offsets = res
+        mask = a["mask"]
+        n, h, w = mask.shape[0], mask.shape[-2], mask.shape[-1]
+        m = mask.reshape(n, h, w)
+        per = (m != 0).reshape(n, -1).sum(1)
+        want_off = torch.cat([per.new_zeros(1), per.cumsum(0)]).to(torch.int32)
+        _require(torch.equal(offsets, want_off), "compact: offsets")
+        if idxmap is not None:
+            _require(torch.equal(idxmap, cr.index_map(m)), "compact: index map")
+        if pixels is not None:
+            lst = cr.pixel_list(m)
+            _require(torch.equal(pixels[:len(lst)], lst), "compact: pixel list")
+        _record("compact", "-", "-", 0.0, 0, n * h * w)
+
+    def _check_gate_map(self, a, out, pre):
+        gate = a["gate"]
+        n, h, w = gate.shape[0], gate.shape[-2], gate.shape[-1]
+        g = gate.reshape(n, h, w) != 0
+        src = a["idxmap"].reshape(n, h, w) if a["idxmap"] is not None else \
+            torch.arange(n * h * w, dtype=torch.int32, device=gate.device).reshape(n, h, w)
+        _require(torch.equal(out, torch.where(g, src, torch.full_like(src, -1))), "gate_map")
+        _record("gate_map", "-", "-", 0.0, 0, n * h * w)
+
+    # ------------------------------------------------------------------------------------------ layout moves
+    def _before_nchw_to_rows(self, a):
+        return self._before_amax(a["amax"])
+
+    def _check_nchw_to_rows(self, a, rows, old_amax):
+        x = a["x"]
+        n, c, h, w = x.shape
+        xr = _nhwc(x.to(rows.device) if not x.is_cuda else x)
+        gate = a["gate"]
+        if gate is not None:
+            sel = gate.reshape(-1) != 0
+            got, want = rows[sel], xr[sel]
+            mode = "gated-host" if not x.is_cuda else "gated"
+        else:
+            sel = None
+            got, want = rows, xr
+            mode = "view" if rows.data_ptr() == x.data_ptr() else "plain"
+        _require(torch.equal(got[:, :c], want), "nchw_to_rows (%s): rows differ from the map" % mode)
+        if got.shape[1] > c:
+            _require(bool((got[:, c:] == 0).all()), "nchw_to_rows: pad columns are not zero")
+        if a["amax"] is not None:
+            cover = gate if gate is not None else a["amax_mask"]
+            vals = xr[cover.reshape(-1) != 0] if cover is not None else xr
+            self._check_amax_out("nchw_to_rows (%s)" % mode, old_amax, a["amax"], vals)
+            mode += "+amax" if a["amax_mask"] is None or gate is not None else "+masked amax"
+        _record("nchw_to_rows", "-", mode, 0.0, 0, n * h * w)
+
+    def _check_rows_to_nchw(self, a, out, pre):
+        rows, n, c, h, w = a["rows"], a["n"], a["c"], a["h"], a["w"]
+        _require(torch.equal(out, rows[:, :c].reshape(n, h, w, c).permute(0, 3, 1, 2)), "rows_to_nchw")
+        _record("rows_to_nchw", "-", "-", 0.0, 0, n * h * w)
+
+    def _check_gather_rows(self, a, rows, pre):
+        x = a["x_nchw"]
+        n, c, h, w = x.shape
+        total = n * h * w
+        max_rows = total if a["max_rows"] is None else a["max_rows"]
+        r = min(self._check_list("gather_rows", a["pixels"], a["count"], max_rows, total), max_rows)
+        xr = _nhwc(x)
+        want = xr[a["pixels"].reshape(-1)[:r].long()] if a["pixels"] is not None else xr[:r]
+        _require(torch.equal(rows[:r, :c], want), "gather_rows")
+        _record("gather_rows", "-", "-", 0.0, 0, r)
+
+    def _before_gather_rows_list(self, a):
+        return self._before_amax(a["amax"])
+
+    def _check_gather_rows_list(self, a, res, old_amax):
+        rows = res[0] if a["stream"] is not None else res
+        x = a["x"]
+        n, c, h, w = x.shape
+        total = n * h * w
+        r = self._check_list("gather_rows_list", a["pixels"], a["count"], total, total)
+        xr = _nhwc(x.to(rows.device) if not x.is_cuda else x)
+        want = xr[a["pixels"].reshape(-1)[:r].long()]
+        _require(torch.equal(rows[:r, :c], want), "gather_rows_list: rows differ from the listed pixels")
+        if rows.shape[1] > c:
+            _require(bool((rows[:r, c:] == 0).all()), "gather_rows_list: pad columns are not zero")
+        if a["amax"] is not None:
+            self._check_amax_out("gather_rows_list", old_amax, a["amax"], want)
+        _record("gather_rows_list", "-", "host" if not x.is_cuda else "device", 0.0, 0, r)
+
+    def _before_scatter_rows(self, a):
+        return a["out"].clone() if a["out"] is not None else None
+
+    def _check_scatter_rows(self, a, out, old):
+        rows, c, n, h, w = a["rows"], a["c"], a["n"], a["h"], a["w"]
+        total = n * h * w
+        max_rows = min(rows.shape[0], total) if a["max_rows"] is None else a["max_rows"]
+        r = min(self._check_list("scatter_rows", a["pixels"], a["count"], max_rows, total), max_rows)
+        want = (old if old is not None else torch.zeros_like(out)).permute(0, 2, 3, 1).reshape(total, c).clone()
+        want[a["pixels"].reshape(-1)[:r].long()] = rows[:r, :c]
+        _require(torch.equal(out, want.reshape(n, h, w, c).permute(0, 3, 1, 2)), "scatter_rows")
+        _record("scatter_rows", "-", "-", 0.0, 0, r)
+
+    def _before_amax_rows(self, a):
+        return self._before_amax(a["out"])
+
+    def _check_amax_rows(self, a, res, old):
+        x, mask = a["x"], a["mask"]
+        vals = x.reshape(x.shape[0], -1)[mask.reshape(-1) != 0] if mask is not None else x
+        self._check_amax_out("amax_rows", old, a["out"], vals)
+        _record("amax_rows", "-", "masked" if mask is not None else "all", 0.0, 0, x.shape[0])
+
+    # ------------------------------------------------------------------------------------------ backward
+    def _dz64(self, y, dy, cout, act, act_param):
+        """dy act'(y) in fp64 from the fp32 inputs (act_param as the fp32 the kernel receives)."""
+        y64, dy64 = y[:, :cout].double(), dy[:, :cout].double()
+        slope = float(torch.tensor(act_param, dtype=_f32))
+        d = {cr.ACT_NONE: torch.ones_like(y64), cr.ACT_ELU: torch.where(y64 > 0, 1.0, y64 + 1),
+             cr.ACT_LRELU: torch.where(y64 > 0, 1.0, slope), cr.ACT_SIGMOID: y64 * (1 - y64)}[act]
+        return dy64 * d
+
+    def _before_act_backward(self, a):
+        return self._before_amax(a["amax"])
+
+    def _check_act_backward(self, a, res, old_amax):
+        dz, db = res
+        cout = a["cout"]
+        want = self._dz64(a["y"], a["dy"], cout, a["act"], a["act_param"])
+        rows = want.shape[0]
+        err = _err(dz[:, :cout], want, want.abs().clamp(min=1e-38))
+        bar = ACT_BWD_ULP * EPS
+        _record("act_backward", "fp32", "dz", err, bar, rows)
+        _require(err <= bar, "%s: act_backward dz %.3g > %.3g relative" % (self.current, err, bar))
+        if a["amax"] is not None:
+            self._check_amax_out("act_backward", old_amax, a["amax"], dz[:, :cout])
+        if db is not None:
+            gb, sb = want.sum(0), want.abs().sum(0)
+            err = _err(db, gb, sb)
+            bar = conv_grad_ref.BARS["db"]
+            _record("act_backward", "fp32", "db", err, bar, rows)
+            _require(err <= bar, "%s: act_backward db err/S %.3g > %.3g" % (self.current, err, bar))
+
+    def _grad_sources(self, a, rows0, with_data):
+        x0, x1 = a.get("x0"), a.get("x1")
+        c0, c1 = a["c0"], a["c1"]
+        dev = a["dz"].device
+        x0r = x0[:, :c0] if with_data else torch.zeros(rows0, c0, dtype=_f32, device=dev)
+        x1r = None
+        if c1:
+            x1r = x1[:, :c1] if with_data else torch.zeros(a["n"] * a["h"] * a["w"], c1, dtype=_f32, device=dev)
+        return x0r, x1r
+
+    def _check_conv_wgrad(self, a, dw, pre):
+        n, h, w, taps, c0, c1, cout = a["n"], a["h"], a["w"], a["taps"], a["c0"], a["c1"], a["cout"]
+        _require(a["map0"] is None, "conv_wgrad: the harness restates dense layers only")
+        x0r, x1r = self._grad_sources(a, None, True)
+        k = 3 if taps == 9 else 1
+        wzero = torch.zeros(cout, c0 + c1, k, k, dtype=_f32, device=dw.device)
+        with torch.enable_grad():                               # the autograd backward calling this runs without
+            ref = conv_grad_ref.conv_grads(x0r, c0, x1r, c1, wzero, a["dz"][:, :cout], n, h, w, taps=taps, pad=a["pad"],
+                                           shift0=a["shift0"])
+        err = _err(dw, *ref["w"])
+        bar = conv_grad_ref.BARS["dW"]
+        _record("conv_wgrad", "tf32x3", "cout<=8" if cout <= 8 else "-", err, bar, n * h * w)
+        _require(err <= bar, "%s: conv_wgrad (n %d, %dx%d, c0 %d, c1 %d, cout %d) err/S %.3g > %.3g"
+                 % (self.current, n, h, w, c0, c1, cout, err, bar))
+
+    def _check_conv_dgrad(self, a, res, pre):
+        dx0, dx1 = res
+        n, h, w, taps, c0, c1, cout, shift0 = a["n"], a["h"], a["w"], a["taps"], a["c0"], a["c1"], a["cout"], a["shift0"]
+        wt = self._weights(a["wt_packed"])                      # W.transpose(0, 1).flip(2, 3)
+        weight = wt.flip(2, 3).transpose(0, 1)
+        rows0 = n * (h >> shift0) * (w >> shift0)
+        a = dict(a, x0=None, x1=None)
+        x0r, x1r = self._grad_sources(a, rows0, False)
+        with torch.enable_grad():
+            ref = conv_grad_ref.conv_grads(x0r, c0, x1r, c1, weight, a["dz"][:, :cout], n, h, w, taps=taps, pad=a["pad"],
+                                           shift0=shift0)
+        err0 = _err(dx0[:, :c0], *ref["x0"])
+        _require(bool((dx0[:, c0:] == 0).all()), "conv_dgrad: dx0 pad columns are not zero")
+        _record("conv_dgrad", "dx0", "taps%d" % taps, err0, conv_grad_ref.BARS["dx0"], rows0)
+        _require(err0 <= conv_grad_ref.BARS["dx0"], "%s: conv_dgrad dx0 err/S %.3g > %.3g"
+                 % (self.current, err0, conv_grad_ref.BARS["dx0"]))
+        if dx1 is not None:
+            want, s = ref["x1"]
+            err1 = _err(_nhwc(dx1), want, s)
+            _record("conv_dgrad", "dx1", "taps%d" % taps, err1, conv_grad_ref.BARS["dx1"], n * h * w)
+            _require(err1 <= conv_grad_ref.BARS["dx1"], "%s: conv_dgrad dx1 err/S %.3g > %.3g"
+                     % (self.current, err1, conv_grad_ref.BARS["dx1"]))

@@ -45,8 +45,7 @@ import conv_ref as cr
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
-BAR = {"tf32x3": 4e-5, "f16x3": 2.5e-5, "simt": 1.5e-5}
-ACT_ALLOW = 5e-7                  # absolute error of the epilogue's ELU / sigmoid
+BAR, ACT_ALLOW = cr.BAR, cr.ACT_ALLOW
 SENTINEL = -3.0e38                # never produced by these layers
 PAD_GARBAGE = 1.0e6               # padding columns of the source rows (must not be read)
 ENGINES = ["tf32x3", "f16x3", "simt"]

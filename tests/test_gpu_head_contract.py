@@ -49,9 +49,8 @@ import head_ref as hr
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
-BAR = {"head_conv3x3": 4e-7, "head_gather": 4.5e-7, "head_idwt": 4.5e-7, "head_mlp": 4e-6}
-BILINEAR_ULP = 2.5                # units of 2^-23 x the largest |disp| around the four neighbours
-ACT_ALLOW = 5e-7                  # absolute error of the kernels' expf-based sigmoid / ELU
+BAR, BILINEAR_ULP = hr.BAR, hr.BILINEAR_ULP
+ACT_ALLOW = cr.ACT_ALLOW          # absolute error of the kernels' expf-based sigmoid / ELU
 SENTINEL = -3.0e38                # never produced by these kernels
 PAD_GARBAGE = 1.0e6               # source columns a launch must not read
 DISTS = ["mixed", "same"]
@@ -548,23 +547,8 @@ def _bilinear_case(n, c, h, w, size, ac, clamp01, scale, seed):
     hf = _uniform((n, c, 3, h, w), -2.0, 2.0, g)
     got = ops.idwt_bilinear(ll, hf, size, disp_scale=scale, clamp01=clamp01, align_corners=ac)
     _, disp = ops.idwt_haar(ll, hf, disp_scale=scale, clamp01=clamp01)
-    want = F.interpolate(disp, size=size, mode="bilinear", align_corners=ac)
-    # a few ulp of the largest of the four neighbours: bound by the largest |disp| of the 3 x 3 window around the
-    # top-left neighbour
-    hs, ws = disp.shape[-2:]
-    m = F.max_pool2d(disp.abs(), 3, stride=1, padding=1)
-    ys, xs = torch.arange(size[0], device=DEV, dtype=torch.float64), torch.arange(size[1], device=DEV, dtype=torch.float64)
-    if ac:
-        fy = ys * ((hs - 1) / max(size[0] - 1, 1))
-        fx = xs * ((ws - 1) / max(size[1] - 1, 1))
-    else:
-        fy = ((ys + 0.5) * (hs / size[0]) - 0.5).clamp(min=0)
-        fx = ((xs + 0.5) * (ws / size[1]) - 0.5).clamp(min=0)
-    y0, x0 = fy.floor().long().clamp(max=hs - 1), fx.floor().long().clamp(max=ws - 1)
-    mag = m[:, :, y0][:, :, :, x0]
-    ulps = float(((got - want).abs() / (mag * 2.0 ** -23).clamp(min=1e-38)).max())
+    ulps = hr.bilinear_ulps(got, disp, size, ac)
     _record("idwt_bilinear", "ulp", "mixed", ulps)
-    assert got.shape == want.shape
     assert ulps <= BILINEAR_ULP, ulps
 
 
