@@ -186,14 +186,19 @@ typedef struct wmd_conv_desc {
                                only the rows of the listed pixels (sparse_upsample's skip[mask], KITTI/layers.py:500, kept
                                compact: wmd_gather_rows_list_f32) */
   int32_t precision;        /* tensor-core engine only.  0 = WMD_PREC_TF32X3: operands split into tf32 hi + lo.  1 = WMD_PREC_F16X3:
-                               operands split into two fp16 pieces of x * 2^k (same 22 mantissa bits; k from amax0 / amax1, so
-                               nothing overflows) - half the MMA instructions and twice their rate; needs amax0 (and amax1 when
-                               c1 > 0) and weights packed by wmd_pack_conv_weight_tc16_f32.  The Python KITTI decoders use
-                               F16X3 by default; launches without source maxima use TF32X3 */
-  const float* amax0;       /* device scalars: max |x0|, max |x1| over the rows the launch can read (upper bounds are fine) */
+                               operands split into two fp16 pieces of x * 2^k - half the MMA instructions and twice their
+                               rate; needs amax0 (and amax1 when c1 > 0) and weights packed by wmd_pack_conv_weight_tc16_f32.
+                               k puts max(amax0, amax1) into [2^13, 2^14) (one k for both sources and every frame; the weights
+                               get their own from max |w|), so no finite operand overflows.  The pair carries tf32x3's 22
+                               mantissa bits only for operands within 2^-11 of their maximum: below that the low piece is an
+                               fp16 subnormal, whose absolute error is 2^-25 of a scaled unit.  See the bound below.  The
+                               Python KITTI decoders use F16X3 by default; launches without source maxima use TF32X3 */
+  const float* amax0;       /* device scalars: max |x0|, max |x1| over the finite values of the rows the launch can read
+                               (upper bounds are fine) */
   const float* amax1;
-  float* amax_out;          /* device scalar, or NULL: atomically raised to max |y| of the rows written (zero it before the
-                               first producer; both precisions, every scheduling mode) */
+  float* amax_out;          /* device scalar, or NULL: atomically raised to max |y| over the finite y of the rows written
+                               (zero it before the first producer; both precisions, every scheduling mode).  Every maximum
+                               libwmd produces skips NaN and +-Inf, so one non-finite value leaves the scales of the rest */
   int32_t rows0;            /* rows allocated in x0, 0 = unknown.  Only used by the tensor-core engine's 1x1 form (taps == 1,
                                map0 == NULL: output row m reads x0 row m): with rows0 > 0 rows past rows0 read zeros */
 } wmd_conv_desc;
@@ -202,8 +207,14 @@ int wmd_conv_rows_f32(const wmd_conv_desc* d, wmd_stream_t stream);
 
 /* Tensor-core engine for the same contract: wgmma tf32 with a 3xTF32 split (hi*hi + lo*hi + hi*lo,
  * fp32 accumulation), so results stay fp32-faithful: |y - exact| <= 1.7e-5 S, S = |bias| + sum |x w| of the element's
- * terms (measured worst, same-sign operands, H100; f16x3: 8.6e-6 S, the SIMT kernel: 6.5e-6 S at K = 18432).  d->w must
- * point to weights packed by wmd_pack_conv_weight_tc_f32 for the same (cout, c0, c1, taps); d->ldw is ignored.
+ * terms (measured worst, same-sign operands, H100; f16x3: 8.6e-6 S for operands within 2^-11 of their maxima, the SIMT
+ * kernel: 6.5e-6 S at K = 18432).  f16x3 in general: |y - exact| <= 2.5e-5 S + F, with the absolute floor
+ *   F = 2^-25 (sum |w| over the nonzero x / s_x + sum |x| over the nonzero w / s_w) + 2^-50 K' / (s_x s_w) + 2^-149
+ * (s_x, s_w the two scales, K' the number of terms with both factors nonzero): each operand's split is off by at most
+ * 2^-22 of itself or 2^-25 / s, whichever is larger (tests/conv_ref.py derives it).  Non-finite inputs: an output is
+ * non-finite exactly where the fp64 contract's is (the rows whose taps read a NaN or +-Inf), though the tensor-core
+ * engines may give NaN where the contract gives +-Inf (the split's remainder is Inf - Inf); other rows are unaffected.
+ * d->w must point to weights packed by wmd_pack_conv_weight_tc_f32 for the same (cout, c0, c1, taps); d->ldw is ignored.
  *   wmd_conv_tc_tile_n(cout)                 N-tile of the kernel for this cout (128 / 64 / 32; the CTA tile is 128 rows x N)
  *   wmd_conv_tc_weight_floats(...)           size of the packed weight buffer, in floats
  *   wmd_pack_conv_weight_tc_f32(w, packed..) (Cout, c0+c1, kh, kw) -> per (n-tile, 32-channel chunk) fp32
@@ -217,9 +228,10 @@ int wmd_conv_rows_f32(const wmd_conv_desc* d, wmd_stream_t stream);
  * per tap; the results are bit-identical to the gather kernel's. */
 enum { WMD_PREC_TF32X3 = 0, WMD_PREC_F16X3 = 1 };
 int wmd_conv_tc_tile_n(int cout);
-/* Weights for precision = WMD_PREC_F16X3: 128-byte header (float 0: 1 / s_w) + per (n-tile, 32-channel chunk) one N x 128 B
- * image whose rows hold [fp16(w s_w): 32 channels | fp16(w s_w - that): 32 channels], s_w = the power of two that puts
- * max |w| into (2^13, 2^14] (computed on the device, no host sync).  `packed` needs wmd_conv_tc16_weight_bytes() bytes. */
+/* Weights for precision = WMD_PREC_F16X3: 128-byte header (float 0: 1 / s_w, float 1: max |w|, int 2: e_w = log2 s_w) +
+ * per (n-tile, 32-channel chunk) one N x 128 B image whose rows hold [fp16(w s_w): 32 channels | fp16(w s_w - that): 32
+ * channels], s_w = 2^e_w the power of two that puts max |w| over the finite w into [2^13, 2^14), e_w <= 127 (computed
+ * on the device, no host sync).  `packed` needs wmd_conv_tc16_weight_bytes() bytes. */
 size_t wmd_conv_tc16_weight_bytes(int cout, int c0, int c1, int taps);
 int wmd_pack_conv_weight_tc16_f32(const float* w, void* packed, int Cout, int c0, int c1, int taps, wmd_stream_t stream);
 /* max |x| of `count` floats, atomically raised into *amax (device scalar, zero it first): for sources that no libwmd

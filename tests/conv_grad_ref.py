@@ -39,3 +39,28 @@ def conv_grads(x0, c0, x1, c1, weight, dz, n, h, w, taps=9, pad=conv_ref.PAD_REF
     out = {"x0": (g[0], s[0]), "w": (g[2], s[2]), "b": (dz64.sum(0), dz64.abs().sum(0))}
     out["x1"] = (g[1], s[1]) if x1 is not None else None
     return out
+
+
+def dgrad_floor(c0, c1, weight, dz, n, h, w, amax_dz, taps=9, pad=conv_ref.PAD_REFLECT, shift0=0, block_elems=1 << 24):
+    """The absolute floor F of the f16x3 data gradient (conv_ref, the f16x3 bound), per element of dx0 and dx1 (rows).
+
+    The data gradient is the forward contract run on dz (scaled by amax_dz) with the flipped, transposed weights, whose
+    scale comes from the same max |W|; a folded element is a sum of up to four such outputs.  So F is the adjoint
+    applied to the floor's terms: 2^-25 (|W| over dz != 0 / s_dz + |dz| over W != 0 / s_w) + 2^-50 (count) / (s_dz s_w),
+    plus 2^-149 for each of the up to four fp32 outputs the fold adds.  Returns {'x0': F0, 'x1': F1 or None}."""
+    block_rows = max(1, block_elems // max(taps * (c0 + c1), 1))
+    s_x, s_w = conv_ref.f16_scale(amax_dz), conv_ref.f16_scale(conv_ref.finite_max(weight))
+    rows0 = n * (h >> shift0) * (w >> shift0)
+    x0 = torch.zeros(rows0, c0, dtype=_f64, device=dz.device)
+    x1 = torch.zeros(n * h * w, c1, dtype=_f64, device=dz.device) if c1 else None
+    nz_w, nz_dz = (weight != 0).to(_f64), (dz != 0).to(_f64)
+
+    def adj(wt, d):
+        with torch.enable_grad():               # also from a backward pass, where autograd records nothing
+            return _adjoint(x0, c0, x1, c1, wt, d, n, h, w, taps, pad, shift0, block_rows)[:2]
+
+    a, b, c = adj(weight.abs(), nz_dz), adj(nz_w, dz.abs()), adj(nz_w, nz_dz)
+    floor = conv_ref.F16_FLOOR
+    out = [floor * (a[i] / s_x + b[i] / s_w) + floor ** 2 * c[i] / (s_x * s_w) + 4 * 2.0 ** -149 if a[i] is not None
+           else None for i in range(2)]
+    return {"x0": out[0], "x1": out[1]}

@@ -11,6 +11,8 @@ small multiple of 2^-22 S whatever the signs of the operands.
 Independent of libwmd and ops.*: index maps are applied with torch indexing, the work is cut into row blocks so that
 K = 9 x 2048 fits in memory, and it runs on whatever device the inputs live on.
 """
+import math
+
 import torch
 
 PAD_ZERO, PAD_REFLECT, PAD_REPLICATE = 0, 1, 2
@@ -20,6 +22,47 @@ _f64 = torch.float64
 # err / S bars of the three engines (the error model and the measurements behind them: tests/test_gpu_conv_contract.py)
 BAR = {"tf32x3": 4e-5, "f16x3": 2.5e-5, "simt": 1.5e-5}
 ACT_ALLOW = 5e-7                  # absolute error of the kernels' expf-based ELU / sigmoid epilogues
+
+
+# f16x3 bound: |y - y64| <= BAR["f16x3"] S + F per element.  Derivation (conv_tc.cu, load_frag / pack_weight_tc16_kernel):
+# an operand v of a launch is scaled by s = 2^e (f16_scale_exp of its maximum: the larger of amax0 / amax1 for the
+# activations, max |w| for the weights), v' = v s with |v'| < 2^14, and split h1 = fp16(v'), h2 = fp16(v' - h1) (the
+# remainder is exact in fp32).  fp16 has 11 significant bits down to 2^-14 and a fixed spacing of 2^-24 below, so each
+# rounding is off by at most 2^-11 of its operand or 2^-25, whichever is larger; h2's error is then at most
+# max(2^-22 |v'|, 2^-25):  |dv| <= 2^-22 |v| + 2^-25 / s, and dv = 0 for v = 0.  The kernel forms
+# h1x h1w + h1x h2w + h2x h1w = (x + dx)(w + dw) - h2x h2w, off from x w by
+#   dx w + x dw + dx dw - h2x h2w.
+# The relative parts (2^-22 |x w| each, and |h2x h2w| <= 2^-22 |x w|) and the fp32 accumulation of the products in scaled
+# units are what the relative bar covers; what is left is the absolute part
+#   F = 2^-25 (sum_{x != 0} |w| / s_x + sum_{w != 0} |x| / s_w) + 2^-50 K' / (s_x s_w)
+# (K' = terms with x != 0 and w != 0; the mixed products 2^-22 |x| 2^-25 / s_w are 2^-22 of F), plus 2^-149 for the
+# one rounding of y = acc 2^-(e + e_w) + bias where y is an fp32 subnormal.  Within 2^-11 of both maxima, F is below
+# 2^-22 S and the pair carries tf32x3's 22 bits; at 2^-m of a maximum F is ~2^(m - 25) of that operand's terms in S.
+F16_FLOOR = 2.0 ** -25
+
+
+def f16_scale(m):
+    """The power-of-two operand scale of an fp16-pair launch whose maximum is m (f16_scale_exp in csrc/conv_tc.cu):
+    m s in [2^13, 2^14), the exponent clamped to [-126, 127]; m = 0 or non-finite: 1."""
+    m = float(m)
+    e = 0
+    if 0.0 < m < float("inf"):
+        e = 14 - math.frexp(m)[1]
+    return 2.0 ** max(-126, min(127, e))
+
+
+def f16_floor(a, wk, s_x, s_w):
+    """F of the f16x3 bound (derivation above) for gathered rows a (rows, K) and weights wk (K, cout), float64."""
+    nza, nzw = (a != 0).to(_f64), (wk != 0).to(_f64)
+    return (F16_FLOOR * (nza @ wk.abs() / s_x + a.abs() @ nzw / s_w) + F16_FLOOR ** 2 * (nza @ nzw) / (s_x * s_w)
+            + 2.0 ** -149)
+
+
+def finite_max(t):
+    """max |t| over the finite values (0 if none): what every libwmd maximum producer reports."""
+    a = t.detach().abs()
+    a = a[torch.isfinite(a)]
+    return float(a.max()) if a.numel() else 0.0
 
 
 def _pad_coord(q, n, pad):
@@ -43,10 +86,10 @@ def activate(y, act, act_param=0.0):
 
 
 def _take(x, rows, c):
-    """x[rows, :c] in float64 with rows < 0 reading zeros."""
+    """x[rows, :c] in float64 with rows < 0 reading zeros (not 0 * x[0]: that row may hold a NaN or an Inf)."""
     ok = rows >= 0
     v = x[rows.clamp(min=0), :c].to(_f64)
-    return v * ok.unsqueeze(-1)
+    return torch.where(ok.unsqueeze(-1), v, torch.zeros((), dtype=_f64, device=v.device))
 
 
 def gather_rows(m, x0, c0, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0, x1=None, c1=0, map1=None, gate=None,
@@ -88,12 +131,14 @@ def gather_rows(m, x0, c0, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0
 
 def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NONE, act_param=0.0, map0=None, shift0=0,
              x1=None, c1=0, map1=None, gate=None, pixels=None, count=None, max_rows=None, rows0=None, block_elems=1 << 24,
-             read_max=False):
+             read_max=False, f16_amax=None):
     """(y64, S) for rows [0, min(count, max_rows)): the arguments of ops.conv_rows, with a plain (cout, c0 + c1, k, k)
     weight and an optional bias (cout,).  count: int or 1-element tensor (with pixels); rows0 (taps == 1, map0 None
     only): rows x0 holds, rows past it read zeros (default: x0.shape[0]).
     read_max: also return the largest |value| the launch reads from source 0 and from source 1 (the maxima its fp16-pair
-    operand scales must cover): (y64, S, max0, max1)."""
+    operand scales must cover): (y64, S, max0, max1).  Non-finite values count as 0 there, as in the kernels.
+    f16_amax: the activation maximum an f16x3 launch scales by (the larger of its amax0 / amax1 scalars): also return F,
+    the absolute floor of the f16x3 bound (f16_floor; the weight scale follows from the finite max |weight|), last."""
     dev = x0.device
     cout = weight.shape[0]
     rows = int(count) if pixels is not None else n * h * w
@@ -107,20 +152,28 @@ def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NON
     b = bias.to(dev, _f64) if bias is not None else torch.zeros(cout, dtype=_f64, device=dev)
     y64 = torch.empty(rows, cout, dtype=_f64, device=dev)
     s = torch.empty(rows, cout, dtype=_f64, device=dev)
+    if f16_amax is not None:
+        s_x, s_w = f16_scale(f16_amax), f16_scale(finite_max(weight))
+        floor = torch.empty(rows, cout, dtype=_f64, device=dev)
     step = max(1, block_elems // max(k, 1))
     max0 = max1 = 0.0
     for r in range(0, rows, step):
         m = torch.arange(r, min(rows, r + step), device=dev)
         a = gather_rows(m, x0, c0, n, h, w, taps, pad, map0, shift0, x1, c1, map1, gate, pixels, rows0)
         if read_max:
-            max0 = max(max0, float(a[..., :c0].abs().max()) if c0 else 0.0)
-            max1 = max(max1, float(a[..., c0:].abs().max()) if c1 else 0.0)
+            max0 = max(max0, finite_max(a[..., :c0]) if c0 else 0.0)
+            max1 = max(max1, finite_max(a[..., c0:]) if c1 else 0.0)
         a = a.reshape(len(m), k)
         y64[r:r + len(m)] = a @ wk + b
         s[r:r + len(m)] = a.abs() @ wa + b.abs()
+        if f16_amax is not None:
+            floor[r:r + len(m)] = f16_floor(a, wk, s_x, s_w)
+    out = (activate(y64, act, act_param), s)
     if read_max:
-        return activate(y64, act, act_param), s, max0, max1
-    return activate(y64, act, act_param), s
+        out += (max0, max1)
+    if f16_amax is not None:
+        out += (floor,)
+    return out
 
 
 def index_map(mask):

@@ -4,6 +4,8 @@ The GPU contract tests (test_gpu_conv_contract.py) measure the kernels' error ag
 right on its own: every gather path it restates is checked here against an independent formulation, exactly (fp64
 sums of the same products in a different order: <= 1e-12 relative).
 """
+import math
+
 import numpy as np
 import pytest
 import torch
@@ -142,3 +144,81 @@ def test_count_and_max_rows():
     assert y8.shape == (8, cout) and torch.equal(y5, y8[:5]) and y0.shape == (0, cout)
     dense, _ = cr.conv_ref(rows_of(x), cin, wt, b, n, h, w)
     assert torch.equal(y8, dense[pix.long()])
+
+
+# ------------------------------------------------------------------------------------------ the f16x3 bound
+def _emulate_f16x3(x, w, amax, wmax):
+    """x (R, K) @ w (K, cout) as the f16x3 engine forms it, in fp64: each operand scaled by its launch's power of two,
+    split into h1 = fp16(v s) and h2 = fp16(v s - h1) (torch float16 casts: round to nearest even, with subnormals), the
+    three products h1 h1 + h1 h2 + h2 h1 summed exactly, the scales undone.  No tensor-core accumulation: this checks the
+    split part of the bound only."""
+    s_x, s_w = cr.f16_scale(amax), cr.f16_scale(wmax)
+
+    def split(v, s):
+        v = (v.double() * s).float()                  # a power of two: exact
+        h1 = v.half().float()
+        h2 = (v - h1).half().float()                  # the remainder is exact in fp32
+        return h1.double(), h2.double()
+
+    x1, x2 = split(x, s_x)
+    w1, w2 = split(w, s_w)
+    return (x1 @ w1 + x1 @ w2 + x2 @ w1) / (s_x * s_w)
+
+
+def _split_err(x, w, amax, wmax):
+    """(|emulated - exact|, S, F) per element."""
+    want = x.double() @ w.double()
+    err = (_emulate_f16x3(x, w, amax, wmax) - want).abs()
+    return err, x.double().abs() @ w.double().abs(), cr.f16_floor(x.double(), w.double(), cr.f16_scale(amax),
+                                                                   cr.f16_scale(wmax))
+
+
+REL_SPLIT = 2.0 ** -20            # the split's relative part: 2^-22 for dx, dw and h2x h2w each, with room
+
+
+@pytest.mark.parametrize("top", [-140, -126, -60, 0, 60, 116, 127])
+@pytest.mark.parametrize("side", ["x", "w"])
+def test_f16x3_floor_bounds_the_emulated_split(top, side):
+    """Rows (or output channels) at 2^-m of the launch maximum 2^top, m = 0 .. 45, mixed signs, K = 64: the emulated
+    split never leaves 2^-20 S + F, and F is what lets it - a plain relative bar fails from m ~ 22 on."""
+    g = torch.Generator().manual_seed(top + 200)
+    ms = torch.arange(46, dtype=torch.float64)
+    x = torch.rand(46, 64, generator=g, dtype=torch.float64) * 2 - 1
+    w = torch.rand(64, 46, generator=g, dtype=torch.float64) * 2 - 1
+    if side == "x":
+        x = x * torch.exp2(top - ms)[:, None]
+        x[0, 0] = 2.0 ** top                          # the maximum sits in row 0
+        w[0, 0] = 1.0
+    else:
+        w = w * torch.exp2(top - ms)[None, :]
+        w[0, 0] = 2.0 ** top
+        x[0, 0] = 1.0
+    x, w = x.float(), w.float()
+    err, s, f = _split_err(x, w, cr.finite_max(x), cr.finite_max(w))
+    assert bool((err <= REL_SPLIT * s + f).all()), float((err / (REL_SPLIT * s + f)).max())
+    if top >= -60:                                    # the deep rows are normal fp32 numbers: the relative bar alone fails
+        assert float((err / s)[s > 0].max()) > cr.BAR["f16x3"]
+
+
+def test_f16x3_floor_is_tight():
+    """One term per element (K = 1), x at 2^-m of its maximum with m = 24 .. 36: there the low piece is an fp16
+    subnormal and the split's error reaches F within a factor of 2 (4096 samples per m); past m ~ 38 x s drops under
+    fp16's smallest subnormal and the error is |x w| itself, below F."""
+    g = torch.Generator().manual_seed(7)
+    w = (torch.rand(1, 32, generator=g) * 0.5 + 0.5)
+    for m in range(24, 37):
+        x = (torch.rand(4096, 1, generator=g, dtype=torch.float64) * 0.5 + 0.5) * 2.0 ** -m
+        x[0, 0] = 1.0
+        err, s, f = _split_err(x.float(), w, 1.0, cr.finite_max(w))
+        ratio = (err / (REL_SPLIT * s + f))[1:]
+        assert float(ratio.max()) <= 1.0 and float(ratio.max()) >= 0.5, (m, float(ratio.max()))
+
+
+def test_f16_scale_matches_the_kernel_rule():
+    """m s in [2^13, 2^14) for every finite m > 0, the exponent clamped to [-126, 127]; 0 and non-finite maxima: 1."""
+    for m in [2.0 ** -149, 2.0 ** -126, 1e-30, 0.3, 1.0, 8191.9, 2.0 ** 116, 3.4e38]:
+        s = cr.f16_scale(m)
+        e = math.log2(s)
+        assert e == int(e) and -126 <= e <= 127
+        assert m * s < 2.0 ** 14 and (m * s >= 2.0 ** 13 or e == 127)
+    assert cr.f16_scale(0.0) == cr.f16_scale(float("inf")) == cr.f16_scale(float("nan")) == 1.0

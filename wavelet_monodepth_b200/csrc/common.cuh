@@ -65,6 +65,14 @@ __device__ __forceinline__ float expm1_nonpos(float v) {
   return v > -0.25f ? near0 : e - 1.f;
 }
 
+// |v| for finite v, 0 for +-Inf and NaN: the operand of every max |x| that sets an fp16-pair scale.  One non-finite value
+// must not change the scale, and with it the bits, of every other value in the launch (an Inf max would leave the whole
+// launch unscaled); the non-finite value itself still reaches the output through the split (wmd.h, precision).
+__device__ __forceinline__ float finite_abs(float v) {
+  const float a = fabsf(v);
+  return a < INFINITY ? a : 0.f;
+}
+
 __device__ __forceinline__ float activate(float v, int act, float p) {
   switch (act) {
     case WMD_ACT_ELU: return v > 0.f ? v : expm1_nonpos(v);

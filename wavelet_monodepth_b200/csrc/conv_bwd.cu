@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(AB_THREADS) act_bwd_kernel(const float* __rest
         const float g = dy[static_cast<long long>(r) * lddy + c] * act_grad(y[static_cast<long long>(r) * ldy + c], act, p);
         dz[static_cast<long long>(r) * lddz + c] = g;
         s += g;
-        vmax = fmaxf(vmax, fabsf(g));
+        vmax = fmaxf(vmax, finite_abs(g));
       }
     }
     red[rl][lane] = s;

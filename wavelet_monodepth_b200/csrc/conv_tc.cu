@@ -294,11 +294,12 @@ template <> struct Wgmma<32, true> {
   }
 };
 
-// two floats -> packed fp16 pair, round to nearest even, saturating at +-65504 (a stray out-of-range value must not turn
-// into inf - inf = NaN in the remainder piece); `lo` lands in bits 0..15 (the lower K index)
+// two floats -> packed fp16 pair, round to nearest even; `lo` lands in bits 0..15 (the lower K index).  Not saturating:
+// the operand scale keeps every finite value below 2^14, and an infinite one must stay infinite (its remainder piece is
+// then Inf - Inf = NaN, so the output is non-finite where the contract's is; saturation made it a finite 131008 2^-e)
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   uint32_t r;
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;\n" : "=r"(r) : "f"(hi), "f"(lo));
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;\n" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
 __device__ __forceinline__ float f16_lo_to_f32(uint32_t pair) {
@@ -310,6 +311,20 @@ __device__ __forceinline__ float f16_hi_to_f32(uint32_t pair) {
   float f;
   asm("{\n\t.reg .f16 l, h;\n\tmov.b32 {l, h}, %1;\n\tcvt.f32.f16 %0, h;\n\t}\n" : "=f"(f) : "r"(pair));
   return f;
+}
+
+// Exponent e of the power-of-two scale of an fp16-pair operand whose (finite-value) maximum is m: m 2^e in [2^13, 2^14),
+// so no finite operand overflows fp16 and the low piece h2 = fp16(v 2^e - h1) stays normal for every |v| >= 2^-11 m.
+// e is clamped to [-126, 127], where 2^e is a normal float: for finite m only the upper end is reached (m < 2^-113),
+// and then m 2^e < 2^14 still.  m = 0 or non-finite: e = 0.
+__host__ __device__ __forceinline__ int f16_scale_exp(float m) {
+  int e = 0;
+  if (m > 0.f && m < INFINITY) {
+    int ex;
+    frexpf(m, &ex);                              // m = f * 2^ex, f in [0.5, 1)
+    e = 14 - ex;
+  }
+  return e < -126 ? -126 : (e > 127 ? 127 : e);
 }
 
 __device__ __forceinline__ float tf32_rna(float x) {
@@ -622,22 +637,24 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
   const int ctid = tid - TC_PRODUCERS;
 
   // F16: operands are fed as fp16 pairs.  Activations are scaled by a power of two chosen from the sources' max |x| (device
-  // scalars written by their producers: layout moves, earlier convolutions) so that max |x| s lies in (2^13, 2^14] - no
-  // overflow, the low piece stays normal for everything within 2^-11 .. 1 of the maximum; weights carry their own
-  // power-of-two scale in the packed image's header.  Both scales are undone exactly in the epilogue.
-  float ascale = 1.f, out_scale = 1.f;
+  // scalars written by their producers: layout moves, earlier convolutions) so that max |x| s lies in [2^13, 2^14)
+  // (f16_scale_exp) - no overflow, the low piece stays normal for everything within 2^-11 .. 1 of the maximum; weights
+  // carry their own power-of-two scale in the packed image's header.  Both scales are undone exactly in the epilogue:
+  // y = acc 2^-(e + e_w) + bias = fma(acc, out_scale, bias) with out_scale = 2^k2, k2 = -(e + e_w) clamped to the
+  // float powers of two [2^-149, 2^127]; the rest, 2^k1, is applied to the sums first (out_pre), in a branch off the
+  // per-element path.  For finite maxima e and e_w lie in [-114, 127], so k is in [-254, 228] and k1 in [-105, 101];
+  // k1 < 0 needs the product of the two maxima below about 2^-121, k1 > 0 needs it above about 2^154: there the
+  // largest terms x w leave fp32, and so does the exact result of any row that reads them.
+  float ascale = 1.f, out_scale = 1.f, out_pre = 1.f;
   if (F16) {
     float amax = d.amax0 ? __ldg(d.amax0) : 0.f;
     if (d.c1 > 0 && d.amax1) amax = fmaxf(amax, __ldg(d.amax1));
-    int e = 0;
-    if (amax > 0.f && amax < INFINITY) {
-      int ex;
-      frexpf(amax, &ex);                         // amax = m * 2^ex, m in [0.5, 1)
-      e = 14 - ex;                               // amax * 2^e in [2^13, 2^14)
-    }
-    e = max(-100, min(100, e));
+    const int e = f16_scale_exp(amax);
     ascale = ldexpf(1.f, e);
-    out_scale = ldexpf(1.f, -e) * __ldg(wtc);    // header word 0: 1 / weight scale
+    const int k = -(e + __ldg(reinterpret_cast<const int*>(wtc) + 2));   // header word 2: e_w, the weight scale's exponent
+    const int k2 = max(-149, min(127, k));
+    out_scale = ldexpf(1.f, k2);
+    out_pre = ldexpf(1.f, k - k2);
   }
 
   // fragment ownership: consumer warpgroup wg, warp wq of it; rows row_a and row_a + 8 of the tile, columns 8j + 2 t4 + {0, 1}
@@ -795,6 +812,10 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
     g += len;
     if (WIN) wc = win_of(len - 1) + 1;
 
+    if (F16 && whole && out_pre != 1.f) {
+#pragma unroll
+      for (int j = 0; j < ACC; ++j) acc[j] *= out_pre;
+    }
     // ---- epilogue: bias, activation, pair stores.  acc[4 j + 2 h + e] = row row_a + 8 h, column 8 j + 2 t4 + e
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -833,7 +854,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
                 o.x = a0 + bq.x; o.y = a1 + bq.y;
               }
               o.x = actf(o.x); o.y = actf(o.y);
-              out_max = fmaxf(out_max, fmaxf(fabsf(o.x), fabsf(o.y)));
+              out_max = fmaxf(out_max, fmaxf(finite_abs(o.x), finite_abs(o.y)));
               *reinterpret_cast<float2*>(yr + co) = o;
             } else {
 #pragma unroll
@@ -841,7 +862,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
                 if (co + e < d.cout) {
                   const float a = F16 ? __fmul_rn(e ? a1 : a0, out_scale) : (e ? a1 : a0);
                   const float o = actf(a + (d.bias ? __ldg(d.bias + co + e) : 0.f));
-                  out_max = fmaxf(out_max, fabsf(o));
+                  out_max = fmaxf(out_max, finite_abs(o));
                   yr[co + e] = o;
                 }
               }
@@ -923,20 +944,21 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
             if (live[q]) {
               float4 o = v[q];
               if (F16) {
+                if (out_pre != 1.f) { o.x *= out_pre; o.y *= out_pre; o.z *= out_pre; o.w *= out_pre; }
                 o.x = __fadd_rn(__fmul_rn(o.x, out_scale), bq[q].x); o.y = __fadd_rn(__fmul_rn(o.y, out_scale), bq[q].y);
                 o.z = __fadd_rn(__fmul_rn(o.z, out_scale), bq[q].z); o.w = __fadd_rn(__fmul_rn(o.w, out_scale), bq[q].w);
               }
               o.x = activate(o.x, d.act, ap); o.y = activate(o.y, d.act, ap);
               o.z = activate(o.z, d.act, ap); o.w = activate(o.w, d.act, ap);
               float* yq = d.y + static_cast<long long>(m0 + r[q]) * d.ldy + co[q];
-              out_max = fmaxf(out_max, fabsf(o.x));
+              out_max = fmaxf(out_max, finite_abs(o.x));
               if (co[q] + 3 < d.cout) {                // balanced mode requires ldy % 4 == 0 and a 16-byte aligned y
-                out_max = fmaxf(fmaxf(out_max, fabsf(o.y)), fmaxf(fabsf(o.z), fabsf(o.w)));
+                out_max = fmaxf(fmaxf(out_max, finite_abs(o.y)), fmaxf(finite_abs(o.z), finite_abs(o.w)));
                 *reinterpret_cast<float4*>(yq) = o;
               } else {
                 yq[0] = o.x;
-                if (co[q] + 1 < d.cout) { yq[1] = o.y; out_max = fmaxf(out_max, fabsf(o.y)); }
-                if (co[q] + 2 < d.cout) { yq[2] = o.z; out_max = fmaxf(out_max, fabsf(o.z)); }
+                if (co[q] + 1 < d.cout) { yq[1] = o.y; out_max = fmaxf(out_max, finite_abs(o.y)); }
+                if (co[q] + 2 < d.cout) { yq[2] = o.z; out_max = fmaxf(out_max, finite_abs(o.z)); }
               }
             }
           }
@@ -1052,14 +1074,14 @@ __global__ void tc_reduce_kernel(const float* __restrict__ partial, int splits, 
       }
       v.x = activate(v.x, act, act_param); v.y = activate(v.y, act, act_param);
       v.z = activate(v.z, act, act_param); v.w = activate(v.w, act, act_param);
-      out_max = fmaxf(out_max, fabsf(v.x));
+      out_max = fmaxf(out_max, finite_abs(v.x));
       if (co + 3 < cout) {
-        out_max = fmaxf(fmaxf(out_max, fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
+        out_max = fmaxf(fmaxf(out_max, finite_abs(v.y)), fmaxf(finite_abs(v.z), finite_abs(v.w)));
         *reinterpret_cast<float4*>(y + o) = v;
       } else {
         y[o] = v.x;
-        if (co + 1 < cout) { y[o + 1] = v.y; out_max = fmaxf(out_max, fabsf(v.y)); }
-        if (co + 2 < cout) { y[o + 2] = v.z; out_max = fmaxf(out_max, fabsf(v.z)); }
+        if (co + 1 < cout) { y[o + 1] = v.y; out_max = fmaxf(out_max, finite_abs(v.y)); }
+        if (co + 2 < cout) { y[o + 2] = v.z; out_max = fmaxf(out_max, finite_abs(v.z)); }
       }
     }
   }
@@ -1073,7 +1095,7 @@ __global__ void tc_reduce_kernel(const float* __restrict__ partial, int splits, 
 __global__ void absmax_kernel(const float* __restrict__ x, long long count, float* __restrict__ out) {
   float m = 0.f;
   const long long step = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += step) m = fmaxf(m, fabsf(__ldg(x + i)));
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < count; i += step) m = fmaxf(m, finite_abs(__ldg(x + i)));
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > __ldcg(out)) atomicMax(reinterpret_cast<unsigned*>(out), __float_as_uint(m));
 }
@@ -1093,7 +1115,7 @@ __global__ void absmax_rows_masked_kernel(const float* __restrict__ x, long long
       const int b = __ffs(marked) - 1;
       marked &= marked - 1;
       const float* row = x + (r0 + b) * cols;
-      for (int c = lane; c < cols; c += 32) m = fmaxf(m, fabsf(__ldg(row + c)));
+      for (int c = lane; c < cols; c += 32) m = fmaxf(m, finite_abs(__ldg(row + c)));
     }
   }
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -1104,15 +1126,8 @@ __global__ void absmax_rows_masked_kernel(const float* __restrict__ x, long long
 // (finish_header) so that every pack thread reads the same maximum.
 __global__ void pack_weight_tc16_kernel(const float* __restrict__ w, unsigned char* __restrict__ out, int Cout, int c0, int c1,
                                         int taps, int BN, long long total) {
-  const float wmax = *reinterpret_cast<const float*>(out);        // header word 0: max |w| (absmax_kernel)
-  int e = 0;
-  if (wmax > 0.f && wmax < INFINITY) {
-    int ex;
-    frexpf(wmax, &ex);
-    e = 14 - ex;
-  }
-  e = max(-100, min(100, e));
-  const float sw = ldexpf(1.f, e);
+  const float wmax = *reinterpret_cast<const float*>(out);        // header word 0: max |w| over finite w (absmax_kernel)
+  const float sw = ldexpf(1.f, f16_scale_exp(wmax));
   const int nch0 = (c0 + TC_BK - 1) / TC_BK, nch1 = (c1 + TC_BK - 1) / TC_BK;
   const int per_tap = nch0 + nch1;
   const int nchunks = taps * per_tap;
@@ -1149,15 +1164,10 @@ __global__ void pack_weight_tc16_kernel(const float* __restrict__ w, unsigned ch
 __global__ void finish_header_tc16_kernel(unsigned char* out) {
   float* h = reinterpret_cast<float*>(out);
   const float wmax = h[0];
-  int e = 0;
-  if (wmax > 0.f && wmax < INFINITY) {
-    int ex;
-    frexpf(wmax, &ex);
-    e = 14 - ex;
-  }
-  e = max(-100, min(100, e));
+  const int e = f16_scale_exp(wmax);
   h[1] = wmax;
-  h[0] = ldexpf(1.f, -e);                          // 1 / s_w: what the conv kernel reads
+  h[0] = ldexpf(1.f, -e);                          // 1 / s_w (subnormal for e = 127)
+  reinterpret_cast<int*>(out)[2] = e;              // e_w: what the conv kernel reads
 }
 
 static int tc_tile_n(int cout) { return cout >= 96 ? 128 : (cout >= 48 ? 64 : 32); }

@@ -81,7 +81,7 @@ __global__ void __launch_bounds__(256) nchw_to_rows_kernel(const float* __restri
 #pragma unroll
     for (int j = 0; j < kLP / 32; ++j) {
       tile[warp + 8 * i][lane + 32 * j] = v[i][j];
-      if (!masked || ((marked[j] >> lane) & 1u)) vmax = fmaxf(vmax, fabsf(v[i][j]));
+      if (!masked || ((marked[j] >> lane) & 1u)) vmax = fmaxf(vmax, finite_abs(v[i][j]));
     }
   }
   if (amax) {                                    // max |x| (of the marked pixels), for the consumers' fp16 operand scaling
@@ -215,7 +215,7 @@ __global__ void __launch_bounds__(256) gather_rows_list_kernel(const float* __re
         const long long b = base[lane + 32 * j];
         const float v = (c < C && b >= 0) ? __ldg(src + b + coff) : 0.f;
         tile[r][lane + 32 * j] = v;
-        vmax = fmaxf(vmax, fabsf(v));
+        vmax = fmaxf(vmax, finite_abs(v));
       }
     }
     __syncthreads();

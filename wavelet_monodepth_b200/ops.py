@@ -351,9 +351,9 @@ def rows_view(x):
 
 @_on_device
 def amax_rows(x, out, mask=None):
-    """out (1-element device tensor, pre-zeroed or holding a lower bound) = max(out, max |x|): for sources no libwmd kernel
-    produced (channels_last maps used in place).  mask: optional uint8 tensor of one byte per row of x (contiguous);
-    then only the marked rows count - the rows the consumer reads."""
+    """out (1-element device tensor, pre-zeroed or holding a lower bound) = max(out, max |x| over the finite x; NaN and
+    +-Inf are skipped): for sources no libwmd kernel produced (channels_last maps used in place).  mask: optional uint8
+    tensor of one byte per row of x (contiguous); then only the marked rows count - the rows the consumer reads."""
     lib = _lib.load()
     if mask is None:
         with _prof('amax', lambda: dict(count=x.numel())):
