@@ -141,7 +141,9 @@ int wmd_pack_conv_weight_f32(const float* w, float* packed, int Cout, int Cin, i
  * z = Wz . lrelu(W1 . x + b1): the 1x1 stages of a level's + / - coefficient heads (Conv1x1 + LeakyReLU(0.1),
  * depth_decoder.py:111-120) chained with the per-row tap products of their 3x3 stages (the 9 x 6 values
  * wmd_head_gather_f32 sums per pixel).  x rows (M, c), W1 (n1, c), Wz (nz <= 56, n1); z rows (M, ldz >= 56), columns
- * nz..55 are written as zeros.  The intermediate (M, n1) never reaches memory.  Supported (c, n1): (32, 64), (64, 128);
+ * nz..55 are written as zeros.  The intermediate (M, n1) never reaches memory.  Both GEMMs run tf32x3: |z - exact| <=
+ * 4e-6 S + F, F the tf32x3 floor of the first stage carried through |Wz| plus that of the second (tests/head_ref.py);
+ * a pre-activation that is non-finite in the contract may be NaN, so a non-finite x makes its own row non-finite.  Supported (c, n1): (32, 64), (64, 128);
  * other shapes return WMD_ERR_UNSUPPORTED (the caller then runs the two stages as wmd_conv_rows launches). */
 int wmd_head_mlp_supported(int c, int n1);
 size_t wmd_head_mlp_weight_floats(int c, int n1);
@@ -206,14 +208,21 @@ typedef struct wmd_conv_desc {
 int wmd_conv_rows_f32(const wmd_conv_desc* d, wmd_stream_t stream);
 
 /* Tensor-core engine for the same contract: wgmma tf32 with a 3xTF32 split (hi*hi + lo*hi + hi*lo,
- * fp32 accumulation), so results stay fp32-faithful: |y - exact| <= 1.7e-5 S, S = |bias| + sum |x w| of the element's
+ * fp32 accumulation), so results stay fp32-faithful: |y - exact| <= 1.7e-5 S + F, S = |bias| + sum |x w| of the element's
  * terms (measured worst, same-sign operands, H100; f16x3: 8.6e-6 S for operands within 2^-11 of their maxima, the SIMT
- * kernel: 6.5e-6 S at K = 18432).  f16x3 in general: |y - exact| <= 2.5e-5 S + F, with the absolute floor
+ * kernel: 6.5e-6 S + F at K = 18432).  F is an absolute floor for the bottom of the fp32 range (tests/conv_ref.py
+ * derives it): tf32x3 F = 2^-126 (sum |w| over the nonzero x + sum |x| over the nonzero w + 6 K') + 16 x 2^-149, which
+ * holds even where subnormal pieces, products and sums are flushed; the fp32 FMA engine F = 2^-149 (K' + 8).  Both are
+ * below 2^-22 S wherever operands and products are normal.  f16x3 in general: |y - exact| <= 2.5e-5 S + F, with the absolute floor
  *   F = 2^-25 (sum |w| over the nonzero x / s_x + sum |x| over the nonzero w / s_w) + 2^-50 K' / (s_x s_w) + 2^-149
  * (s_x, s_w the two scales, K' the number of terms with both factors nonzero): each operand's split is off by at most
  * 2^-22 of itself or 2^-25 / s, whichever is larger (tests/conv_ref.py derives it).  Non-finite inputs: an output is
- * non-finite exactly where the fp64 contract's is (the rows whose taps read a NaN or +-Inf), though the tensor-core
- * engines may give NaN where the contract gives +-Inf (the split's remainder is Inf - Inf); other rows are unaffected.
+ * non-finite exactly where the fp64 contract's is (the rows whose taps read a NaN or +-Inf), except on the tensor-core
+ * engines: their split's remainder of an Inf is Inf - Inf, so the activation is applied to a pre-activation that may be
+ * NaN wherever the contract's pre-activation is non-finite, and an output may be NaN where the contract's is +-Inf or
+ * where ELU(-Inf) = -1 or sigmoid(+-Inf) is finite.  The SIMT engine follows the contract exactly.  Other rows are
+ * unaffected.  The weight packs split to nearest, except that a finite |w| >= (2 - 2^-11) 2^127, which would round up
+ * to Inf, takes the truncated high piece.
  * d->w must point to weights packed by wmd_pack_conv_weight_tc_f32 for the same (cout, c0, c1, taps); d->ldw is ignored.
  *   wmd_conv_tc_tile_n(cout)                 N-tile of the kernel for this cout (128 / 64 / 32; the CTA tile is 128 rows x N)
  *   wmd_conv_tc_weight_floats(...)           size of the packed weight buffer, in floats
@@ -367,7 +376,9 @@ int wmd_head_idwt_f32(const wmd_head_idwt_desc* d, void* ws, size_t ws_bytes, wm
  * x: rows (N*H*W, ld) at half resolution H x W (upconv(0,0)'s output as wmd_conv_rows_f32 writes it: ld >= 16,
  * ld % 4 == 0, 16-byte aligned); disp: (N, cout, 2H, 2W) NCHW, cout = 1..4; nothing else is written.  u never reaches
  * memory.  The 16 -> 16 stage runs on tensor cores with the 3xTF32 split (fp32-faithful, fp32 accumulation), the
- * dispconv in fp32 FMAs.  N = 0 launches nothing.
+ * dispconv in fp32 FMAs: |disp - exact| <= 3e-8 S + F plus the ELU / sigmoid's own absolute error, F the tf32x3 floor
+ * carried through |W2| plus the FMA floor (tests/disp_tail_ref.py).  A non-finite x gives NaN over its up2, 3x3, 3x3
+ * footprint (sigmoid of a NaN pre-activation, where the contract's may be sigmoid(-Inf) = 0).  N = 0 launches nothing.
  * The weights are packed once by wmd_pack_disp_tail16_f32: w1 (16,16,3,3), b1 (16) or NULL, w2 (cout,16,3,3), b2 (cout)
  * or NULL -> packed, WMD_DISP_TAIL16_PACKED_FLOATS floats, 16-byte aligned. */
 enum { WMD_DISP_TAIL16_PACKED_FLOATS = 5332 };
@@ -393,7 +404,8 @@ int wmd_act_bwd_f32(const float* y, int ldy, const float* dy, int lddy, int rows
  * and act are not read.  Tensor cores (mma.sync tf32) with the operands split into tf32 hi + lo (3 MMAs per product)
  * and each 32-pixel chunk's MMA sum added into fp32 sums with round-to-nearest adds.  taps = 1 needs shift0 = 0.  Layers with few output tiles split the
  * pixel reduction across CTAs; the last CTA of a tile to arrive sums the partial slabs in slab order, so results are
- * deterministic (no float atomics).  ws: wmd_conv_wgrad_ws_bytes(d) bytes (0: none needed) whose first 4 KiB (per-tile
+ * deterministic (no float atomics).  |dw - exact| <= 2.5e-6 S + F with the tf32x3 floor of A against dz plus 2^-149 per
+ * chunk add (tests/conv_grad_ref.py, wgrad_floor).  ws: wmd_conv_wgrad_ws_bytes(d) bytes (0: none needed) whose first 4 KiB (per-tile
  * arrival counters) are zero before the first use; the kernel leaves them zero. */
 size_t wmd_conv_wgrad_ws_bytes(const wmd_conv_desc* d);
 int wmd_conv_wgrad_f32(const wmd_conv_desc* d, const float* dz, int lddz, float* dw, void* ws, size_t ws_bytes,

@@ -41,6 +41,30 @@ def conv_grads(x0, c0, x1, c1, weight, dz, n, h, w, taps=9, pad=conv_ref.PAD_REF
     return out
 
 
+def wgrad_floor(x0, c0, x1, c1, weight, dz, n, h, w, taps=9, pad=conv_ref.PAD_REFLECT, shift0=0, block_elems=1 << 24):
+    """F of the tf32x3 weight gradient's bound BAR S + F, per element of dW (weight layout): A and dz are both split to
+    nearest into tf32 hi + lo (conv_bwd.cu), so conv_ref.tf32_floor applies with A in the role of x and dz in that of
+    w - 2^-126 (sum |dz| over A != 0 + sum |A| over dz != 0 + 6 K') - plus 2^-149 for each 32-pixel chunk's
+    round-to-nearest add and each partial slab (at most rows / 32 + 8 of them)."""
+    block_rows = max(1, block_elems // max(taps * (c0 + c1), 1))
+    nz = lambda t: (t != 0).to(_f64) if t is not None else None      # noqa: E731
+    ab = lambda t: t.abs() if t is not None else None                # noqa: E731
+    a = _adjoint(nz(x0), c0, nz(x1), c1, weight, dz.abs(), n, h, w, taps, pad, shift0, block_rows)[2]
+    b = _adjoint(ab(x0), c0, ab(x1), c1, weight, nz(dz), n, h, w, taps, pad, shift0, block_rows)[2]
+    k = _adjoint(nz(x0), c0, nz(x1), c1, weight, nz(dz), n, h, w, taps, pad, shift0, block_rows)[2]
+    return conv_ref.TF32_FLOOR * (a + b + 6 * k) + conv_ref.FMA_FLOOR * (n * h * w / 32 + 24)
+
+
+def act_bwd_floor(dy, rows_summed=None):
+    """F of act_backward's dz = dy act'(y), per element: |dz - exact| <= 4 x 2^-24 |exact| + F, F = 2^-149 (1 + |dy|) for
+    the two roundings (act'(y) = y (1 - y) and the product) that may land among the subnormals.  rows_summed: also the
+    floor of db = sum over rows of dz, the rows' F plus 2^-149 per add of the fixed-order sum."""
+    f = conv_ref.FMA_FLOOR * (1 + dy.to(_f64).abs())
+    if rows_summed is None:
+        return f
+    return f, f.sum(0) + conv_ref.FMA_FLOOR * (rows_summed + 1100)
+
+
 def dgrad_floor(c0, c1, weight, dz, n, h, w, amax_dz, taps=9, pad=conv_ref.PAD_REFLECT, shift0=0, block_elems=1 << 24):
     """The absolute floor F of the f16x3 data gradient (conv_ref, the f16x3 bound), per element of dx0 and dx1 (rows).
 

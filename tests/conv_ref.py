@@ -41,6 +41,47 @@ ACT_ALLOW = 5e-7                  # absolute error of the kernels' expf-based EL
 F16_FLOOR = 2.0 ** -25
 
 
+# tf32x3 and fp32 FMA bounds: |y - y64| <= BAR[engine] S + F per element, F an absolute floor for the bottom of the fp32
+# range (the relative bars alone hold only while every piece, product and partial sum is a normal number).
+#
+# tf32x3 (conv_tc.cu load_frag / pack_weight_tc_kernel; head_mlp.cu, disp_tail.cu and conv_bwd.cu split the same way):
+# each operand v is split into hi + lo (activations: hi truncated, lo the exact remainder, which the MMA reads truncated
+# to tf32; weights: both pieces rounded to tf32), the MMA forms hi_x hi_w + hi_x lo_w + lo_x hi_w with fp32
+# accumulation.  The worst case assumed is a tensor core that flushes every subnormal input piece, every subnormal
+# product and every subnormal accumulator to zero (what H100 does is measured by tests/test_gpu_conv_range.py; keeping
+# them is only more accurate).  Then:
+#   * a piece is lost only if it is below 2^-126, so the represented operand is off by |dv| < 2^-126 beyond the
+#     relative part (tf32 rounding of the pieces and the dropped lo lo: the relative bar);
+#   * x' w' - x w = dx w + x dw + dx dw: 2^-126 (|w| for x != 0 + |x| for w != 0), and |dx dw| < 2^-252;
+#   * each of the three products of a term is lost only if below 2^-126: 3 x 2^-126 per term with x != 0 and w != 0;
+#   * an accumulator is flushed only if below 2^-126, once per MMA instruction that adds a nonzero product: at most
+#     3 x 2^-126 per such term (the round-to-nearest epoch and split-K adds on the CUDA cores keep subnormals: 2^-150
+#     each, far below);
+#   * the bias add, the split-K / stream-K partial sums and the epilogue: a few fp32 roundings of 2^-150 each.
+#   F = 2^-126 (sum_{x != 0} |w| + sum_{w != 0} |x| + 6 K') + 16 x 2^-149,  K' = terms with x != 0 and w != 0.
+# Where every nonzero operand is >= 2^-102 and every nonzero product >= 2^-99, F < 2^-22 S + 2^-145: the normal range
+# keeps its relative bar.  The tightest case is a subnormal operand against a large one: x in [2^-127, 2^-126) flushed
+# against w = 2^20 is off by |x w| ~ F / 2.
+# fp32 FMA (conv.cu, head.cu, the second stage of disp_tail.cu): acc = fma(x, w, acc) with denormals kept (no -ftz); a
+# rounding is off by at most 2^-24 of its result or 2^-150, whichever is larger.  The relative parts are the bar's; the
+# absolute parts add up to 2^-150 per rounding: one per term with x w != 0 (a zero product leaves acc exactly), plus the
+# bias, the reduction tree and the epilogue.  Each is counted as 2^-149 to cover their (1 + 2^-24)^K growth:
+#   F = 2^-149 (K' + extra).
+TF32_FLOOR = 2.0 ** -126
+FMA_FLOOR = 2.0 ** -149
+
+
+def tf32_floor(a, wk):
+    """F of the tf32x3 bound for gathered rows a (rows, K) and weights wk (K, cout), float64 (derivation above)."""
+    nza, nzw = (a != 0).to(_f64), (wk != 0).to(_f64)
+    return TF32_FLOOR * (nza @ wk.abs() + a.abs() @ nzw + 6 * (nza @ nzw)) + 16 * 2.0 ** -149
+
+
+def fma_floor(a, wk, extra=8):
+    """F of the fp32 FMA bound: 2^-149 per rounding, K' terms with a w != 0 plus `extra` (bias, reduction, epilogue)."""
+    return FMA_FLOOR * (((a != 0).to(_f64) @ (wk != 0).to(_f64)) + extra)
+
+
 def f16_scale(m):
     """The power-of-two operand scale of an fp16-pair launch whose maximum is m (f16_scale_exp in csrc/conv_tc.cu):
     m s in [2^13, 2^14), the exponent clamped to [-126, 127]; m = 0 or non-finite: 1."""
@@ -131,14 +172,17 @@ def gather_rows(m, x0, c0, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0
 
 def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NONE, act_param=0.0, map0=None, shift0=0,
              x1=None, c1=0, map1=None, gate=None, pixels=None, count=None, max_rows=None, rows0=None, block_elems=1 << 24,
-             read_max=False, f16_amax=None):
+             read_max=False, f16_amax=None, floor=None):
     """(y64, S) for rows [0, min(count, max_rows)): the arguments of ops.conv_rows, with a plain (cout, c0 + c1, k, k)
     weight and an optional bias (cout,).  count: int or 1-element tensor (with pixels); rows0 (taps == 1, map0 None
     only): rows x0 holds, rows past it read zeros (default: x0.shape[0]).
     read_max: also return the largest |value| the launch reads from source 0 and from source 1 (the maxima its fp16-pair
     operand scales must cover): (y64, S, max0, max1).  Non-finite values count as 0 there, as in the kernels.
     f16_amax: the activation maximum an f16x3 launch scales by (the larger of its amax0 / amax1 scalars): also return F,
-    the absolute floor of the f16x3 bound (f16_floor; the weight scale follows from the finite max |weight|), last."""
+    the absolute floor of the f16x3 bound (f16_floor; the weight scale follows from the finite max |weight|), last.
+    floor: 'tf32x3' or 'simt': also return that engine's F (tf32_floor / fma_floor), last."""
+    if f16_amax is not None:
+        floor = "f16x3"
     dev = x0.device
     cout = weight.shape[0]
     rows = int(count) if pixels is not None else n * h * w
@@ -152,9 +196,10 @@ def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NON
     b = bias.to(dev, _f64) if bias is not None else torch.zeros(cout, dtype=_f64, device=dev)
     y64 = torch.empty(rows, cout, dtype=_f64, device=dev)
     s = torch.empty(rows, cout, dtype=_f64, device=dev)
-    if f16_amax is not None:
+    if floor == "f16x3":
         s_x, s_w = f16_scale(f16_amax), f16_scale(finite_max(weight))
-        floor = torch.empty(rows, cout, dtype=_f64, device=dev)
+    if floor is not None:
+        fl = torch.empty(rows, cout, dtype=_f64, device=dev)
     step = max(1, block_elems // max(k, 1))
     max0 = max1 = 0.0
     for r in range(0, rows, step):
@@ -166,13 +211,17 @@ def conv_ref(x0, c0, weight, bias, n, h, w, taps=9, pad=PAD_REFLECT, act=ACT_NON
         a = a.reshape(len(m), k)
         y64[r:r + len(m)] = a @ wk + b
         s[r:r + len(m)] = a.abs() @ wa + b.abs()
-        if f16_amax is not None:
-            floor[r:r + len(m)] = f16_floor(a, wk, s_x, s_w)
+        if floor == "f16x3":
+            fl[r:r + len(m)] = f16_floor(a, wk, s_x, s_w)
+        elif floor == "tf32x3":
+            fl[r:r + len(m)] = tf32_floor(a, wk)
+        elif floor == "simt":
+            fl[r:r + len(m)] = fma_floor(a, wk)
     out = (activate(y64, act, act_param), s)
     if read_max:
         out += (max0, max1)
-    if f16_amax is not None:
-        out += (floor,)
+    if floor is not None:
+        out += (fl,)
     return out
 
 

@@ -112,11 +112,14 @@ def head_idwt_ref(z, col0, map, mask, bias, scale, pad, ll, disp_scale, clamp01,
     return dict(yh=yh, s_yh=s_yh, out=out, s_out=s_out, disp=disp, s_disp=s_out * abs(float(disp_scale)))
 
 
-def head_mlp_ref(x, c, w1, b1, wz, slope, count, max_rows):
+def head_mlp_ref(x, c, w1, b1, wz, slope, count, max_rows, floor=False):
     """x rows (R, ldx >= c), w1 (n1, c[, 1, 1]), b1 (n1,) or None, wz (nz, n1[, 1, 1]) -> (z (rows, nz), S).
 
     rows = min(count, max_rows) (count None: max_rows).  S = |Wz| S1 + |Wz| |t| with S1 = |b1| + |W1| |x| the scale of
-    t's pre-activation sums and t = lrelu(W1 x + b1)."""
+    t's pre-activation sums and t = lrelu(W1 x + b1).
+    floor: also return F of the bound BAR S + F, both stages being tf32x3 (conv_ref.tf32_floor): F1 of the first stage
+    plus 2 x 2^-149 for its bias add and LeakyReLU product, carried through |Wz| (slope <= 1), plus the second stage's
+    own floor, with every t counted as nonzero (the kernel's t may be nonzero where the exact one is 0)."""
     dev = x.device
     rows = int(max_rows) if count is None else min(int(count), int(max_rows))
     w1 = w1.to(dev, _f64).reshape(w1.shape[0], c)
@@ -126,6 +129,9 @@ def head_mlp_ref(x, c, w1, b1, wz, slope, count, max_rows):
     pre = xs @ w1.T + b
     s1 = xs.abs() @ w1.abs().T + b.abs()
     t = cr.activate(pre, cr.ACT_LRELU, slope)
+    if floor:
+        f1 = cr.tf32_floor(xs, w1.T) + 2 * 2.0 ** -149
+        return t @ wz.T, (s1 + t.abs()) @ wz.abs().T, f1 @ wz.abs().T + cr.tf32_floor(t.abs() + f1, wz.T)
     return t @ wz.T, (s1 + t.abs()) @ wz.abs().T
 
 

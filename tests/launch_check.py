@@ -312,9 +312,9 @@ class Harness:
                           act_param=a["act_param"], map0=a["map0"], shift0=a["shift0"], x1=x1, c1=c1,
                           map1=a["map1"], gate=a["gate"], pixels=a["pixels"], count=a["count"],
                           max_rows=max_rows, rows0=rows0 if (taps == 1 and a["map0"] is None) else None,
-                          read_max=True, f16_amax=amax16)
+                          read_max=True, f16_amax=amax16, floor=engine)
         y64, s, m0, m1 = ref[:4]
-        floor = ref[4] if use16 else 0.0        # f16x3: BAR S + F (conv_ref, the f16x3 bound)
+        floor = ref[4]                          # BAR S + F with the engine's floor (conv_ref, the f16x3 / tf32x3 / FMA bounds)
         if use16:
             _require(_scalar(a["amax0"]) >= m0, "conv_rows: amax0 %.9g below the largest |x0| read, %.9g"
                      % (_scalar(a["amax0"]), m0))
@@ -340,10 +340,10 @@ class Harness:
         if count is not None:
             _require(count <= max_rows, "head_mlp: count %d > max_rows %d" % (count, max_rows))
         rows = max_rows if count is None else min(count, max_rows)
-        want, s = hr.head_mlp_ref(x, a["c"], w1, b1, wz, a["slope"], count, max_rows)
+        want, s, floor = hr.head_mlp_ref(x, a["c"], w1, b1, wz, a["slope"], count, max_rows, floor=True)
         nz = a["nz"]
         _require(bool((z[:rows, nz:56] == 0).all()), "head_mlp: columns nz..55 are not zero")
-        err = _err(z[:rows, :nz], want, s)
+        err = _err(z[:rows, :nz], want, s, floor)
         bar = hr.BAR["head_mlp"]
         _record("head_mlp", "tf32x3", "-", err, bar, rows)
         _require(err <= bar, "%s: head_mlp err/S %.3g > %.3g" % (self.current, err, bar))
@@ -476,8 +476,8 @@ class Harness:
         if n == 0:
             return
         w1, b1, w2, b2 = self._weights(a["packed"])
-        want, s = disp_tail_ref.disp_tail_ref(a["x"], w1, b1, w2, b2, n, a["h"], a["w"])
-        err = _err(out, want, s)
+        want, s, floor = disp_tail_ref.disp_tail_ref(a["x"], w1, b1, w2, b2, n, a["h"], a["w"], floor=True)
+        err = _err(out, want, s, floor)
         _record("disp_tail16", "tf32x3", "-", err, disp_tail_ref.BAR, n * a["h"] * a["w"] * 4)
         _require(err <= disp_tail_ref.BAR, "%s: disp_tail16 err/S %.3g > %.3g" % (self.current, err, disp_tail_ref.BAR))
 
@@ -636,7 +636,8 @@ class Harness:
         cout = a["cout"]
         want = self._dz64(a["y"], a["dy"], cout, a["act"], a["act_param"])
         rows = want.shape[0]
-        err = _err(dz[:, :cout], want, want.abs().clamp(min=1e-38))
+        dz_floor, db_floor = conv_grad_ref.act_bwd_floor(a["dy"][:, :cout], rows_summed=rows)
+        err = _err(dz[:, :cout], want, want.abs().clamp(min=1e-38), dz_floor)
         bar = ACT_BWD_ULP * EPS
         _record("act_backward", "fp32", "dz", err, bar, rows)
         _require(err <= bar, "%s: act_backward dz %.3g > %.3g relative" % (self.current, err, bar))
@@ -644,7 +645,7 @@ class Harness:
             self._check_amax_out("act_backward", old_amax, a["amax"], dz[:, :cout])
         if db is not None:
             gb, sb = want.sum(0), want.abs().sum(0)
-            err = _err(db, gb, sb)
+            err = _err(db, gb, sb, db_floor)
             bar = conv_grad_ref.BARS["db"]
             _record("act_backward", "fp32", "db", err, bar, rows)
             _require(err <= bar, "%s: act_backward db err/S %.3g > %.3g" % (self.current, err, bar))
@@ -668,7 +669,9 @@ class Harness:
         with torch.enable_grad():                               # the autograd backward calling this runs without
             ref = conv_grad_ref.conv_grads(x0r, c0, x1r, c1, wzero, a["dz"][:, :cout], n, h, w, taps=taps, pad=a["pad"],
                                            shift0=a["shift0"])
-        err = _err(dw, *ref["w"])
+            floor = conv_grad_ref.wgrad_floor(x0r, c0, x1r, c1, wzero, a["dz"][:, :cout], n, h, w, taps=taps,
+                                              pad=a["pad"], shift0=a["shift0"])
+        err = _err(dw, *ref["w"], floor)
         bar = conv_grad_ref.BARS["dW"]
         _record("conv_wgrad", "tf32x3", "cout<=8" if cout <= 8 else "-", err, bar, n * h * w)
         _require(err <= bar, "%s: conv_wgrad (n %d, %dx%d, c0 %d, c1 %d, cout %d) err/S %.3g > %.3g"

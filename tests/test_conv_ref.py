@@ -222,3 +222,147 @@ def test_f16_scale_matches_the_kernel_rule():
         assert e == int(e) and -126 <= e <= 127
         assert m * s < 2.0 ** 14 and (m * s >= 2.0 ** 13 or e == 127)
     assert cr.f16_scale(0.0) == cr.f16_scale(float("inf")) == cr.f16_scale(float("nan")) == 1.0
+
+
+# ------------------------------------------------------------------------------------------ the tf32x3 and FMA floors
+TINY = 2.0 ** -126                 # the smallest normal fp32
+
+
+def _tf32(v, rna):
+    """float32 array -> tf32 values (13 low mantissa bits cleared): truncated, or rounded to nearest with ties away
+    (cvt.rna) except where that overflows a finite v, which is truncated (tf32_rna_finite in csrc/common.cuh)."""
+    bits = v.view(np.uint32)
+    t = (bits & np.uint32(0xFFFFE000)).view(np.float32)
+    if not rna:
+        return t
+    r = ((bits + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
+    return np.where(np.isinf(r) & np.isfinite(v), t, r)
+
+
+def _flush(v, on):
+    return np.where(np.abs(v) < TINY, 0.0, v) if on else v
+
+
+def _emulate_tf32x3(x, w, flush):
+    """x (R, K) @ w (K, C) as the tf32x3 engine forms it: activations split by truncation (the MMA reads the exact
+    remainder truncated to tf32), weights split to nearest (both pieces), products lo_x hi_w, hi_x lo_w, hi_x hi_w exact,
+    one accumulator rounding to fp32 per MMA of 8 k (in the kernel's order: small terms first).  flush: every subnormal
+    piece, product and accumulator becomes 0 (the worst case the floor assumes); else subnormals are kept."""
+    x, w = x.numpy(), w.numpy()
+    xh = _tf32(x, False)
+    xl = _tf32((x - xh).astype(np.float32), False)
+    wh = _tf32(w, True)
+    wl = _tf32((w - wh).astype(np.float32), True)
+    xh, xl, wh, wl = (_flush(v.astype(np.float64), flush) for v in (xh, xl, wh, wl))
+    acc = np.zeros((x.shape[0], w.shape[1]), dtype=np.float32)
+    for k0 in range(0, x.shape[1], 8):
+        ks = slice(k0, k0 + 8)
+        for a, b in ((xl, wh), (xh, wl), (xh, wh)):
+            p = _flush(a[:, ks, None] * b[None, ks, :], flush).sum(1)
+            acc = _flush((acc.astype(np.float64) + p).astype(np.float32), flush).astype(np.float32)
+    return torch.from_numpy(acc.astype(np.float64))
+
+
+def _emulate_fma(x, w):
+    """x (R, K) @ w (K, C) as an fp32 FMA chain: acc = fp32(acc + x w) in k order (x w is exact in fp64), subnormals kept."""
+    x, w = x.numpy().astype(np.float64), w.numpy().astype(np.float64)
+    acc = np.zeros((x.shape[0], w.shape[1]), dtype=np.float32)
+    for k in range(x.shape[1]):
+        acc = (acc.astype(np.float64) + x[:, k, None] * w[None, k, :]).astype(np.float32)
+    return torch.from_numpy(acc.astype(np.float64))
+
+
+def _engine_err(engine, x, w, flush=True):
+    """(|emulated - exact|, S, F) per element of x @ w for 'tf32x3' or 'simt'."""
+    got = _emulate_tf32x3(x, w, flush) if engine == "tf32x3" else _emulate_fma(x, w)
+    x64, w64 = x.double(), w.double()
+    floor = cr.tf32_floor(x64, w64) if engine == "tf32x3" else cr.fma_floor(x64, w64)
+    return (got - x64 @ w64).abs(), x64.abs() @ w64.abs(), floor
+
+
+def _spread(top, side, seed):
+    """x (46, 64) and w (64, 46), mixed signs; the rows of x (side 'x'), the columns of w ('w') or both at 2^-m of
+    2^top, m = 0 .. 45; the other operand at most 2^-7, so that no sum overflows."""
+    g = torch.Generator().manual_seed(seed)
+    ms = torch.arange(46, dtype=torch.float64)
+    x = torch.rand(46, 64, generator=g, dtype=torch.float64) * 2 - 1
+    w = torch.rand(64, 46, generator=g, dtype=torch.float64) * 2 - 1
+    if side in ("x", "both"):
+        x = x * torch.exp2(top - ms)[:, None]
+    else:
+        x = x * 2.0 ** -7
+    if side in ("w", "both"):
+        w = w * torch.exp2(top - ms)[None, :]
+    else:
+        w = w * 2.0 ** -7
+    return x.float(), w.float()
+
+
+FLOOR_CASES = ([(side, top) for side in ("x", "w") for top in (-149, -140, -126, -100, -60, 0, 60, 116, 127)]
+               + [("both", top) for top in (-75, -70, -63, -40, 0, 60)])
+
+
+@pytest.mark.parametrize("side,top", FLOOR_CASES)
+@pytest.mark.parametrize("engine,flush", [("tf32x3", True), ("tf32x3", False), ("simt", False)],
+                         ids=["tf32x3-flush", "tf32x3-keep", "simt"])
+def test_floor_bounds_the_emulated_engine(engine, flush, side, top):
+    """From 2^-149 to 2^127 the emulated engine never leaves BAR S + F, with subnormals flushed or kept; where pieces,
+    products or sums are subnormal the plain relative bar fails, so F is what lets it."""
+    x, w = _spread(top, side, seed=top + 300 + len(side))
+    err, s, f = _engine_err(engine, x, w, flush)
+    bound = cr.BAR[engine] * s + f
+    assert bool((err <= bound).all()), float((err / bound).max())
+    if side == "both" and top <= -63 or side != "both" and top - 7 <= -140:
+        assert float((err / s)[s > 0].max()) > cr.BAR[engine]
+
+
+def test_floor_is_negligible_in_the_normal_range():
+    """Operands >= 2^-102 and products >= 2^-99: F < 2^-22 S + 2^-145, so the relative bar is unchanged there."""
+    x, w = _spread(-40, "both", seed=5)
+    x = torch.where(x.abs() < 2.0 ** -50, torch.full_like(x, 2.0 ** -50), x)
+    w = torch.where(w.abs() < 2.0 ** -49, torch.full_like(w, 2.0 ** -49), w)
+    x64, w64 = x.double(), w.double()
+    s = x64.abs() @ w64.abs()
+    for f in (cr.tf32_floor(x64, w64), cr.fma_floor(x64, w64)):
+        assert bool((f < 2.0 ** -22 * s + 2.0 ** -145).all())
+
+
+def test_tf32_floor_is_tight():
+    """x in [2^-127, 2^-126) against w = +-2^20, K = 1: a tensor core that flushes subnormal pieces loses x whole, an
+    error of |x w|, which reaches F within a factor of 2 (4096 samples)."""
+    g = torch.Generator().manual_seed(9)
+    x = ((torch.rand(4096, 1, generator=g, dtype=torch.float64) * 0.5 + 0.5) * TINY).float()
+    w = torch.tensor([[2.0 ** 20, -2.0 ** 20]])
+    err, s, f = _engine_err("tf32x3", x, w, flush=True)
+    ratio = err / (cr.BAR["tf32x3"] * s + f)
+    assert 0.5 <= float(ratio.max()) <= 1.0, float(ratio.max())
+
+
+def test_fma_floor_is_tight():
+    """64 products of 2^-150 (1 + 2^-10) each, all in the subnormal range: every rounding of the chain goes up by
+    nearly 2^-150, and the chain's error reaches F (2^-149 per rounding, plus 8 for the epilogue) within a factor of 2.5."""
+    x = torch.full((1, 64), 2.0 ** -75 * (1 + 2.0 ** -10))
+    w = torch.full((64, 1), 2.0 ** -75)
+    err, s, f = _engine_err("simt", x, w)
+    ratio = float((err / (cr.BAR["simt"] * s + f)).max())
+    assert 0.4 <= ratio <= 1.0, ratio
+
+
+def test_round_to_nearest_split_keeps_the_top_binade_finite():
+    """cvt.rna rounds a finite |w| >= (2 - 2^-11) 2^127 up to Inf; the split truncates there instead, so hi + lo is
+    finite and FLT_MAX weights against tiny activations stay within the bound.  Below the threshold the split is the
+    plain round to nearest."""
+    fmax = np.float32(np.finfo(np.float32).max)
+    edge = np.float32(np.ldexp(2 - 2.0 ** -11, 127))
+    below = np.nextafter(edge, np.float32(0))
+    v = np.array([fmax, -fmax, edge, below, np.float32(1.5)], dtype=np.float32)
+    hi = _tf32(v, True)
+    assert np.isfinite(hi).all() and np.isfinite(v - hi).all()
+    assert hi[2] == (v[2].view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)      # the tie: truncated
+    assert hi[3] == np.float32(np.ldexp(2 - 2.0 ** -10, 127))                          # below it: to nearest
+    x = torch.full((3, 16), 2.0 ** -100)
+    x[1] *= -1
+    w = torch.full((16, 2), float(fmax))
+    w[:, 1] = -float(fmax)
+    err, s, f = _engine_err("tf32x3", x, w, flush=True)
+    assert bool((err <= cr.BAR["tf32x3"] * s + f).all())

@@ -4,13 +4,17 @@ fp64 contract (tests/conv_ref.py).
 The fp16-pair engine (f16x3) scales a launch's activations by one power of two taken from the larger source maximum
 (shared by every frame and both sources) and its weights by one taken from max |w|.  An operand far below its maximum
 has its low fp16 piece in the subnormal range, so f16x3 is held to BAR S + F (conv_ref, the f16x3 bound), not to the
-plain relative bar; tf32x3 and the fp32 FMA engine run the same inputs as a control at their plain bars.  The cases:
+plain relative bar.  tf32x3 and the fp32 FMA engine are held to BAR S + F with their own floors (conv_ref, the tf32x3
+and FMA bounds), which matter only where pieces, products or sums are fp32 subnormals.  The cases:
   * spread within one launch: frames, the skip source or output channels at 2^-m of the maximum, m = 0 .. 45, through
     the window kernel, the gather path and the 1x1 form, whole and balanced (stream-K); maxima up to 2^20 loose;
-  * exponent edges: source maxima from 2^-126 to 2^127 against weight maxima of 2^-40, 1 and 2^40;
+  * exponent edges, every engine: source maxima from 2^-126 to 2^127 against weight maxima from 2^-126 to FLT_MAX,
+    products and partial sums down in the subnormal range; tf32x3 also split-K (2 and 4 splits);
   * all-zero sources (maximum 0): y = act(bias) exactly;
-  * a NaN, +Inf or -Inf at one pixel of one frame: the non-finite outputs are exactly the fp64 reference's (the
-    pixel's 3x3 halo and its pad-mode mirrors) and every other output meets its bar;
+  * a NaN, +Inf or -Inf at one pixel of one frame, under no activation, ELU and sigmoid: the non-finite outputs are
+    exactly the fp64 reference's (the pixel's 3x3 halo and its pad-mode mirrors), except that the tensor-core engines may
+    give NaN wherever the reference's pre-activation is non-finite (ELU(-Inf) = -1 and sigmoid(+-Inf) are finite); every
+    other output meets its bar;
   * backward: f16x3 data gradients whose dz spans decades (saturated sigmoid, deep ELU rows), at conv_grad_ref.BARS S
     + F; a non-finite upstream gradient in one frame leaves the other frame's data gradients bit-identical;
   * a decoder batch with one corrupted frame: the other frames' outputs (dense) and input-feature gradients (native
@@ -67,12 +71,15 @@ def _pack(wt, c1, engine):
 
 
 class Geo:
-    """One launch's geometry: layout 'window' (dense 3x3), 'gather' (pixel list), '1x1'; '-balanced': stream-K."""
+    """One launch's geometry: layout 'window' (dense 3x3), 'gather' (pixel list), '1x1'; '-balanced': stream-K,
+    '-splitK' (tf32x3 only): the reduction cut into K equal ranges."""
 
     def __init__(self, layout, n, h, w, c0, c1, cout):
         self.layout, self.n, self.h, self.w, self.c0, self.c1, self.cout = layout, n, h, w, c0, c1, cout
         self.taps = 1 if layout.startswith("1x1") else 9
         self.splits = 0 if layout.endswith("-balanced") else None
+        if "-split" in layout:
+            self.splits = int(layout.rsplit("-split", 1)[1])
         total = n * h * w
         self.pixels = None
         if layout.startswith("gather"):
@@ -99,22 +106,33 @@ def run(engine, g, x0, x1, wt, b, amax0=None, amax1=None, pad=PAD_REFLECT, act=A
 
 
 def reference(engine, g, x0, x1, wt, b, maxima, pad=PAD_REFLECT, act=ACT_NONE):
-    """(y64, S, F): F = 0 except for f16x3, whose floor follows from the scalars the launch scaled by."""
+    """(y64, S, F, pre64): F the engine's floor (f16x3: from the scalars the launch scaled by), pre64 the fp64
+    pre-activation."""
     amax16 = None
     if engine == "f16x3":
         amax16 = max(float(maxima[0]), float(maxima[1]) if maxima[1] is not None else 0.0)
-    ref = cr.conv_ref(x0, g.c0, wt, b, g.n, g.h, g.w, taps=g.taps, pad=pad, act=act, x1=x1, c1=g.c1,
-                      pixels=g.pixels, count=g.rows, f16_amax=amax16)
-    return ref[0], ref[1], (ref[2] if engine == "f16x3" else torch.zeros_like(ref[1]))
+    ref = cr.conv_ref(x0, g.c0, wt, b, g.n, g.h, g.w, taps=g.taps, pad=pad, x1=x1, c1=g.c1, pixels=g.pixels,
+                      count=g.rows, f16_amax=amax16, floor=engine)
+    return cr.activate(ref[0], act), ref[1], ref[2], ref[0]
 
 
-def check(engine, y, y64, s, f, group, key, act=ACT_NONE):
-    """Non-finite exactly where y64 is; elsewhere |y - y64| <= BAR S + F (+ the activation's own error)."""
+def check(engine, y, y64, s, f, group, key, act=ACT_NONE, pre64=None):
+    """Non-finite exactly where y64 is; elsewhere |y - y64| <= BAR S + F (+ the activation's own error).  The tensor-core
+    engines may also give NaN where pre64 (the fp64 pre-activation) is non-finite: their split's remainder of an Inf is
+    Inf - Inf, so the activation sees NaN where ELU / sigmoid of +-Inf is finite (wmd.h)."""
     bad64 = ~torch.isfinite(y64)
     bad = ~torch.isfinite(y)
-    assert torch.equal(bad, bad64), "%s %s %s: %d non-finite outputs where the reference has %d (%d differ)" % (
-        engine, group, key, int(bad.sum()), int(bad64.sum()), int((bad ^ bad64).sum()))
-    ok = ~bad64
+    extra = bad & ~bad64
+    if engine != "simt" and pre64 is not None:
+        may = ~torch.isfinite(pre64)
+        assert bool(torch.isnan(y[extra]).all()) and bool(may[extra].all()), \
+            "%s %s %s: %d non-finite outputs where the pre-activation is finite" % (engine, group, key,
+                                                                                  int((extra & ~may).sum()))
+        extra = torch.zeros_like(extra)
+    assert not bool(extra.any()) and torch.equal(bad64 & bad, bad64), \
+        "%s %s %s: %d non-finite outputs where the reference has %d (%d differ)" % (
+            engine, group, key, int(bad.sum()), int(bad64.sum()), int((bad ^ bad64).sum()))
+    ok = ~bad
     allow = 0.0 if act in (ACT_NONE, ACT_LRELU) else cr.ACT_ALLOW
     d = ((y.double() - y64).abs() - allow).clamp(min=0)[ok]
     s, f = s[ok], f[ok]
@@ -161,7 +179,7 @@ def test_spread_within_one_launch(layout, kind, m):
     x0, x1, wt, b = _spread_operands(g, kind, m, seed=m * 31 + len(kind) + len(layout))
     for engine in ENGINES:
         y, maxima = run(engine, g, x0, x1, wt, b)
-        y64, s, f = reference(engine, g, x0, x1, wt, b, maxima)
+        y64, s, f, _ = reference(engine, g, x0, x1, wt, b, maxima)
         check(engine, y, y64, s, f, "spread/" + kind, m)
 
 
@@ -174,7 +192,7 @@ def test_loose_maxima(layout, loose, m):
     x0, x1, wt, b = _spread_operands(g, "frames", m, seed=m + 7 * loose)
     amax0 = _amax(x0) * 2.0 ** loose
     y, maxima = run("f16x3", g, x0, x1, wt, b, amax0=amax0)
-    y64, s, f = reference("f16x3", g, x0, x1, wt, b, maxima)
+    y64, s, f, _ = reference("f16x3", g, x0, x1, wt, b, maxima)
     check("f16x3", y, y64, s, f, "loose", "%d/%d" % (loose, m))
 
 
@@ -185,25 +203,52 @@ EDGES = [-126, -110, -87, 100, 115, 116, 120, 127]
 # K = 9 x 16 terms of 2^(xexp + wexp): past xexp + wexp = 118 the exact result itself leaves fp32
 EDGE_PAIRS = [(x, wx) for x in EDGES for wx in (-40, 0, 40) if x + wx <= 118]
 
+# weights at both ends too (128: up to FLT_MAX = (1 - 2^-24) 2^128); pairs such as (-87, -40) and (-70, -70) put every
+# product and partial sum among the fp32 subnormals
+WIDE_EDGES = [-126, -110, -87, -70, 100, 115, 120, 127]
+W_EDGES = [-126, -100, -70, -40, 0, 40, 100, 128]
+WIDE_PAIRS = [(x, wx) for x in WIDE_EDGES for wx in W_EDGES if x + wx <= 118 and (x, wx) not in EDGE_PAIRS]
+WIDE_RUNS = ([("f16x3", lay) for lay in ("window", "window-balanced", "gather", "gather-balanced")]
+             + [("tf32x3", lay) for lay in ("window", "window-balanced", "gather", "gather-balanced", "window-split2",
+                                            "gather-split4")]
+             + [("simt", lay) for lay in ("window", "gather")])
 
-@pytest.mark.parametrize("xexp,wexp", EDGE_PAIRS)
-@pytest.mark.parametrize("layout", ["window", "window-balanced", "gather", "gather-balanced"])
-def test_exponent_edges(layout, xexp, wexp):
-    """Source maxima near both ends of fp32 (2^-126: most values subnormal) against weight maxima far from 1: wherever
-    the fp64 result is a finite fp32 number, the output is finite and within BAR S + F.  The small pairs (2^-126 /
-    2^-110 against 2^-40) put 2^-(e + e_w) below the float range: the whole-tile epilogue and the stream-K fix-up
-    (balanced) then rescale the sums first."""
+
+def _edge_case(engine, layout, xexp, wexp):
+    """One launch with source maxima 2^xexp and weight maxima 2^wexp, the largest value of each at the top of its binade:
+    the fp64 result is a finite fp32 number, and the output must be finite and within BAR S + F."""
     g = Geo(layout, 2, 5, 12, 8, 8, 40)
     gen = torch.Generator(device=DEV).manual_seed(xexp * 3 + wexp)
     x0 = (_rand((g.n * g.h * g.w, g.c0), gen).double() * 2.0 ** xexp).float()
     x1 = (_rand((g.n * g.h * g.w, g.c1), gen).double() * 2.0 ** (xexp - 3)).float()
     x0[0, 0] = 2.0 ** xexp * (1 - 2.0 ** -24)       # the top of the binade: the largest scaled value the exponent allows
-    wt = (_rand((g.cout, g.c0 + g.c1, 3, 3), gen).double() * 2.0 ** wexp).float()
+    wt = (_rand((g.cout, g.c0 + g.c1, 3, 3), gen).double() * 2.0 ** (wexp - 1) * 2).float()
+    wt[0, 0, 1, 1] = 2.0 ** (wexp - 1) * 2 * (1 - 2.0 ** -24)
+    wt[1, 3, 0, 2] = -wt[0, 0, 1, 1]
     b = (_rand((g.cout,), gen).double() * 2.0 ** (xexp + wexp)).float()
-    y, maxima = run("f16x3", g, x0, x1, wt, b)
-    y64, s, f = reference("f16x3", g, x0, x1, wt, b, maxima)
+    y, maxima = run(engine, g, x0, x1, wt, b)
+    y64, s, f, _ = reference(engine, g, x0, x1, wt, b, maxima)
     assert bool((y64.abs() < FLT_MAX).all())
-    check("f16x3", y, y64, s, f, "edges", "%d/%d" % (xexp, wexp))
+    check(engine, y, y64, s, f, "edges", "%d/%d" % (xexp, wexp))
+
+
+@pytest.mark.parametrize("xexp,wexp", EDGE_PAIRS)
+@pytest.mark.parametrize("layout", ["window", "window-balanced", "gather", "gather-balanced"])
+def test_exponent_edges(layout, xexp, wexp):
+    """Source maxima near both ends of fp32 (2^-126: most values subnormal) against weight maxima far from 1, on all
+    three engines: wherever the fp64 result is a finite fp32 number, the output is finite and within BAR S + F.  The
+    small pairs (2^-126 / 2^-110 against 2^-40) put f16x3's 2^-(e + e_w) below the float range: the whole-tile epilogue
+    and the stream-K fix-up (balanced) then rescale the sums first."""
+    for engine in ENGINES:
+        _edge_case(engine, layout, xexp, wexp)
+
+
+@pytest.mark.parametrize("xexp,wexp", WIDE_PAIRS)
+@pytest.mark.parametrize("engine,layout", WIDE_RUNS, ids=["%s-%s" % r for r in WIDE_RUNS])
+def test_exponent_edges_of_the_weights(engine, layout, xexp, wexp):
+    """The same with weight maxima from 2^-126 to FLT_MAX and subnormal products, tf32x3 also split-K (2 and 4 splits).
+    FLT_MAX weights round to Inf under a plain round-to-nearest tf32 split; the weight pack truncates those instead."""
+    _edge_case(engine, layout, xexp, wexp)
 
 
 @pytest.mark.parametrize("act", [ACT_NONE, ACT_LRELU])
@@ -231,7 +276,8 @@ def test_all_zero_sources_give_the_bias(engine, layout, act):
 @pytest.mark.parametrize("value", ["nan", "inf", "-inf"])
 def test_non_finite_input_stays_in_its_halo(value, source, pad, layout):
     """One non-finite value at a corner pixel of frame 2 (63-pixel frames: tiles span two frames; balanced: stream-K cut
-    tiles): the non-finite outputs are exactly the reference's, the rest of the batch meets its bar."""
+    tiles), under no activation, ELU and sigmoid: the non-finite outputs are the reference's (tensor cores: NaN also
+    allowed where the pre-activation is non-finite), the rest of the batch meets its bar."""
     g = Geo(layout, 4, 7, 9, 40, 24, 48)
     gen = torch.Generator(device=DEV).manual_seed(11)
     hw = g.h * g.w
@@ -241,13 +287,13 @@ def test_non_finite_input_stays_in_its_halo(value, source, pad, layout):
     b = _rand((g.cout,), gen)
     pix = 2 * hw + 0 * g.w + (g.w - 1)               # frame 2, y = 0, x = W - 1
     (x0 if source == "x0" else x1)[pix, 5] = float(value)
-    for engine in ENGINES:
-        y, maxima = run(engine, g, x0, x1, wt, b, pad=pad)
+    for act, engine in ((act, engine) for act in (ACT_NONE, ACT_ELU, ACT_SIGMOID) for engine in ENGINES):
+        y, maxima = run(engine, g, x0, x1, wt, b, pad=pad, act=act)
         if engine == "f16x3":                       # the library's maxima skip the non-finite value
             assert float(maxima[0]) == cr.finite_max(x0) and float(maxima[1]) == cr.finite_max(x1)
-        y64, s, f = reference(engine, g, x0, x1, wt, b, maxima, pad=pad)
-        assert 0 < int((~torch.isfinite(y64)).any(1).sum()) <= 9
-        check(engine, y, y64, s, f, "non-finite", value)
+        y64, s, f, pre64 = reference(engine, g, x0, x1, wt, b, maxima, pad=pad, act=act)
+        assert 0 < int((~torch.isfinite(pre64)).any(1).sum()) <= 9
+        check(engine, y, y64, s, f, "non-finite/%d" % act, value, act=act, pre64=pre64)
 
 
 # ------------------------------------------------------------------------------------------ decoder batch isolation

@@ -73,6 +73,16 @@ __device__ __forceinline__ float finite_abs(float v) {
   return a < INFINITY ? a : 0.f;
 }
 
+// v rounded to tf32 to nearest (cvt.rna), the hi piece of a round-to-nearest tf32 split.  A finite |v| >= (2 - 2^-11)
+// 2^127 rounds up to Inf, and its remainder v - hi would be -Inf: there hi is v truncated to tf32 instead, which never
+// overflows and leaves an exact finite remainder.  Every other v keeps cvt.rna's bits.
+__device__ __forceinline__ float tf32_rna_finite(float v) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(v));
+  const float hi = __uint_as_float(r);
+  return (fabsf(hi) == INFINITY && fabsf(v) < INFINITY) ? __uint_as_float(__float_as_uint(v) & 0xFFFFE000u) : hi;
+}
+
 __device__ __forceinline__ float activate(float v, int act, float p) {
   switch (act) {
     case WMD_ACT_ELU: return v > 0.f ? v : expm1_nonpos(v);

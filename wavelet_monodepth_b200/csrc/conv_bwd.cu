@@ -126,11 +126,7 @@ static WgPlan wg_plan(const wmd_conv_desc& d) {
   return p;
 }
 
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
-  return r;
-}
+__device__ __forceinline__ uint32_t to_tf32(float x) { return __float_as_uint(tf32_rna_finite(x)); }
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = to_tf32(x);
   lo = to_tf32(x - __uint_as_float(hi));

@@ -327,12 +327,6 @@ __host__ __device__ __forceinline__ int f16_scale_exp(float m) {
   return e < -126 ? -126 : (e > 127 ? 127 : e);
 }
 
-__device__ __forceinline__ float tf32_rna(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
 // Balanced mode plan, shared by the conv kernel and the reduce pass (both derive it from the device-side row count).
 // All but the last full round of tiles run data-parallel (whole tiles); the last full round and the partial round
 // after it - between 1 and 2 x CTAs - 1 tiles - are cut stream-K style into equal ranges of U units per CTA.  Merging
@@ -1015,8 +1009,8 @@ __global__ void pack_weight_tc_kernel(const float* __restrict__ w, float* __rest
       const int ci = (src1 ? c0 : 0) + ci_local;
       v = __ldg(w + (static_cast<long long>(co) * Cin + ci) * taps + tap);
     }
-    const float hi = tf32_rna(v);
-    const float val = hilo == 0 ? hi : tf32_rna(v - hi);
+    const float hi = tf32_rna_finite(v);
+    const float val = hilo == 0 ? hi : tf32_rna_finite(v - hi);
     const long long tile_base = ((static_cast<long long>(nt) * nchunks + c) * 2 + hilo) * tile_floats;
     const int piece = kk >> 2, within = kk & 3;
     out[tile_base + static_cast<long long>(n) * TC_BK + ((piece ^ (n & 7)) << 2) + within] = val;

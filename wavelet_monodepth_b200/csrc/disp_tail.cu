@@ -41,12 +41,6 @@ static_assert(PACKED % 4 == 0 && (PACKED + PPIX * CP) % 4 == 0, "16-byte aligned
 static_assert(TH * TW == 2 * THREADS, "two output pixels per thread");
 }  // namespace dt
 
-__device__ __forceinline__ float dt_tf32_round(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
 __device__ __forceinline__ void dt_mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};\n"
@@ -74,8 +68,8 @@ __global__ void pack_disp_tail16_kernel(const float* __restrict__ w1, const floa
       if (k < 144) {
         const int tap = k >> 4, ci = k & 15;
         const float w = __ldg(w1 + (n * 16 + ci) * 9 + tap);
-        const float hi = dt_tf32_round(w);
-        v = lo ? dt_tf32_round(w - hi) : hi;
+        const float hi = tf32_rna_finite(w);
+        v = lo ? tf32_rna_finite(w - hi) : hi;
       }
     } else if (i < OFF_W2) {
       v = b1 ? __ldg(b1 + (i - OFF_B1)) : 0.f;

@@ -31,12 +31,6 @@ struct HeadMlpCfg {
   static_assert(C % 16 == 0 && N1 % 32 == 0, "k-steps are taken in pairs, n8-tiles four at a time");
 };
 
-__device__ __forceinline__ float tf32_round(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
 __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
       "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};\n"
@@ -83,8 +77,8 @@ __global__ void pack_head_mlp_kernel(const float* __restrict__ w1, const float* 
       out[i] = b1 ? __ldg(b1 + j) : 0.f;
       continue;
     }
-    const float hi = tf32_round(v);
-    out[i] = lo ? tf32_round(v - hi) : hi;
+    const float hi = tf32_rna_finite(v);
+    out[i] = lo ? tf32_rna_finite(v - hi) : hi;
   }
 }
 
