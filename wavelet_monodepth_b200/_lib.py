@@ -6,7 +6,7 @@ infrastructure and is never imported from here.)
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_longlong, c_size_t, c_void_p)
+from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_longlong, c_size_t, c_void_p)
 
 import torch
 
@@ -139,6 +139,17 @@ SIGNATURES = {
     "wmd_pack_disp_tail16_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "wmd_disp_tail16_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
+# include/wmd_eval.h: the KITTI evaluation entry points (tests/test_oracle_kitti_eval.py checks this table against it)
+EVAL_SIGNATURES = {
+    "wmd_eval_gt_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "wmd_eval_gather_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "wmd_eval_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_int, c_int, c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p]),
+    "wmd_eval_errors_f64": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "wmd_post_process_disparity": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
+}
+EVAL_EIGEN, EVAL_GT_POSITIVE = 0, 1
 DISP_TAIL16_PACKED_FLOATS = 5332          # WMD_DISP_TAIL16_PACKED_FLOATS
 
 _lib = None
@@ -167,7 +178,7 @@ def load():
             except OSError:
                 continue
         lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in list(SIGNATURES.items()) + list(EVAL_SIGNATURES.items()):
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args

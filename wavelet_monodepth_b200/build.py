@@ -26,7 +26,7 @@ def sources():
 
 
 def _deps():
-    return sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + [os.path.join(REPO, "include", "wmd.h")]
+    return sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(REPO, "include", "*.h"))
 
 
 def is_stale():
