@@ -1,5 +1,6 @@
 /*
- * wmd_eval.h - KITTI depth evaluation entry points of libwmd.so (KITTI/evaluate_depth.py on the device).
+ * wmd_eval.h - depth evaluation entry points of libwmd.so: KITTI (KITTI/evaluate_depth.py) and NYUv2
+ * (NYUv2/utils.py: add_results, evaluate, compute_errors_nyu) on the device.
  *
  * Same conventions as wmd.h (device pointers, caller-owned buffers, asynchronous on `stream`, no host sync, wmd_status
  * return codes).  Kept apart from wmd.h: these kernels score decoder output, they are not part of the decoder path
@@ -50,6 +51,40 @@ int wmd_eval_errors_f64(const double* gt, const double* pred, int n, double* err
  * -> out fp64, with linspace(0, 1, w) as numpy forms it and m_disp = 0.5 (l + r) in the inputs' precision. */
 int wmd_post_process_disparity(const void* l_disp, const void* r_disp, int in_f64, double* out, int N, int h, int w,
                                wmd_stream_t stream);
+
+/* ---------------------------------------------------------------- NYUv2 depth evaluation (NYUv2/utils.py)
+ * evaluate() / add_results() (:183-335) for n frames.  disp (n, h, w) fp32 is the decoder's ("disp", 0).  Per frame,
+ * in fp64 from the fp32 values:
+ *   1. p = disp / 100, or with use_disparity DepthNorm(disp, 1000) / 10000 as torch evaluates it:
+ *      (reciprocal(disp) * 1000) / 10000;
+ *   WMD_EVAL_NYU_EIGEN (any h x w):
+ *   2. bilinear, align_corners=True, to (224, 304);  3. ReplicationPad2d(8) to (240, 320);
+ *   4. bilinear, align_corners=True, to (480, 640) (scale_factor 2 plays no part: the scale is (in - 1) / (out - 1));
+ *   5. clamp to [0.4, 10];  6. crop rows 20..459, columns 24..615 -> (440, 592);
+ *   WMD_EVAL_NYU_224 (h = w = 224): steps 1 and 5 only -> (224, 224).
+ * Each resize is torch's formula and order, h0 * (w0 * x00 + w1 * x01) + h1 * (w0 * x10 + w1 * x11), with
+ * src = scale * d, lambda = src - (int)src, w0 = 1 - lambda and the second tap at i0 + (i0 < in - 1), all with
+ * explicit _rn operations.  Taps with zero weight are still read and multiplied, as torch does, so a NaN or +-Inf
+ * disparity spreads NaN to outputs that give it zero weight; the clamp compares, so NaN stays NaN.
+ * gt, gt_log10: (n, 440, 592) or (n, 224, 224) fp32, the ground truth as the metrics see it (the Eigen crop, or the
+ * border-cropped 224 x 224 resize) and its float32 log10 (the reference takes torch.log10 of the float32 values).
+ * compute_errors_nyu (:85-98) with y = gt, x = the prediction, summed per frame in fp64 in a fixed order (a fixed grid
+ * of CTAs per frame, a fixed tree in each, the slabs added in order; no atomics):
+ *   sums (n, 7) = sum |y - x| / y, sum (y - x)^2, sum |log10 y - log10 x| (log10 x in fp64), the counts of
+ *   max(y / x, x / y) < 1.25, 1.25^2, 1.25^3 (NaN-propagating max), and the pixel count.
+ * No pixel is masked.  depth_out (nullable): the fp64 prediction map, the reference's `predictions`.  ws: at least
+ * wmd_eval_nyu_ws_bytes(n, mode) bytes (0 for a bad mode or n < 0).  Bits do not depend on n or timing. */
+enum { WMD_EVAL_NYU_EIGEN = 0, WMD_EVAL_NYU_224 = 1, WMD_EVAL_NYU_CROP_H = 440, WMD_EVAL_NYU_CROP_W = 592 };
+size_t wmd_eval_nyu_ws_bytes(int n, int mode);
+int wmd_eval_nyu_frames(const float* disp, int n, int h, int w, int mode, int use_disparity, const float* gt,
+                        const float* gt_log10, double* depth_out, void* ws, size_t ws_bytes, double* sums,
+                        wmd_stream_t stream);
+/* compute_errors_nyu (:85-98) of n fp64 pairs, log10 y in fp64 too: the same sums, pooled over a fixed grid of CTAs
+ * of 4096 pixels each and added in CTA order -> errors[6] = rel, rms, log_10, a1, a2, a3.  ws: at least
+ * wmd_eval_nyu_errors_ws_bytes(n) bytes. */
+size_t wmd_eval_nyu_errors_ws_bytes(long long n);
+int wmd_eval_nyu_errors_f64(const double* pred, const double* gt, long long n, void* ws, size_t ws_bytes,
+                            double* errors, wmd_stream_t stream);
 
 #ifdef __cplusplus
 }

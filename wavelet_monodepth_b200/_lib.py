@@ -139,7 +139,7 @@ SIGNATURES = {
     "wmd_pack_disp_tail16_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "wmd_disp_tail16_f32": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
 }
-# include/wmd_eval.h: the KITTI evaluation entry points (tests/test_oracle_kitti_eval.py checks this table against it)
+# include/wmd_eval.h: the KITTI and NYUv2 evaluation entry points (tests/test_oracle_kitti_eval.py checks this table against it)
 EVAL_SIGNATURES = {
     "wmd_eval_gt_mask": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "wmd_eval_gather_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
@@ -148,8 +148,15 @@ EVAL_SIGNATURES = {
                                 c_void_p]),
     "wmd_eval_errors_f64": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "wmd_post_process_disparity": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "wmd_eval_nyu_ws_bytes": (c_size_t, [c_int, c_int]),
+    "wmd_eval_nyu_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_size_t, c_void_p, c_void_p]),
+    "wmd_eval_nyu_errors_ws_bytes": (c_size_t, [c_longlong]),
+    "wmd_eval_nyu_errors_f64": (c_int, [c_void_p, c_void_p, c_longlong, c_void_p, c_size_t, c_void_p, c_void_p]),
 }
 EVAL_EIGEN, EVAL_GT_POSITIVE = 0, 1
+EVAL_NYU_EIGEN, EVAL_NYU_224 = 0, 1                       # WMD_EVAL_NYU_EIGEN, WMD_EVAL_NYU_224
+EVAL_NYU_CROP_H, EVAL_NYU_CROP_W = 440, 592
 DISP_TAIL16_PACKED_FLOATS = 5332          # WMD_DISP_TAIL16_PACKED_FLOATS
 
 _lib = None
