@@ -110,13 +110,32 @@ __host__ __device__ __forceinline__ int win_base(int m0, int W, int shift) {
   return (Y0 > 0 ? (Y0 - 1) >> 1 : -1) * (W >> 1);
 }
 
-// Window mode: a ring of weight-only stages beside two window slots, the producer's tap tables, the barriers (full[s],
-// empty[s] of the ring, then full / empty of the two slots) and the alignment slack: 4 stages for tf32 N = 128, 8 for
-// the rest.
-template <int BN, bool F16>
+// Row-set mode (conv_rows_tc_kernel_rowset): a 3x3 launch through a pixel list, index maps or a gate reads no contiguous
+// range, but the 9 x 128 tap rows a tile reads from one source repeat heavily (a 128-pixel tile of the KITTI decoder's
+// sparse levels reads 100 - 470 distinct rows of a source in its 1152 tap slots).  So once per tile and source the
+// producer collects the distinct rows - a bitmap over the tile's [min, max] row range, thread t owning word t, then
+// popcount ranks: ascending order, whatever the thread timing - and a uint16 table [tap][row] of ranks (dead and padded
+// taps: the zero row).  Per channel chunk it then loads the distinct rows' 32-channel slices into a slot, as the window
+// form does, and the consumers read the slot through the same table form.  A source whose range exceeds the bitmap
+// (TC_SET_SPAN) or whose distinct rows exceed the slot (TC_SET_ROWS) stages one slot per tap instead - the tap's 128
+// gathered rows, identity table - and says so in the slot's flag word, so the consumers wait for a slot at every step.
+// The rows a step reads, and so the bits, are the same either way.
+constexpr int TC_SET_ROWS = 480;
+constexpr int TC_SET_SPAN = 32 * TC_PRODUCERS;                     // bitmap rows: one 32-bit word per producer thread
+constexpr int TC_SET_DATA = (TC_SET_ROWS + 1) * TC_A_LD * 4;
+constexpr int TC_SET_SLOT = TC_SET_DATA + TC_WIN_TAB + 16;         // rows + zero row, the table, the flag word (per tap)
+// the producer's per-source scratch: rank tables, distinct rows, bitmap words, their rank bases; then 128 B of reductions
+constexpr int TC_SET_SCRATCH = 2 * (TC_WIN_TAB + TC_SET_ROWS * 4 + 2 * TC_PRODUCERS * 4) + 128;
+static_assert(TC_SET_DATA % 16 == 0 && TC_SET_SLOT % 16 == 0 && TC_SET_SCRATCH % 16 == 0, "slot rows take 16-byte cp.async");
+
+// Window and row-set modes: a ring of weight-only stages beside two slots, the producer's tap tables (and the row-set
+// scratch), the barriers (full[s], empty[s] of the ring, then full / empty of the two slots) and the alignment slack.
+// Window: 4 stages for tf32 N = 128, 8 for the rest; row set: 4 for the 16 KB weight images (f16 N = 128, tf32
+// N = 64), 8 for the smaller ones (tf32 N = 128, two stages, is not built: tc_rowset_takes).
+template <int BN, bool F16, bool SET = false>
 struct TcWinCfg {
   static constexpr int B_IMG = TcCfg<BN, F16>::B_IMG;
-  static constexpr int FIXED = 2 * TC_WIN_SLOT + TC_TABLES + 4 * 8 + 1024;
+  static constexpr int FIXED = 2 * (SET ? TC_SET_SLOT : TC_WIN_SLOT) + TC_TABLES + (SET ? TC_SET_SCRATCH : 0) + 4 * 8 + 1024;
   static constexpr int FIT = (TC_SMEM_MAX - FIXED) / (B_IMG + 2 * 8);
   static constexpr int STAGES = FIT < TC_MAX_STAGES ? FIT : TC_MAX_STAGES;
   static constexpr size_t SMEM = static_cast<size_t>(STAGES) * B_IMG + FIXED + 2 * STAGES * 8;
@@ -413,17 +432,26 @@ struct TcWalk {
 template <int V>
 struct Ic { static constexpr int value = V; };   // a compile-time register-set index
 
-// WIN: window mode (dense 3x3 layers, see TC_WIN_ROWS): stages hold weights only, A comes from the window slots.
-template <int BN, bool F16, bool WIN>
+// How A reaches shared memory: gathered per (chunk, tap) into the stage, or loaded once per channel chunk into a slot as
+// a window (dense 3x3 layers, see TC_WIN_ROWS) or as a tile's distinct rows (the other 3x3 layers, see TC_SET_ROWS).
+enum TcFeed { kFeedGather = 0, kFeedWindow = 1, kFeedRowset = 2 };
+
+template <int BN, bool F16, int FEED>
 __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const float* __restrict__ wtc, const int splits,
                                                   float* __restrict__ partial) {
   using Cfg = TcCfg<BN, F16>;
+  constexpr bool WIN = FEED != kFeedGather;                 // stages hold weights only, A comes from the two slots
+  constexpr bool SET = FEED == kFeedRowset;
   constexpr int TC_B_TILE = Cfg::B_TILE;
   constexpr int B_IMG = Cfg::B_IMG;                         // bytes of one chunk's weight image
   constexpr int ACC = Cfg::ACC;
   constexpr int STAGE = WIN ? B_IMG : Cfg::STAGE;
-  constexpr int STAGES = WIN ? TcWinCfg<BN, F16>::STAGES : Cfg::STAGES;
-  constexpr int SLOTS = WIN ? 2 * TC_WIN_SLOT : 0;
+  constexpr int STAGES = WIN ? TcWinCfg<BN, F16, SET>::STAGES : Cfg::STAGES;
+  constexpr int SLOT_ROWS = SET ? TC_SET_ROWS : TC_WIN_ROWS;  // slot row SLOT_ROWS holds zeros
+  constexpr int SLOT_DATA = SET ? TC_SET_DATA : TC_WIN_DATA;
+  constexpr int SLOT = SET ? TC_SET_SLOT : TC_WIN_SLOT;
+  constexpr int SLOTS = WIN ? 2 * SLOT : 0;
+  constexpr int SCRATCH = SET ? TC_SET_SCRATCH : 0;
   extern __shared__ unsigned char smem_dyn[];
   __shared__ int s_fixup;                                  // balanced mode: segments of the tile to reduce here (0 = not the last)
 
@@ -432,12 +460,19 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
   // diverge inside a warp, and are not serialised
   const int warpgroup = __shfl_sync(0xffffffffu, tid / 128, 0);
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~static_cast<uintptr_t>(1023));
-  unsigned char* wslot = base + STAGES * STAGE;                            // window slots j = 0, 1: rows, then the table
+  unsigned char* wslot = base + STAGES * STAGE;                            // slots j = 0, 1: rows, the table (, the flag)
   int32_t* tab0 = reinterpret_cast<int32_t*>(base + STAGES * STAGE + SLOTS);   // [tap][row]: source row in x0, -1 = none
   int32_t* tab1 = tab0 + 9 * TC_BM;                                        // ... in x1
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + STAGES * STAGE + SLOTS + TC_TABLES);   // stage s holds its chunk
+  // row-set scratch (producer only), per source: rank tables [tap][row], distinct rows, bitmap words, their rank bases
+  unsigned char* sx = base + STAGES * STAGE + SLOTS + TC_TABLES;
+  uint16_t* set_tab = reinterpret_cast<uint16_t*>(sx);
+  int32_t* set_rows = reinterpret_cast<int32_t*>(sx + 2 * TC_WIN_TAB);
+  uint32_t* set_bits = reinterpret_cast<uint32_t*>(set_rows + 2 * TC_SET_ROWS);
+  int32_t* set_rank = reinterpret_cast<int32_t*>(set_bits + 2 * TC_PRODUCERS);
+  int32_t* set_red = set_rank + 2 * TC_PRODUCERS;          // [0, 8): warp min / max, [8, 12): warp counts, [12, 16): per source staged, count
+  uint64_t* full = reinterpret_cast<uint64_t*>(sx + SCRATCH);   // stage s holds its chunk
   uint64_t* empty = full + STAGES;                                                       // both consumers are done with s
-  uint64_t* wfull = empty + STAGES;                        // window mode: slot j holds its channel chunk's rows and table
+  uint64_t* wfull = empty + STAGES;                        // window / row set: slot j holds its channel chunk's rows and table
   uint64_t* wempty = wfull + 2;                            // ... every consumer warp has read slot j for the last time
 
   const long long HW = static_cast<long long>(d.H) * d.W;
@@ -471,7 +506,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
   }
   if (WIN && tid < 2 * TC_A_LD) {                          // the zero row of each slot, never overwritten
     const int j = tid / TC_A_LD;
-    reinterpret_cast<float*>(wslot + j * TC_WIN_SLOT)[TC_WIN_ROWS * TC_A_LD + tid % TC_A_LD] = 0.f;
+    reinterpret_cast<float*>(wslot + j * SLOT)[SLOT_ROWS * TC_A_LD + tid % TC_A_LD] = 0.f;
   }
   __syncthreads();
 
@@ -554,6 +589,76 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
         }
       }
       named_bar_sync(kProducerBar, TC_PRODUCERS);
+      if constexpr (SET) {
+        // Row-set mode: each source's distinct rows in ascending order and the rank table (see TC_SET_ROWS).  Thread t
+        // owns bitmap word t and tile row t of the tables; the scratch is free again for the same reason the tap table is.
+        const int warp = tid >> 5;
+#pragma unroll 1
+        for (int s = 0; s < (d.c1 > 0 ? 2 : 1); ++s) {
+          const int32_t* tab = s ? tab1 : tab0;
+          uint32_t* bits = set_bits + s * TC_PRODUCERS;
+          int32_t* rank = set_rank + s * TC_PRODUCERS;
+          int lo = 0x7fffffff, hi = -1;                    // the tile's row range in this source
+#pragma unroll 1
+          for (int t = 0; t < 9; ++t) {
+            const int32_t a = tab[t * TC_BM + tid];
+            if (a >= 0) { lo = min(lo, a); hi = max(hi, a); }
+          }
+          lo = __reduce_min_sync(0xffffffffu, lo);
+          hi = __reduce_max_sync(0xffffffffu, hi);
+          if (lane == 0) { set_red[2 * warp] = lo; set_red[2 * warp + 1] = hi; }
+          bits[tid] = 0u;
+          named_bar_sync(kProducerBar, TC_PRODUCERS);
+#pragma unroll
+          for (int k = 0; k < TC_PRODUCERS / 32; ++k) { lo = min(lo, set_red[2 * k]); hi = max(hi, set_red[2 * k + 1]); }
+          const bool fits = hi < lo || hi - lo < TC_SET_SPAN;   // hi < lo: no live tap
+          if (fits) {
+#pragma unroll 1
+            for (int t = 0; t < 9; ++t) {
+              const int32_t a = tab[t * TC_BM + tid];
+              if (a >= 0) atomicOr(bits + ((a - lo) >> 5), 1u << ((a - lo) & 31));
+            }
+          }
+          named_bar_sync(kProducerBar, TC_PRODUCERS);
+          const uint32_t w = bits[tid];
+          int incl = __popc(w);                            // inclusive prefix of the words' popcounts
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+          }
+          if (lane == 31) set_red[8 + warp] = incl;
+          named_bar_sync(kProducerBar, TC_PRODUCERS);
+          int r = incl - __popc(w), total = 0;
+#pragma unroll
+          for (int k = 0; k < TC_PRODUCERS / 32; ++k) {
+            const int n = set_red[8 + k];
+            total += n;
+            if (k < warp) r += n;
+          }
+          const bool staged = fits && total <= TC_SET_ROWS;
+          if (tid == 0) { set_red[12 + 2 * s] = staged; set_red[13 + 2 * s] = total; }
+          if (staged) {
+            rank[tid] = r;
+            int32_t* rows_s = set_rows + s * TC_SET_ROWS;
+            for (uint32_t m = w; m; m &= m - 1) rows_s[r++] = lo + 32 * tid + (__ffs(m) - 1);
+          }
+          named_bar_sync(kProducerBar, TC_PRODUCERS);
+          if (staged) {
+            uint16_t* st = set_tab + s * 9 * TC_BM;
+#pragma unroll 1
+            for (int t = 0; t < 9; ++t) {
+              const int32_t a = tab[t * TC_BM + tid];
+              int v = TC_SET_ROWS;
+              if (a >= 0) {
+                const int o = a - lo;
+                v = rank[o >> 5] + __popc(bits[o >> 5] & ((1u << (o & 31)) - 1u));
+              }
+              st[t * TC_BM + tid] = static_cast<uint16_t>(v);
+            }
+          }
+        }
+      }
 
       // Chunk c of the tile into stage s: the weight image as it is (one bulk copy), and the implicit im2col - for every
       // tile row the 32-channel slice of its tap's source row (channel chunk outermost, taps innermost: the nine taps of
@@ -577,33 +682,60 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
         const long long ld = src1 ? d.ld1 : d.ld0;
         const int csrc = src1 ? d.c1 : d.c0;
         if constexpr (WIN) {
-          // A channel chunk's first step in this segment (a stream-K segment may start at any tap) loads its window
-          // into the next slot: the table made window-relative, then the rows, zero filled as the gather does.
-          if (c != it.cb && tap != 0) continue;
+          // A channel chunk's first step in this segment (a stream-K segment may start at any tap) loads its window or
+          // row set into the next slot: the table, then the rows, zero filled as the gather does.  A row-set source
+          // staged per tap loads a slot at every step: the tap's 128 gathered rows, identity table.
+          const bool tap_slots = SET && !set_red[12 + 2 * src1];
+          if (c != it.cb && tap != 0 && !tap_slots) continue;
           const int j = static_cast<int>(wi & 1);
           if (wi >= 2) mbar_wait(wempty + j, ((wi >> 1) - 1) & 1);
-          float* sw = reinterpret_cast<float*>(wslot + j * TC_WIN_SLOT);
-          uint16_t* wt = reinterpret_cast<uint16_t*>(wslot + j * TC_WIN_SLOT + TC_WIN_DATA);
-          const int shift = src1 ? 0 : d.shift0;
-          const int wb = win_base(m0, d.W, shift), wn = win_rows(d.W, shift);
-          const long long nrows = src1 ? rows_x1 : rows_x0;
-          const int32_t* tab = src1 ? tab1 : tab0;
-#pragma unroll
-          for (int t = 0; t < 9; ++t) {
-            const int32_t a = tab[t * TC_BM + tid];
-            const int o = a - wb;
-            wt[t * TC_BM + tid] = static_cast<uint16_t>(a != kNoRow && o >= 0 && o < wn ? o : TC_WIN_ROWS);
-          }
+          float* sw = reinterpret_cast<float*>(wslot + j * SLOT);
+          uint16_t* wt = reinterpret_cast<uint16_t*>(wslot + j * SLOT + SLOT_DATA);
+          if constexpr (SET) {
+            // slot row r holds source row rows_s[r] (-1: zeros): the distinct rows and their rank table, or the tap's
+            // gathered rows and the identity
+            const int32_t* rows_s = tab0 + (src1 * 9 + tap) * TC_BM;
+            int n = TC_BM;
+            if (tap_slots) {
+              wt[tap * TC_BM + tid] = static_cast<uint16_t>(tid);
+            } else {
+              const uint16_t* stb = set_tab + src1 * 9 * TC_BM;
 #pragma unroll 1
-          for (int pc = tid; pc < wn * 8; pc += TC_PRODUCERS) {
-            const int r = pc >> 3, q = pc & 7;
-            const long long srow = static_cast<long long>(wb) + r;
-            const int cc = col + 4 * q;
-            const int bytes = (srow >= 0 && srow < nrows) ? min(16, max(0, (csrc - cc) * 4)) : 0;
-            cp_async16(sw + r * TC_A_LD + 4 * q, bytes ? x + srow * ld + cc : x, bytes);
+              for (int t = 0; t < 9; ++t) wt[t * TC_BM + tid] = stb[t * TC_BM + tid];
+              rows_s = set_rows + src1 * TC_SET_ROWS;
+              n = set_red[13 + 2 * src1];
+            }
+            if (tid == 0) *reinterpret_cast<uint32_t*>(wslot + j * SLOT + SLOT_DATA + TC_WIN_TAB) = tap_slots;
+#pragma unroll 1
+            for (int pc = tid; pc < n * 8; pc += TC_PRODUCERS) {
+              const int r = pc >> 3, q = pc & 7;
+              const int32_t srow = rows_s[r];
+              const int cc = col + 4 * q;
+              const int bytes = srow >= 0 ? min(16, max(0, (csrc - cc) * 4)) : 0;
+              cp_async16(sw + r * TC_A_LD + 4 * q, bytes ? x + static_cast<long long>(srow) * ld + cc : x, bytes);
+            }
+          } else {
+            const int32_t* tab = src1 ? tab1 : tab0;
+            const int shift = src1 ? 0 : d.shift0;
+            const int wb = win_base(m0, d.W, shift), wn = win_rows(d.W, shift);
+            const long long nrows = src1 ? rows_x1 : rows_x0;
+#pragma unroll
+            for (int t = 0; t < 9; ++t) {
+              const int32_t a = tab[t * TC_BM + tid];
+              const int o = a - wb;
+              wt[t * TC_BM + tid] = static_cast<uint16_t>(a != kNoRow && o >= 0 && o < wn ? o : TC_WIN_ROWS);
+            }
+#pragma unroll 1
+            for (int pc = tid; pc < wn * 8; pc += TC_PRODUCERS) {
+              const int r = pc >> 3, q = pc & 7;
+              const long long srow = static_cast<long long>(wb) + r;
+              const int cc = col + 4 * q;
+              const int bytes = (srow >= 0 && srow < nrows) ? min(16, max(0, (csrc - cc) * 4)) : 0;
+              cp_async16(sw + r * TC_A_LD + 4 * q, bytes ? x + srow * ld + cc : x, bytes);
+            }
           }
-          // cp.async's arrival tracks only its copies; the plain arrive (release) publishes this thread's table stores
-          // to the consumers' wait (acquire)
+          // cp.async's arrival tracks only its copies; the plain arrive (release) publishes this thread's table (and
+          // flag) stores to the consumers' wait (acquire)
           cp_async_mbar_arrive(wfull + j);
           mbar_arrive(wfull + j);
           ++wi;
@@ -667,14 +799,14 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
 #pragma unroll
   for (int j = 0; j < ACC; ++j) dacc[j] = 0.f;
 
-  // Window mode: chunk c of a segment that starts at chunk cb reads window number wc + c / 9 - cb / 9 (wc: windows this
-  // CTA consumed in earlier segments), slot (that number) & 1.
-  uint32_t wc = 0;
+  // Window and row-set modes: a segment's first chunk and every channel chunk's first tap start the next slot (slot
+  // number & 1), and so does every step of a row-set source staged per tap (the flag word of the slot in use).
+  uint32_t wnext = 0, wcur = 0;                            // slots this CTA has started; the slot of the chunk last loaded
+  bool tap_slots = false;
   int seg_cb = 0;
-  auto win_of = [&](int i) { return wc + static_cast<uint32_t>((seg_cb + i) / 9 - seg_cb / 9); };
 
-  // wait for stage gi % STAGES to hold chunk gi (and in window mode, at the chunk's first step of the segment, for its
-  // window), then read this thread's fragment elements (chunk i of the segment) into register set B
+  // wait for stage gi % STAGES to hold chunk gi (and in window / row-set mode, at a slot's first step, for its slot),
+  // then read this thread's fragment elements (chunk i of the segment) into register set B
   auto load_frag = [&](auto B, uint32_t gi, int i) {
     constexpr int b = decltype(B)::value;
     const int s = static_cast<int>(gi % STAGES);
@@ -682,12 +814,15 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
     const float* sa = reinterpret_cast<const float*>(base + s * STAGE + B_IMG);
     int pr0 = row_a * TC_A_LD, pr1 = (row_a + 8) * TC_A_LD;   // float offsets of this thread's two fragment rows
     if constexpr (WIN) {
-      const uint32_t wn = win_of(i);
-      const int j = static_cast<int>(wn & 1);
       const int tap = (seg_cb + i) % 9;
-      if (i == 0 || tap == 0) mbar_wait(wfull + j, (wn >> 1) & 1);
-      sa = reinterpret_cast<const float*>(wslot + j * TC_WIN_SLOT);
-      const uint16_t* wt = reinterpret_cast<const uint16_t*>(wslot + j * TC_WIN_SLOT + TC_WIN_DATA) + tap * TC_BM;
+      if (i == 0 || tap == 0 || tap_slots) {
+        wcur = wnext++;
+        mbar_wait(wfull + (wcur & 1), (wcur >> 1) & 1);
+        if constexpr (SET) tap_slots = *reinterpret_cast<const uint32_t*>(wslot + (wcur & 1) * SLOT + SLOT_DATA + TC_WIN_TAB) != 0u;
+      }
+      const int j = static_cast<int>(wcur & 1);
+      sa = reinterpret_cast<const float*>(wslot + j * SLOT);
+      const uint16_t* wt = reinterpret_cast<const uint16_t*>(wslot + j * SLOT + SLOT_DATA) + tap * TC_BM;
       pr0 = wt[row_a] * TC_A_LD;
       pr1 = wt[row_a + 8] * TC_A_LD;
     }
@@ -769,11 +904,11 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
       }
       wgmma_commit();
       if constexpr (WIN) {
-        // chunk i's fragments are in registers (its MMAs are issued): after its channel chunk's last step in this
-        // segment, the window slot goes back to the producer
-        if ((seg_cb + i) % 9 == 8 || i + 1 == len) {
+        // chunk i's fragments are in registers (its MMAs are issued): after the slot's last step in this segment, the
+        // slot goes back to the producer
+        if ((seg_cb + i) % 9 == 8 || i + 1 == len || tap_slots) {
           __syncwarp();
-          if (lane == 0) mbar_arrive(wempty + (win_of(i) & 1));
+          if (lane == 0) mbar_arrive(wempty + (wcur & 1));
         }
       }
       wgmma_wait<1>();                                     // chunk i - 1 has retired
@@ -804,7 +939,6 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
     }
     release(g + len - 1);
     g += len;
-    if (WIN) wc = win_of(len - 1) + 1;
 
     if (F16 && whole && out_pre != 1.f) {
 #pragma unroll
@@ -966,18 +1100,24 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
   }
 }
 
-// Two kernels with their own names, so that a profile tells them apart; the window form's name extends the gather
-// form's, so a search for the tensor-core engine by name finds both.  The window form runs the dense 3x3 launches whose
-// windows fit (tc_window_fits), the gather form every other launch.  Both give the same bits.
+// Three kernels with their own names, so that a profile tells them apart; the window and row-set forms' names extend the
+// gather form's, so a search for the tensor-core engine by name finds all three.  The window form runs the dense 3x3
+// launches whose windows fit (tc_window_fits), the row-set form the other 3x3 launches that are not split
+// (tc_rowset_takes), the gather form every other launch.  All three give the same bits.
 template <int BN, bool F16>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel(const wmd_conv_desc d, const float* __restrict__ wtc,
                                                                      const int splits, float* __restrict__ partial) {
-  conv_rows_tc_body<BN, F16, false>(d, wtc, splits, partial);
+  conv_rows_tc_body<BN, F16, kFeedGather>(d, wtc, splits, partial);
 }
 template <int BN, bool F16>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel_window(const wmd_conv_desc d, const float* __restrict__ wtc,
                                                                          const int splits, float* __restrict__ partial) {
-  conv_rows_tc_body<BN, F16, true>(d, wtc, splits, partial);
+  conv_rows_tc_body<BN, F16, kFeedWindow>(d, wtc, splits, partial);
+}
+template <int BN, bool F16>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_rows_tc_kernel_rowset(const wmd_conv_desc d, const float* __restrict__ wtc,
+                                                                         const int splits, float* __restrict__ partial) {
+  conv_rows_tc_body<BN, F16, kFeedRowset>(d, wtc, splits, partial);
 }
 
 // w (Cout, Cin, taps) fp32 -> per (n-tile, chunk) smem image [tf32 hi: BN x 32 | tf32 lo: BN x 32], K-major,
@@ -1174,11 +1314,22 @@ static bool tc_window_fits(const wmd_conv_desc& d, int splits) {
   if (d.taps != 9 || d.pixels || d.map0 || d.map1 || d.gate || splits > 1 || d.W > TC_WIN_ROWS) return false;
   return win_rows(d.W, d.shift0) <= TC_WIN_ROWS && (d.c1 == 0 || win_rows(d.W, 0) <= TC_WIN_ROWS);
 }
+// Row-set mode (TC_SET_ROWS) takes the 3x3 launches that read through a pixel list, an index map or a gate, when their
+// tiles are not split (whole tiles or balanced).  tf32 N = 128 keeps the gather form: beside the two row-set slots its
+// ring holds only two 32 KB weight images, and the NYU decoder's sparse launches (all of that form) ran ~9 % slower so.
+static bool tc_rowset_takes(const wmd_conv_desc& d, int splits) {
+  if (d.precision == WMD_PREC_TF32X3 && tc_tile_n(d.cout) == 128) return false;
+  return d.taps == 9 && (d.pixels || d.map0 || d.map1 || d.gate) && splits <= 1;
+}
 
-template <int BN, bool F16, bool WIN>
+template <int BN, bool F16, int FEED>
 static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStream_t stream) {
-  const size_t smem = WIN ? TcWinCfg<BN, F16>::SMEM : TcCfg<BN, F16>::SMEM;
-  auto kernel = WIN ? conv_rows_tc_kernel_window<BN, F16> : conv_rows_tc_kernel<BN, F16>;
+  const size_t smem = FEED == kFeedGather ? TcCfg<BN, F16>::SMEM : TcWinCfg<BN, F16, FEED == kFeedRowset>::SMEM;
+  auto kernel = [] {                               // only the form launched here is instantiated
+    if constexpr (FEED == kFeedWindow) return conv_rows_tc_kernel_window<BN, F16>;
+    else if constexpr (FEED == kFeedRowset) return conv_rows_tc_kernel_rowset<BN, F16>;
+    else return conv_rows_tc_kernel<BN, F16>;
+  }();
   static bool attr_done[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -1200,6 +1351,15 @@ static int launch_tc(const wmd_conv_desc& d, int splits, float* partial, cudaStr
                                                               d.count, d.N * d.H * d.W, d.max_rows,
                                                               d.act, d.act_param, d.amax_out);
   return launched();
+}
+// The launch's feed form; tf32 N = 128 has no row-set build (tc_rowset_takes never picks it)
+template <int BN, bool F16>
+static int launch_feed(int feed, const wmd_conv_desc& d, int splits, float* partial, cudaStream_t stream) {
+  if (feed == kFeedWindow) return launch_tc<BN, F16, kFeedWindow>(d, splits, partial, stream);
+  if constexpr (F16 || BN != 128) {
+    if (feed == kFeedRowset) return launch_tc<BN, F16, kFeedRowset>(d, splits, partial, stream);
+  }
+  return launch_tc<BN, F16, kFeedGather>(d, splits, partial, stream);
 }
 
 }  // namespace wmd
@@ -1334,14 +1494,10 @@ extern "C" int wmd_conv_rows_tc_splitk_f32(const wmd_conv_desc* dp, int splits, 
   if (f16) WMD_REQUIRE(d.amax0 != nullptr && (d.c1 == 0 || d.amax1 != nullptr), WMD_ERR_ARG);
   if (f16) WMD_REQUIRE(splits <= 1, WMD_ERR_UNSUPPORTED);   // tc_reduce_kernel sums unscaled slabs: tf32 operands only
   cudaStream_t st = as_stream(stream);
-  const bool win = tc_window_fits(d, splits);
-#define WMD_TC_LAUNCH(BN_)                                                                                   \
-  return f16 ? (win ? launch_tc<BN_, true, true>(d, splits, partial, st) : launch_tc<BN_, true, false>(d, splits, partial, st)) \
-             : (win ? launch_tc<BN_, false, true>(d, splits, partial, st) : launch_tc<BN_, false, false>(d, splits, partial, st))
+  const int feed = tc_window_fits(d, splits) ? kFeedWindow : (tc_rowset_takes(d, splits) ? kFeedRowset : kFeedGather);
   switch (tc_tile_n(d.cout)) {
-    case 128: WMD_TC_LAUNCH(128);
-    case 64: WMD_TC_LAUNCH(64);
-    default: WMD_TC_LAUNCH(32);
+    case 128: return f16 ? launch_feed<128, true>(feed, d, splits, partial, st) : launch_feed<128, false>(feed, d, splits, partial, st);
+    case 64: return f16 ? launch_feed<64, true>(feed, d, splits, partial, st) : launch_feed<64, false>(feed, d, splits, partial, st);
+    default: return f16 ? launch_feed<32, true>(feed, d, splits, partial, st) : launch_feed<32, false>(feed, d, splits, partial, st);
   }
-#undef WMD_TC_LAUNCH
 }
