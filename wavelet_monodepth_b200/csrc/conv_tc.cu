@@ -33,6 +33,9 @@
 //     order, cooperatively and coalesced.
 // Optional fp16-pair operand form (F16 = true, wmd_conv_desc.precision): x 2^e = h1 + h2 as fp16, f16 MMAs with K = 16
 // (half the instructions), scale from the sources' max |x| (device scalars), weights' scale in the packed image's header.
+// The window and row-set forms (one slot of rows per channel chunk, read by all nine taps) split in shared memory
+// instead: at a slot's first step the 256 consumer threads turn its rows into fp16 pairs in place (split_slot_rows, the
+// same split_f16x2 the registers use), and every k-step's fragments come from one ldmatrix.x4 per piece.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -93,11 +96,13 @@ struct TcCfg {
 //     most ((D + 1) >> 1) + 2 rows of Ws (the count for Y0 even; Y0 odd gives (D >> 1) + 2), starting at
 //     ((Y0 - 1) >> 1) Ws.
 // Slots hold TC_WIN_ROWS rows plus one row of zeros (padded taps and dead rows point at it); a launch whose window is
-// larger keeps the gather path.
+// larger keeps the gather path.  After the rows and the table a slot has a 16-byte header: word 0 the row-set form's
+// per-tap flag, word 1 the number of rows loaded (the rows the f16 form's consumers split in place).
 constexpr int TC_WIN_ROWS = 288;                                   // shift 0: W <= 79
 constexpr int TC_WIN_DATA = (TC_WIN_ROWS + 1) * TC_A_LD * 4;       // rows + the zero row, 144-byte pitch
 constexpr int TC_WIN_TAB = 9 * TC_BM * 2;                          // [tap][row] uint16 window rows
-constexpr int TC_WIN_SLOT = TC_WIN_DATA + TC_WIN_TAB;
+constexpr int TC_SLOT_HDR = 16;
+constexpr int TC_WIN_SLOT = TC_WIN_DATA + TC_WIN_TAB + TC_SLOT_HDR;
 static_assert(TC_WIN_DATA % 16 == 0 && TC_WIN_SLOT % 16 == 0, "window rows take 16-byte cp.async");
 __host__ __device__ __forceinline__ int win_rows(int W, int shift) {
   if (shift == 0) return TC_BM + 2 * (W + 1);
@@ -123,7 +128,7 @@ __host__ __device__ __forceinline__ int win_base(int m0, int W, int shift) {
 constexpr int TC_SET_ROWS = 480;
 constexpr int TC_SET_SPAN = 32 * TC_PRODUCERS;                     // bitmap rows: one 32-bit word per producer thread
 constexpr int TC_SET_DATA = (TC_SET_ROWS + 1) * TC_A_LD * 4;
-constexpr int TC_SET_SLOT = TC_SET_DATA + TC_WIN_TAB + 16;         // rows + zero row, the table, the flag word (per tap)
+constexpr int TC_SET_SLOT = TC_SET_DATA + TC_WIN_TAB + TC_SLOT_HDR;   // rows + zero row, the table, the header
 // the producer's per-source scratch: rank tables, distinct rows, bitmap words, their rank bases; then 128 B of reductions
 constexpr int TC_SET_SCRATCH = 2 * (TC_WIN_TAB + TC_SET_ROWS * 4 + 2 * TC_PRODUCERS * 4) + 128;
 static_assert(TC_SET_DATA % 16 == 0 && TC_SET_SLOT % 16 == 0 && TC_SET_SCRATCH % 16 == 0, "slot rows take 16-byte cp.async");
@@ -184,7 +189,13 @@ __device__ __forceinline__ void bulk_copy_g2s(void* dst, const void* src, uint32
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
 }
-constexpr int kProducerBar = 1, kConsumerBar = 2;   // named barrier ids (0 is __syncthreads)
+// named barrier ids (0 is __syncthreads): the producer warpgroup's, the consumers' epilogue, the consumers' slot split
+constexpr int kProducerBar = 1, kConsumerBar = 2, kSplitBar = 3;
+// the four 8 x 8 b16 matrices whose rows lanes 8i .. 8i + 7 address, into r[i] (the mma fragment layout)
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];\n"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
+}
 // keeps a register that an asynchronous wgmma reads or writes live and unmoved across the wait
 __device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
@@ -330,6 +341,33 @@ __device__ __forceinline__ float f16_hi_to_f32(uint32_t pair) {
   float f;
   asm("{\n\t.reg .f16 l, h;\n\tmov.b32 {l, h}, %1;\n\tcvt.f32.f16 %0, h;\n\t}\n" : "=f"(f) : "r"(pair));
   return f;
+}
+// The fp16-pair split of two adjacent channels: x s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and
+// h2 = fp16(x s - h1), 22 mantissa bits, the precision of the tf32 hi / lo pair; each piece packed with the lower
+// channel in bits 0..15.  The gather kernel splits its fragment elements in registers, the window and row-set kernels
+// split their slots' rows in place (split_slot_rows): both through this function, so the two give the same bits.
+__device__ __forceinline__ void split_f16x2(float x0, float x1, float s, uint32_t& h1, uint32_t& h2) {
+  const float b0f = x0 * s, b1f = x1 * s;
+  h1 = pack_f16x2(b0f, b1f);
+  h2 = pack_f16x2(b0f - f16_lo_to_f32(h1), b1f - f16_hi_to_f32(h1));
+}
+// The window and row-set kernels' f16 form: the consumers (thread ctid of TC_CONSUMERS) split the first `rows` rows of a
+// slot in place, once per slot instead of once per tap that reads them.  Each 32-byte group of 8 fp32 channels becomes
+// [h1: 8 x fp16 | h2: 8 x fp16]: channels 8 q .. 8 q + 7 of a row keep bytes 32 q .. 32 q + 31, and the pitch stays
+// 144 bytes.  The zero row needs no split: fp32 zeros are fp16 zeros.
+__device__ __forceinline__ void split_slot_rows(unsigned char* slot, int rows, float s, int ctid) {
+#pragma unroll 1
+  for (int q = ctid; q < rows * 4; q += TC_CONSUMERS) {
+    uint4* p = reinterpret_cast<uint4*>(slot + (q >> 2) * (TC_A_LD * 4) + (q & 3) * 32);
+    const uint4 u = p[0], v = p[1];
+    uint4 h1, h2;
+    split_f16x2(__uint_as_float(u.x), __uint_as_float(u.y), s, h1.x, h2.x);
+    split_f16x2(__uint_as_float(u.z), __uint_as_float(u.w), s, h1.y, h2.y);
+    split_f16x2(__uint_as_float(v.x), __uint_as_float(v.y), s, h1.z, h2.z);
+    split_f16x2(__uint_as_float(v.z), __uint_as_float(v.w), s, h1.w, h2.w);
+    p[0] = h1;
+    p[1] = h2;
+  }
 }
 
 // Exponent e of the power-of-two scale of an fp16-pair operand whose (finite-value) maximum is m: m 2^e in [2^13, 2^14),
@@ -691,6 +729,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
           if (wi >= 2) mbar_wait(wempty + j, ((wi >> 1) - 1) & 1);
           float* sw = reinterpret_cast<float*>(wslot + j * SLOT);
           uint16_t* wt = reinterpret_cast<uint16_t*>(wslot + j * SLOT + SLOT_DATA);
+          uint32_t* hdr = reinterpret_cast<uint32_t*>(wslot + j * SLOT + SLOT_DATA + TC_WIN_TAB);
           if constexpr (SET) {
             // slot row r holds source row rows_s[r] (-1: zeros): the distinct rows and their rank table, or the tap's
             // gathered rows and the identity
@@ -705,7 +744,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
               rows_s = set_rows + src1 * TC_SET_ROWS;
               n = set_red[13 + 2 * src1];
             }
-            if (tid == 0) *reinterpret_cast<uint32_t*>(wslot + j * SLOT + SLOT_DATA + TC_WIN_TAB) = tap_slots;
+            if (tid == 0) { hdr[0] = tap_slots; hdr[1] = n; }
 #pragma unroll 1
             for (int pc = tid; pc < n * 8; pc += TC_PRODUCERS) {
               const int r = pc >> 3, q = pc & 7;
@@ -719,6 +758,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
             const int shift = src1 ? 0 : d.shift0;
             const int wb = win_base(m0, d.W, shift), wn = win_rows(d.W, shift);
             const long long nrows = src1 ? rows_x1 : rows_x0;
+            if (tid == 0) hdr[1] = wn;
 #pragma unroll
             for (int t = 0; t < 9; ++t) {
               const int32_t a = tab[t * TC_BM + tid];
@@ -735,7 +775,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
             }
           }
           // cp.async's arrival tracks only its copies; the plain arrive (release) publishes this thread's table (and
-          // flag) stores to the consumers' wait (acquire)
+          // header) stores to the consumers' wait (acquire)
           cp_async_mbar_arrive(wfull + j);
           mbar_arrive(wfull + j);
           ++wi;
@@ -786,6 +826,7 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
   // fragment ownership: consumer warpgroup wg, warp wq of it; rows row_a and row_a + 8 of the tile, columns 8j + 2 t4 + {0, 1}
   const int wg = ctid >> 7, wq = (ctid >> 5) & 3, t4 = lane & 3;
   const int row_a = wg * 64 + wq * 16 + (lane >> 2);
+  const int row_l = wg * 64 + wq * 16 + (lane & 15);       // the row whose address the lane gives ldmatrix
   // rows / bias 8-byte aligned: the epilogue's pair form for the pairs inside cout
   const bool al_ok = (d.ldy % 2 == 0) && ((reinterpret_cast<uintptr_t>(d.y) & 7) == 0) &&
                      ((reinterpret_cast<uintptr_t>(d.bias) & 7) == 0);
@@ -815,29 +856,45 @@ __device__ __forceinline__ void conv_rows_tc_body(const wmd_conv_desc& d, const 
     int pr0 = row_a * TC_A_LD, pr1 = (row_a + 8) * TC_A_LD;   // float offsets of this thread's two fragment rows
     if constexpr (WIN) {
       const int tap = (seg_cb + i) % 9;
-      if (i == 0 || tap == 0 || tap_slots) {
-        wcur = wnext++;
-        mbar_wait(wfull + (wcur & 1), (wcur >> 1) & 1);
-        if constexpr (SET) tap_slots = *reinterpret_cast<const uint32_t*>(wslot + (wcur & 1) * SLOT + SLOT_DATA + TC_WIN_TAB) != 0u;
-      }
+      const bool start = i == 0 || tap == 0 || tap_slots;
+      if (start) wcur = wnext++;
       const int j = static_cast<int>(wcur & 1);
-      sa = reinterpret_cast<const float*>(wslot + j * SLOT);
-      const uint16_t* wt = reinterpret_cast<const uint16_t*>(wslot + j * SLOT + SLOT_DATA) + tap * TC_BM;
+      unsigned char* slot = wslot + j * SLOT;
+      if (start) {
+        mbar_wait(wfull + j, (wcur >> 1) & 1);
+        [[maybe_unused]] const uint32_t* hdr = reinterpret_cast<const uint32_t*>(slot + SLOT_DATA + TC_WIN_TAB);
+        if constexpr (SET) tap_slots = hdr[0] != 0u;
+        if constexpr (F16) {
+          // the slot's rows become fp16 pairs once, for every tap that reads them; both consumer warpgroups walk the
+          // same chunks, so all 256 threads start every slot together
+          split_slot_rows(slot, static_cast<int>(hdr[1]), ascale, ctid);
+          named_bar_sync(kSplitBar, TC_CONSUMERS);
+        }
+      }
+      const uint16_t* wt = reinterpret_cast<const uint16_t*>(slot + SLOT_DATA) + tap * TC_BM;
+      if constexpr (F16) {
+        // Fragment of k-step ks from the split rows: per piece one ldmatrix.x4 over the warp's 16 rows, lane l giving
+        // the address of row l & 15 in channels 16 ks + 8 (l >> 4) .. + 7: h1 at byte 32 g of its group g, h2 at 32 g + 16
+        const uint32_t pa = smem_u32(slot) + wt[row_l] * (TC_A_LD * 4) + (lane >> 4) * 32;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          ldmatrix_x4(fa[b][ks], pa + 64 * ks);
+          ldmatrix_x4(fb[b][ks], pa + 64 * ks + 16);
+        }
+        return;
+      }
+      sa = reinterpret_cast<const float*>(slot);
       pr0 = wt[row_a] * TC_A_LD;
       pr1 = wt[row_a + 8] * TC_A_LD;
     }
     if (F16) {
-      // x * s (s a power of two: exact) = h1 + h2 with h1 = fp16(x s) and h2 = fp16(x s - h1): 22 mantissa bits, the
-      // precision of the tf32 hi / lo pair.  Fragment of k-step ks: rows (r, r + 8) x channels 16 ks + 2 t4 + {0, 1}, + 8
+      // Fragment of k-step ks: rows (r, r + 8) x channels 16 ks + 2 t4 + {0, 1}, + 8, split in registers
 #pragma unroll
       for (int ks = 0; ks < KS; ++ks) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const float2 v = *reinterpret_cast<const float2*>(sa + ((e & 1) ? pr1 : pr0) + ks * 16 + 2 * t4 + (e >> 1) * 8);
-          const float b0f = v.x * ascale, b1f = v.y * ascale;
-          const uint32_t p = pack_f16x2(b0f, b1f);
-          fa[b][ks][e] = p;
-          fb[b][ks][e] = pack_f16x2(b0f - f16_lo_to_f32(p), b1f - f16_hi_to_f32(p));
+          split_f16x2(v.x, v.y, ascale, fa[b][ks][e], fb[b][ks][e]);
         }
       }
     } else {
