@@ -86,6 +86,40 @@ size_t wmd_eval_nyu_errors_ws_bytes(long long n);
 int wmd_eval_nyu_errors_f64(const double* pred, const double* gt, long long n, void* ws, size_t ws_bytes,
                             double* errors, wmd_stream_t stream);
 
+/* ---------------------------------------------------------------- NYUv2 depth boundary error (NYUv2/utils.py:122-169)
+ * compute_depth_boundary_error for n frames of any h x w (h, w >= 1, n h w < 2^31).  pred (n, h, w) is fp32
+ * (pred_f64 = 0) or fp64, which is rounded to fp32 first (the reference's pred.astype('f')).  Per frame:
+ *   1. p = pred with zeros as NaN, p = (p - nanmin p) / fl(nanmax p - nanmin p), both operations in fp32;
+ *   2. scikit-image 0.16.2's canny(p, sigma sqrt(2)) with thresholds `low`, `high`:
+ *      sm = the 13-tap gaussian `taps` (w0 .. w6, scipy's weights) in scipy's order, mode constant 0, along axis 0 and
+ *      then axis 1, each pass accumulated in fp64 as t = x w0, t += (x[-j] + x[+j]) wj for j = 6 .. 1 and stored in
+ *      fp32; smoothed = sm / (bleed + DBL_EPSILON) in fp64, `bleed` (h, w) fp64 the same gaussian of ones (scipy's);
+ *      isobel, jsobel = ndi.sobel(smoothed, 0 / 1) (reflect): d = 0 s + (s[+1] - s[-1]) along the axis, then
+ *      2 d + (d[-1] + d[+1]) along the other; magnitude = glibc's non-FMA hypot kernel; local maxima of the interior
+ *      pixels with magnitude > 0 by skimage's four octants in its order (a later octant's assignment stands), each
+ *      side c2 w + c1 (1 - w) <= m; low / high = local maxima with magnitude >= low / high; edges_est = the
+ *      8-connected components of low that hold a high pixel (union-find: the result is a set, timing-independent);
+ *   3. d_est = the exact Euclidean distance of each pixel to the nearest edges_est pixel (scipy's
+ *      distance_transform_edt(1 - edges_est)), sqrt of the integer squared distance; with no edge pixel at all,
+ *      scipy's sqrt((y + 1)^2 + x^2);
+ *   4. with edges_gt (n, h, w) fp32, d_gt (n, h, w) fp64 its distance map (wmd_eval_edt of edges_gt == 1) and
+ *      gt_sums (n, 2) fp64 = (np.sum(edges_gt), np.nansum(edges_gt)) as numpy's float32 sums: near = edges_est &
+ *      (d_gt < 10);  scores (n, 2) = NaN, NaN if gt_sums[0] == 0;  10, 10 if near is empty;  else
+ *      acc = sum_near d_gt / |near|,  comp = (sum_est min(d_gt, 10) + nansum min(d_est edges_gt, 10)) /
+ *      (|edges_est| + gt_sums[1]), each sum in fp64 over a fixed grid of CTAs and a fixed tree, without atomics.
+ * edges_est (n, h, w) bytes 0 / 1, d_est (n, h, w) fp64.  ws: at least wmd_eval_edges_ws_bytes(n, h, w) bytes (0 for
+ * a bad shape).  Bits do not depend on n or timing. */
+size_t wmd_eval_edges_ws_bytes(int n, int h, int w);
+int wmd_eval_edges_frames(const void* pred, int pred_f64, int n, int h, int w, const double* taps,
+                          const double* bleed, double low, double high, const float* edges_gt, const double* d_gt,
+                          const double* gt_sums, uint8_t* edges_est, double* d_est, double* scores, void* ws,
+                          size_t ws_bytes, wmd_stream_t stream);
+/* the exact Euclidean distance transform of n (h, w) feature masks (bytes, non-zero = feature): dist (n, h, w) fp64
+ * as in step 3 above.  ws: at least wmd_eval_edt_ws_bytes(n, h, w) bytes. */
+size_t wmd_eval_edt_ws_bytes(int n, int h, int w);
+int wmd_eval_edt(const uint8_t* features, int n, int h, int w, double* dist, void* ws, size_t ws_bytes,
+                 wmd_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -153,6 +153,12 @@ EVAL_SIGNATURES = {
                                     c_void_p, c_size_t, c_void_p, c_void_p]),
     "wmd_eval_nyu_errors_ws_bytes": (c_size_t, [c_longlong]),
     "wmd_eval_nyu_errors_f64": (c_int, [c_void_p, c_void_p, c_longlong, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "wmd_eval_edges_ws_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "wmd_eval_edges_frames": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_double, c_double,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                      c_void_p]),
+    "wmd_eval_edt_ws_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "wmd_eval_edt": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 EVAL_EIGEN, EVAL_GT_POSITIVE = 0, 1
 EVAL_NYU_EIGEN, EVAL_NYU_224 = 0, 1                       # WMD_EVAL_NYU_EIGEN, WMD_EVAL_NYU_224
