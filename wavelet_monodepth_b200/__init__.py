@@ -8,6 +8,8 @@ Public surface = the reference's (nianticlabs/wavelet-monodepth) own API for thi
                  SparseDepthWaveProgressiveDecoder                 <- KITTI/networks/decoders/depth_decoder.py
   nyu_decoders   Conv3x3, UpSampleBlock, DecoderWave,
                  SparseDecoderWave                                 <- NYUv2/networks/{layers,decoders/densedepth_decoder}.py
+  nyu_loss       NyuDepthLoss: the NYUv2 training objective,
+                 forward and backward, deterministic               <- NYUv2/train.py:279-327
   shard          batch sharding + the single all-gather (one process per GPU)
   ops / _lib     tensor-level wrappers over the C ABI of libwmd.so (include/wmd.h)
 

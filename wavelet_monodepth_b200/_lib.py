@@ -165,6 +165,21 @@ EVAL_NYU_EIGEN, EVAL_NYU_224 = 0, 1                       # WMD_EVAL_NYU_EIGEN, 
 EVAL_NYU_CROP_H, EVAL_NYU_CROP_W = 440, 592
 DISP_TAIL16_PACKED_FLOATS = 5332          # WMD_DISP_TAIL16_PACKED_FLOATS
 
+
+class LossTerm(Structure):
+    """struct wmd_loss_term (include/wmd_loss.h)."""
+    _fields_ = [("pred", c_void_p), ("h", c_int32), ("w", c_int32), ("log2_factor", c_int32)]
+
+
+# include/wmd_loss.h: the training-loss entry points (tests/test_oracle_nyu_loss.py checks this table against it)
+LOSS_SIGNATURES = {
+    "wmd_loss_nyu_ws_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "wmd_loss_nyu_fwd": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(LossTerm), c_int, c_void_p, c_void_p, c_size_t,
+                                 c_void_p, c_void_p]),
+    "wmd_loss_nyu_bwd": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(LossTerm), c_int, c_void_p, POINTER(c_void_p),
+                                 c_void_p]),
+}
+
 _lib = None
 
 
@@ -191,7 +206,7 @@ def load():
             except OSError:
                 continue
         lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in list(SIGNATURES.items()) + list(EVAL_SIGNATURES.items()):
+    for name, (res, args) in list(SIGNATURES.items()) + list(EVAL_SIGNATURES.items()) + list(LOSS_SIGNATURES.items()):
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
