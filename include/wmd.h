@@ -392,7 +392,8 @@ int wmd_disp_tail16_f32(const float* x, int ld, const float* packed, int cout, f
  *
  * Activation backward: dz[r, o] = dy[r, o] * act'(y[r, o]) from the saved post-activation output y (ELU: y > 0 ? 1 : y + 1;
  * LeakyReLU: y > 0 ? 1 : act_param; sigmoid: y (1 - y); none: 1), for rows r < rows and o < cout.  db (nullable) = sum over
- * rows of dz, summed in a fixed order (per-block partials, then block order), so the bits do not depend on timing.
+ * rows of dz, summed in fp64 in a fixed order (per-block partials, then block order) and rounded to fp32 once, so the bits
+ * do not depend on timing.
  * amax_dz (nullable) is raised to max |dz|: the fp16-pair operand form of the data-gradient launch needs it.  ws (with db):
  * wmd_act_bwd_ws_bytes() bytes whose first 4 KiB are zero before the first use; the kernel leaves them zero.  The same
  * buffer may serve wmd_conv_wgrad_f32 launches on the same stream. */

@@ -1,16 +1,20 @@
 """Launch-checking harness: every libwmd launch a workload makes, checked against the fp64 contract of its kernel.
 
-`Harness(monkeypatch)` wraps the public entry points of wavelet_monodepth_b200.ops.  The decoders, train_native and
-wavelets call `ops.<name>` through the module, and calls inside ops (conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows)
-resolve through the module's globals, so wrapping the module attributes catches every call, nested ones included.
+`Harness(monkeypatch)` wraps the entry points of ENTRY_POINTS, (owner, attribute) pairs whose owner is a module or a
+class: the public functions of wavelet_monodepth_b200.ops, and the evaluation and loss entry points of nyu_loss, nyu_eval
+and kitti_eval.  The decoders, train_native and wavelets call `ops.<name>` through the module, calls inside a module
+(conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows, _NyuLossFn -> _loss_fwd / _loss_bwd, NyuDepthEvaluator.add ->
+_edges_frames) resolve through its globals, and methods through their class, so wrapping the owners' attributes catches
+every call, nested ones included.
 
 Each call runs the original function, synchronises (compactions and list gathers run on side streams), recomputes the
 result from the call's actual inputs with the references of the kernel contract tests (conv_ref, head_ref, disp_tail_ref,
-conv_grad_ref, oracle.haar, plain torch restatements of the wmd.h comments: none of them uses ops or libwmd) and compares
-at that kernel's bar.  It also checks the preconditions a launch's contract relies on: source maxima that cover what an
-fp16-pair launch reads, exact amax outputs, index maps inside their sources, strictly increasing pixel lists, and
-count <= max_rows.  Pack calls record the plain weights behind each packed object; a pack is right when every launch
-that uses it is right.
+conv_grad_ref, oracle.haar, oracle.nyu_loss, oracle.nyu_eval, oracle.nyu_edges, oracle.kitti_eval, plain torch
+restatements of the wmd.h comments: none of them uses ops or libwmd) and compares at that kernel's bar.  It also checks
+the preconditions a launch's contract relies on: source maxima that cover what an fp16-pair launch reads, exact amax
+outputs, index maps inside their sources, strictly increasing pixel lists, and count <= max_rows.  Pack calls record the
+plain weights behind each packed object; a pack is right when every launch that uses it is right.  State a checker needs
+from before the call (an evaluator's next frame and the rows the call writes) comes from the entry's `_before_` hook.
 
 Completeness: around each outermost wrapped call the harness takes the `launch_count()` delta; at the end of a workload the
 checked deltas must add up to the whole delta, and any libwmd symbol called outside a wrapped call is named.
@@ -19,11 +23,16 @@ import contextlib
 import inspect
 import threading
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 from oracle import haar as ohaar
-from wavelet_monodepth_b200 import _lib, ops
+from oracle import kitti_eval as oke
+from oracle import nyu_edges as ne
+from oracle import nyu_eval as one
+from oracle import nyu_loss as onl
+from wavelet_monodepth_b200 import _lib, kitti_eval, nyu_eval, nyu_loss, ops
 
 import conv_grad_ref
 import conv_ref as cr
@@ -38,8 +47,31 @@ CHECKED = ("conv_rows", "head_mlp", "head_gather", "head_conv3x3", "head_idwt", 
            "disp_tail16", "range_thresh", "level_masks", "compact", "gate_map", "nchw_to_rows", "gather_rows",
            "gather_rows_list", "rows_to_nchw", "scatter_rows", "amax_rows", "act_backward", "conv_wgrad", "conv_dgrad")
 PACKS = ("pack_weight", "pack_head_weight", "pack_head_mlp", "pack_disp_tail16")
+# the evaluation and loss entry points that launch kernels, (owner, attribute)
+EVAL_LOSS = ((nyu_loss, "_loss_fwd"), (nyu_loss, "_loss_bwd"),
+             (nyu_eval, "compute_errors_nyu"), (nyu_eval, "_edt"), (nyu_eval, "_edges_frames"),
+             (nyu_eval.NyuDepthEvaluator, "add"),
+             (kitti_eval, "compute_errors"), (kitti_eval, "batch_post_process_disparity"),
+             (kitti_eval.KittiDepthEvaluator, "__init__"), (kitti_eval.KittiDepthEvaluator, "add"))
+ENTRY_POINTS = tuple((ops, name) for name in CHECKED) + EVAL_LOSS
 
-# every symbol of _lib.SIGNATURES: ("launch", ops entry point whose checker covers it) | ("pack", ops entry point) | "query"
+
+def entry_name(owner, attr):
+    """'conv_rows', '_loss_fwd', 'NyuDepthEvaluator.add', 'KittiDepthEvaluator.__init__'"""
+    return attr if inspect.ismodule(owner) else "%s.%s" % (owner.__name__, attr)
+
+
+ENTRIES = tuple(entry_name(o, a) for o, a in ENTRY_POINTS)
+
+
+def hook(prefix, entry):
+    """The Harness method of an entry point: hook("_check_", "KittiDepthEvaluator.__init__") is
+    "_check_KittiDepthEvaluator_init", hook("_before_", "_loss_fwd") "_before_loss_fwd"."""
+    return prefix + entry.replace(".__init__", ".init").strip("_").replace(".", "_")
+
+
+# every symbol of _lib.SIGNATURES, EVAL_SIGNATURES and LOSS_SIGNATURES: ("launch", entry point whose checker covers it) |
+# ("pack", ops entry point) | "query"
 SYMBOLS = {
     "wmd_version": "query", "wmd_status_string": "query", "wmd_last_cuda_error": "query", "wmd_launch_count": "query",
     "wmd_idwt_haar_f32": ("launch", "idwt_haar"),
@@ -90,11 +122,35 @@ SYMBOLS = {
     "wmd_conv_wgrad_ws_bytes": "query",
     "wmd_conv_wgrad_f32": ("launch", "conv_wgrad"),
     "wmd_conv_dgrad_fold_f32": ("launch", "conv_dgrad"),
+    # include/wmd_eval.h
+    "wmd_eval_gt_mask": ("launch", "KittiDepthEvaluator.__init__"),
+    "wmd_eval_gather_f32": ("launch", "KittiDepthEvaluator.__init__"),
+    "wmd_eval_frames": ("launch", "KittiDepthEvaluator.add"),
+    "wmd_eval_errors_f64": ("launch", "compute_errors"),
+    "wmd_post_process_disparity": ("launch", "batch_post_process_disparity"),
+    "wmd_eval_nyu_ws_bytes": "query",
+    "wmd_eval_nyu_frames": ("launch", "NyuDepthEvaluator.add"),
+    "wmd_eval_nyu_errors_ws_bytes": "query",
+    "wmd_eval_nyu_errors_f64": ("launch", "compute_errors_nyu"),
+    "wmd_eval_edges_ws_bytes": "query",
+    "wmd_eval_edges_frames": ("launch", "_edges_frames"),
+    "wmd_eval_edt_ws_bytes": "query",
+    "wmd_eval_edt": ("launch", "_edt"),
+    # include/wmd_loss.h
+    "wmd_loss_nyu_ws_bytes": "query",
+    "wmd_loss_nyu_fwd": ("launch", "_loss_fwd"),
+    "wmd_loss_nyu_bwd": ("launch", "_loss_bwd"),
 }
 
 # bars of the checks this file adds on top of the contract tests' (units of 2^-24 of the element's scale)
 DWT_ULP = 8            # four roundings on each path of a one-level analysis bound the error by 4 x 2^-24 S; twice that
 ACT_BWD_ULP = 4        # dz = dy act'(y): at most three roundings (sigmoid: 1 - y, y (1 - y), the product with dy)
+# bars of the evaluation and loss checks: those of their own tests (test_gpu_nyu_loss, test_gpu_nyu_eval,
+# test_gpu_nyu_edges, test_gpu_kitti_eval)
+LOSS_MEAN_ULP = 1      # a loss term: the device's fp64 sum and the oracle's differ in order only, one fp32 rounding apart
+EVAL_REL = 1e-12       # fp64 sums of a fixed order against math.fsum / numpy's pairwise sums
+NYU_SUM_ABS = 1e-15    # per pixel: the fp64 log10's ulp, all a log_10 sum of equal depths is made of
+POST_REL = 1e-15       # batch_post_process_disparity: numpy's expression, evaluated in the same precision
 
 REPORT = {}            # (entry, engine, mode) -> [worst err, bar, launches, largest row count]
 
@@ -110,7 +166,7 @@ def report_lines():
     lines = ["worst err per (entry point, engine / precision, mode): worst (bar, launches, most rows)"]
     for k in sorted(REPORT):
         worst, bar, count, rows = REPORT[k]
-        lines.append("  %-16s %-8s %-18s %.2e  (bar %s, %d launches, %d rows)"
+        lines.append("  %-28s %-8s %-18s %.2e  (bar %s, %d launches, %d rows)"
                      % (k + (worst, "exact" if bar == 0 else "%.2g" % bar, count, rows)))
     return lines
 
@@ -176,15 +232,16 @@ class Harness:
         self.calls = {}
         lib = _lib.load()
         monkeypatch.setattr(_lib, "_lib", _LibSpy(lib, self))
-        for name in CHECKED:
-            monkeypatch.setattr(ops, name, self._wrap(name, getattr(ops, name), getattr(self, "_check_" + name)))
+        for owner, attr in ENTRY_POINTS:
+            name = entry_name(owner, attr)
+            monkeypatch.setattr(owner, attr, self._wrap(name, getattr(owner, attr), getattr(self, hook("_check_", name))))
         for name in PACKS:
             monkeypatch.setattr(ops, name, self._wrap(name, getattr(ops, name), getattr(self, "_pack_" + name)))
 
     # ------------------------------------------------------------------------------------------ plumbing
     def _wrap(self, name, orig, check):
         sig = inspect.signature(orig)
-        before = getattr(self, "_before_" + name, None)
+        before = getattr(self, hook("_before_", name), None)
 
         def wrapped(*args, **kwargs):
             a = sig.bind(*args, **kwargs)
@@ -703,3 +760,217 @@ class Harness:
             _record("conv_dgrad", "dx1", "taps%d" % taps, err1, conv_grad_ref.BARS["dx1"], n * h * w)
             _require(err1 <= conv_grad_ref.BARS["dx1"], "%s: conv_dgrad dx1 err/S %.3g > %.3g"
                      % (self.current, err1, conv_grad_ref.BARS["dx1"]))
+
+    # ------------------------------------------------------------------------------------------ NYUv2 training loss
+    def _check_loss_fwd(self, a, signs, pre):
+        """means[k] within LOSS_MEAN_ULP fp32 ulp of oracle.nyu_loss.term, NaN where it is NaN; int8 signs equal"""
+        target = _np(a["target"])[:, 0]
+        n, H, W = target.shape
+        means = _np(a["means"])
+        worst = 0.0
+        for k, (p, lg) in enumerate(zip(a["preds"], a["log2s"])):
+            pk = _np(p)[:, 0]
+            _require(pk.shape[1] << lg == H and pk.shape[2] << lg == W, "_loss_fwd: term %d is not the target / 2^%d"
+                     % (k, lg))
+            want = onl.term(pk, target)
+            _require(np.isnan(means[k]) == np.isnan(want), "_loss_fwd: term %d is %r, want %r" % (k, means[k], want))
+            if not np.isnan(want):
+                worst = max(worst, _ulps(means[k], want))
+            if signs is not None:
+                ws = onl.signs(onl.upsample(pk, H, W), target)
+                bad = int((_np(signs[k]) != ws).sum())
+                _require(bad == 0, "%s: _loss_fwd term %d (%dx%d, factor 2^%d): %d signs differ"
+                         % (self.current, k, pk.shape[1], pk.shape[2], lg, bad))
+        _record("_loss_fwd", "fp64", "ulp" + ("+signs" if signs is not None else ""), worst, LOSS_MEAN_ULP,
+                n * H * W * len(a["preds"]))
+        _require(worst <= LOSS_MEAN_ULP, "%s: _loss_fwd %.3g fp32 ulp > %d" % (self.current, worst, LOSS_MEAN_ULP))
+
+    def _check_loss_bwd(self, a, grads, pre):
+        """grads[k] = fp32((g_k / (N H W)) S) of oracle.nyu_loss.adjoint on the call's own signs, bit for bit"""
+        n, _, H, W = a["target_shape"]
+        sg = _np(a["signs"])
+        g = _np(a["grad_means"]).astype(np.float32)
+        worst = 0.0
+        for k, p in enumerate(a["preds"]):
+            h, w = int(p.shape[2]), int(p.shape[3])
+            coef = np.float64(g[k]) / np.float64(n * H * W)
+            want = (coef * onl.adjoint(sg[k], h, w)).astype(np.float32)
+            got = _np(grads[k])[:, 0]
+            if not np.array_equal(got, want, equal_nan=True):
+                bad = ~((got == want) | (np.isnan(got) & np.isnan(want)))
+                worst = max(worst, float(np.nan_to_num(_ulps(got[bad], want[bad]), nan=np.inf).max()))
+                _require(False, "%s: _loss_bwd term %d (%dx%d from %dx%d): %d gradients differ, worst %.3g ulp"
+                         % (self.current, k, h, w, H, W, int(bad.sum()), worst))
+        _record("_loss_bwd", "fp64", "bits", worst, 0, n * H * W * len(a["preds"]))
+
+    # ------------------------------------------------------------------------------------------ NYUv2 evaluation
+    def _before_NyuDepthEvaluator_add(self, a):
+        ev = a["self"]
+        return ev.next_frame, ev.sums.clone()
+
+    def _check_NyuDepthEvaluator_add(self, a, res, pre):
+        """oracle.nyu_eval.predict and frame_sums fed the evaluator's own gt / gt_log10: the map bit for bit, NaN pattern
+        included; counts exact; the three sums within EVAL_REL relative plus NYU_SUM_ABS per pixel; other rows kept"""
+        ev = a["self"]
+        f0, old = pre
+        disp = a["disp"]
+        d = disp[:, 0] if disp.dim() == 4 and disp.shape[1] == 1 else disp
+        n = int(d.shape[0])
+        if n == 0:
+            return
+        _require(ev.next_frame == f0 + n, "NyuDepthEvaluator.add: next_frame %d, want %d" % (ev.next_frame, f0 + n))
+        want_map = one.predict(_np(d), ev.use_224, ev.use_disparity)
+        if a["depth_out"] is not None:
+            dm = _np(a["depth_out"])
+            _require(np.array_equal(dm, want_map, equal_nan=True),
+                     "%s: NyuDepthEvaluator.add: %d prediction-map values differ from oracle.nyu_eval.predict"
+                     % (self.current, int((~((dm == want_map) | (np.isnan(dm) & np.isnan(want_map)))).sum())))
+        want = one.frame_sums(want_map, _np(ev.gt[f0:f0 + n]), _np(ev.gt_log10[f0:f0 + n]))
+        got = _np(ev.sums[f0:f0 + n])
+        _require(np.array_equal(got[:, 3:], want[:, 3:]), "%s: NyuDepthEvaluator.add: a_k / pixel counts %s, want %s"
+                 % (self.current, got[:, 3:].tolist(), want[:, 3:].tolist()))
+        err = _rel_err(got[:, :3], want[:, :3], "NyuDepthEvaluator.add sums", NYU_SUM_ABS * want[:, 6:7])
+        rest = old.clone()
+        rest[f0:f0 + n] = ev.sums[f0:f0 + n]
+        _require(torch.equal(_bits(rest), _bits(ev.sums)), "NyuDepthEvaluator.add wrote rows outside its frames")
+        mode = ("224" if ev.use_224 else "eigen") + ("/disparity" if ev.use_disparity else "")
+        _record("NyuDepthEvaluator.add", "fp64", mode, err, EVAL_REL, n * want_map[0].size)
+        _require(err <= EVAL_REL, "%s: NyuDepthEvaluator.add sums err %.3g > %.3g" % (self.current, err, EVAL_REL))
+
+    def _check_compute_errors_nyu(self, a, out, pre):
+        want = one.compute_errors_nyu(_np(a["pred"]), _np(a["gt"]))
+        err = _rel_err(_np(out), want, "compute_errors_nyu")
+        _record("compute_errors_nyu", "fp64", "-", err, EVAL_REL, a["pred"].numel())
+        _require(err <= EVAL_REL, "%s: compute_errors_nyu err %.3g > %.3g" % (self.current, err, EVAL_REL))
+
+    def _check_edt(self, a, out, pre):
+        """each frame's distance map equals scipy's distance_transform_edt bit for bit"""
+        f = _np(a["features"]) != 0
+        got = _np(out)
+        for i in range(f.shape[0]):
+            _require(np.array_equal(got[i].view(np.int64), ne.edt(f[i]).view(np.int64)),
+                     "%s: _edt frame %d (%dx%d) differs from scipy's distance transform" % (self.current, i, *f.shape[1:]))
+        _record("_edt", "fp64", "-", 0.0, 0, f.size)
+
+    def _check_edges_frames(self, a, res, pre):
+        """oracle.nyu_edges.dbe per frame on the prediction rounded to fp32: edges and distance map bit for bit, scores
+        within EVAL_REL relative, NaN and 10 exact"""
+        edges_est, d_est = _np(res[0]), _np(res[1])
+        p = _np(a["pred"]).astype(np.float32)
+        g, scores = _np(a["edges_gt"]), _np(a["scores"])
+        worst = 0.0
+        for i in range(p.shape[0]):
+            acc, comp, e, d = ne.dbe(g[i], p[i], a["low"], a["high"])
+            _require(np.array_equal(edges_est[i] != 0, e), "%s: _edges_frames frame %d: %d edge pixels differ"
+                     % (self.current, i, int(((edges_est[i] != 0) != e).sum())))
+            _require(np.array_equal(d_est[i].view(np.int64), d.view(np.int64)),
+                     "%s: _edges_frames frame %d: the distance map differs from scipy's" % (self.current, i))
+            want = np.array([acc, comp])
+            ten = want == ne.MAX_DIST
+            _require(np.array_equal(scores[i][ten], want[ten]), "_edges_frames frame %d: score not exactly 10" % i)
+            worst = max(worst, _rel_err(scores[i], want, "_edges_frames frame %d scores" % i))
+        _record("_edges_frames", "fp64", "-", worst, EVAL_REL, p.size)
+        _require(worst <= EVAL_REL, "%s: _edges_frames scores err %.3g > %.3g" % (self.current, worst, EVAL_REL))
+
+    # ------------------------------------------------------------------------------------------ KITTI evaluation
+    def _check_KittiDepthEvaluator_init(self, a, res, pre):
+        """oracle.kitti_eval.valid_mask of each frame: frame sizes, offsets, the pixel list and the gathered ground
+        truth exact"""
+        ev = a["self"]
+        frames = [(g.detach().cpu().numpy() if torch.is_tensor(g) else np.asarray(g)).astype(np.float32)
+                  for g in a["gt_depths"]]
+        hm, wm = ev.h_max, ev.w_max
+        pixels, values, counts = [], [], [0]
+        for i, g in enumerate(frames):
+            ys, xs = np.nonzero(oke.valid_mask(g, a["eval_split"]))
+            pixels.append(i * hm * wm + ys * wm + xs)
+            values.append(g[ys, xs])
+            counts.append(ys.size)
+        off = np.cumsum(counts)
+        total = int(off[-1])
+        _require(np.array_equal(_np(ev.hw), np.array([g.shape for g in frames])), "KittiDepthEvaluator: frame sizes")
+        _require(np.array_equal(_np(ev.offsets), off), "%s: KittiDepthEvaluator: valid counts %s, want %s"
+                 % (self.current, np.diff(_np(ev.offsets)).tolist(), counts[1:]))
+        _require(np.array_equal(_np(ev.pixels[:total]), np.concatenate(pixels)), "KittiDepthEvaluator: pixel list")
+        _require(np.array_equal(_np(ev.gt[:total]), np.concatenate(values)), "KittiDepthEvaluator: gathered gt")
+        _record("KittiDepthEvaluator.__init__", "-", a["eval_split"], 0.0, 0, total)
+
+    def _before_KittiDepthEvaluator_add(self, a):
+        ev = a["self"]
+        return ev.next_frame, [t.clone() for t in (ev.errors, ev.ratios, ev.counts)]
+
+    def _check_KittiDepthEvaluator_add(self, a, res, pre):
+        """oracle.kitti_eval.evaluate_frame on each frame's ground truth (rebuilt from the split's checked valid pixels):
+        counts, a1..a3 and the median ratio exact, the other metrics within EVAL_REL relative; other rows kept"""
+        ev = a["self"]
+        f0, old = pre
+        d = a["pred_disp"]
+        d = _np(d[:, 0] if d.dim() == 4 and d.shape[1] == 1 else d)
+        n = d.shape[0]
+        _require(ev.next_frame == f0 + n, "KittiDepthEvaluator.add: next_frame %d, want %d" % (ev.next_frame, f0 + n))
+        hw, off, pix, gtv = _np(ev.hw), _np(ev.offsets), _np(ev.pixels), _np(ev.gt)
+        errors, ratios, counts = _np(ev.errors), _np(ev.ratios), _np(ev.counts)
+        split = ev.eval_split
+        worst = 0.0
+        for i in range(n):
+            f = f0 + i
+            g = np.zeros(tuple(hw[f]), np.float32)
+            p = pix[off[f]:off[f + 1]].astype(np.int64) - f * ev.h_max * ev.w_max
+            g[p // ev.w_max, p % ev.w_max] = gtv[off[f]:off[f + 1]]
+            we, wr, wc = oke.evaluate_frame(g, d[i], split, ev.median_scaling, ev.pred_depth_scale_factor)
+            _require(int(counts[f]) == wc, "%s: KittiDepthEvaluator.add frame %d: count %d, want %d"
+                     % (self.current, f, counts[f], wc))
+            _require(np.array_equal(errors[f, 4:], we[4:], equal_nan=True), "%s: KittiDepthEvaluator.add frame %d: "
+                     "a1..a3 %s, want %s" % (self.current, f, errors[f, 4:].tolist(), we[4:].tolist()))
+            _require(ratios[f] == wr or (np.isnan(ratios[f]) and np.isnan(wr)),
+                     "%s: KittiDepthEvaluator.add frame %d: ratio %r, want %r" % (self.current, f, ratios[f], wr))
+            worst = max(worst, _rel_err(errors[f, :4], we[:4], "KittiDepthEvaluator.add frame %d" % f))
+        for t, o in zip((ev.errors, ev.ratios, ev.counts), old):
+            rest = o.clone()
+            rest[f0:f0 + n] = t[f0:f0 + n]
+            _require(torch.equal(_bits(rest), _bits(t)), "KittiDepthEvaluator.add wrote rows outside its frames")
+        mode = "%s/%s" % (split, "median" if ev.median_scaling else "x%g" % ev.pred_depth_scale_factor)
+        _record("KittiDepthEvaluator.add", "fp64", mode, worst, EVAL_REL, int(off[f0 + n] - off[f0]))
+        _require(worst <= EVAL_REL, "%s: KittiDepthEvaluator.add err %.3g > %.3g" % (self.current, worst, EVAL_REL))
+
+    def _check_batch_post_process_disparity(self, a, out, pre):
+        """the reference's numpy expression on the call's inputs, in their precision"""
+        want = oke.batch_post_process_disparity(_np(a["l_disp"]), _np(a["r_disp"]))
+        err = _rel_err(_np(out), want, "batch_post_process_disparity")
+        _record("batch_post_process_disparity", "fp64", str(a["l_disp"].dtype).split(".")[-1], err, POST_REL, out.numel())
+        _require(err <= POST_REL, "%s: batch_post_process_disparity err %.3g > %.3g" % (self.current, err, POST_REL))
+
+    def _check_compute_errors(self, a, out, pre):
+        want = np.array(oke.compute_errors(_np(a["gt"]).astype(np.float64), _np(a["pred"]).astype(np.float64)))
+        err = _rel_err(_np(out), want, "compute_errors")
+        _record("compute_errors", "fp64", "-", err, EVAL_REL, a["gt"].numel())
+        _require(err <= EVAL_REL, "%s: compute_errors err %.3g > %.3g" % (self.current, err, EVAL_REL))
+
+
+def _np(t):
+    return t.detach().cpu().numpy()
+
+
+def _bits(t):
+    t = t.detach().cpu().contiguous()
+    return t.view(torch.int64) if t.dtype == torch.float64 else t
+
+
+def _ulps(got, want):
+    """|got - want| in units of the fp32 spacing at want"""
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    return np.abs(got - want) / np.spacing(np.abs(want).astype(np.float32)).astype(np.float64)
+
+
+def _rel_err(got, want, what, allow=0.0):
+    """max over the elements of (|got - want| - allow) / |want|, after requiring the same NaN pattern and +-Inf exact"""
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    _require(np.array_equal(np.isnan(got), np.isnan(want)), "%s: NaN pattern %s, want %s" % (what, got, want))
+    inf = np.isinf(want)
+    _require(np.array_equal(got[inf], want[inf]), "%s: %s, want %s" % (what, got, want))
+    f = np.isfinite(want)
+    if not f.any():
+        return 0.0
+    allow = np.broadcast_to(np.asarray(allow, np.float64), want.shape)
+    e = (np.abs(got[f] - want[f]) - allow[f]).clip(min=0) / np.maximum(np.abs(want[f]), 1e-300)
+    return float(e.max())

@@ -9,7 +9,7 @@ Measured worst err / S over all cases, mixed- and same-sign, on one H100 80GB HB
     dW  (wgrad, 3xTF32 mma.sync, 32-pixel epochs)   9.5e-7
     dx0 (forward engine f16x3 + fold)               8.5e-6
     dx1 (skip columns of the fold)                  3.9e-6
-    db  (fixed-order column sums)                   1.2e-6
+    db  (fixed-order fp64 column sums)              1.2e-6 (measured with the earlier fp32 sums)
 Each quantity's bar (BARS) is 2.3-2.6x its worst.
 
 The whole decoders' parameter and input-feature gradients (allow_tf32 False) are compared with an fp64 CPU run of the
@@ -64,6 +64,9 @@ CASES = [
     ("long_reduction", 64, 0, 64, 4, 96, 100, 9, "reflect", "elu", 0),
     ("kitti_r50_level1_upconv1", 32, 64, 32, 8, 160, 512, 9, "reflect", "elu", 1),
     ("nyu_conv2", 2208, 0, 1104, 8, 15, 20, 9, "replicate", "none", 0),
+    # NYU Decoder's up3 convA at 640x480 x8: a whole-tile reduction of 1200 32-pixel chunks, whose fp32 chunk sums
+    # drifted past the dW bar in the launch check of the Decoder's training step
+    ("nyu_decoder_up3_conva", 552, 192, 276, 8, 60, 80, 9, "zero", "lrelu", 1),
 ]
 
 
@@ -126,6 +129,24 @@ def test_layer_gradients_vs_fp64(case, same_sign):
     if x1 is not None:
         want, s = ref["x1"]
         _check("dx1", x1d.grad, want.reshape(n, h, w, c1).permute(0, 3, 1, 2), s.reshape(n, h, w, c1).permute(0, 3, 1, 2), BARS["dx1"])
+
+
+@pytest.mark.parametrize("rows,cout,spread", [(8 * 240 * 320, 1, 0.0), (8 * 240 * 320, 3, 1.0), (1000, 1, 1.0),
+                                              (64 * 1024 + 7, 40, 1.0)])
+def test_bias_gradient_of_many_same_sign_rows(rows, cout, spread):
+    """db over the rows of NYU's Decoder's last convolution (cout 1, 8 frames of 240 x 320) under a mean loss, where
+    every dz is the same 1 / rows, and over same-sign rows of several sizes.  Summed in fp32 (a per-thread chain, then
+    up to 1024 block partials in block order) db drifted by 1.0e-5 of the sum, 3.4x BARS['db'] (the launch check of
+    the Decoder's training step found it); summed in fp64 and rounded once it is within one fp32 rounding of the sum."""
+    g = torch.Generator(device="cpu").manual_seed(rows + cout)
+    y = torch.randn((rows, cout), generator=g).to(DEV)
+    dy = ((1.0 + spread * torch.rand((rows, cout), generator=g)) / rows).to(DEV)
+    dz, db = ops.act_backward(y, dy, cout, _lib.ACT_NONE)
+    assert torch.equal(dz[:, :cout], dy)
+    want = dy.double().sum(0)
+    err = float(((db.double() - want).abs() / want).max())
+    assert err <= 2.0 ** -23, (rows, cout, err)
+    assert err <= BARS["db"]
 
 
 # ------------------------------------------------------------------------------------------ whole decoders

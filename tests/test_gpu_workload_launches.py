@@ -1,0 +1,229 @@
+"""GPU: every libwmd launch of the decoders, training steps, evaluations and losses the package ships beyond the
+benchmarked decoders, against the fp64 contract of its kernel (tests/launch_check.py).
+
+tests/test_gpu_production_launches.py checks the benchmarked decoders; this file checks the rest at production batch and
+image sizes, where the size-dependent parts of their kernels are: the 224-pixel wavelet decoder (its MobileNetV2-light
+pyramid's fine levels take the FMA engine) and the 224-pixel baseline decoder; native training of those two, of NYU's
+baseline Decoder, of DecoderWave with NyuDepthLoss (the loss's CTA partials and its backward's footprint gather) and of
+the KITTI R50 1024x320 wave decoder; the KITTI dense decoder without skips; the sparse NYU decoder at its threshold
+extremes; NYU evaluation with depth boundary errors on 440x592 frames (fixed CTA grids, union-find hysteresis, the
+exact distance transform) and in 224 mode; KITTI evaluation of post-processed disparities, whose medians are taken by
+radix select over full LiDAR frames.  Inputs are synthetic (synth, oracle.nyu_edges.edge_split,
+oracle.kitti_eval.synthetic_split).  The entry points are called through their modules, as the package's users do: a
+name imported from a module would bypass the harness's wrapper, and the completeness check would name its symbol.
+
+Each workload runs once plainly and once under the harness, which checks each launch at its kernel's bar and that every
+kernel launched ran inside a checked call; the two runs must agree bit for bit.  Each prints its per-entry-point call
+counts and wall times; the module prints the worst error of every (entry point, engine, mode) at the end.
+"""
+import gc
+import time
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import kitti_eval as oke
+from oracle import nyu_edges as ne
+from wavelet_monodepth_b200 import kitti_decoders as kd, kitti_eval, nyu_decoders as nd, nyu_eval, synth
+from wavelet_monodepth_b200.nyu_loss import NyuDepthLoss
+
+import launch_check as lc
+import test_gpu_production_launches as prod
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda"
+MNV2_LIGHT_CH = (32, 24, 32, 64, 160)
+D161, R18, R50 = prod.D161, prod.R18, prod.R50
+D161_224 = (synth.DENSENET161_CH, 224, 224)
+MNV2_224 = (MNV2_LIGHT_CH, 224, 224)
+EVAL_FRAMES = 16
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report():
+    yield
+    if lc.REPORT:
+        print("\n" + "\n".join(lc.report_lines()))
+
+
+@pytest.fixture(autouse=True)
+def _fp32_convs():
+    prev = torch.backends.cudnn.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False
+    yield
+    torch.backends.cudnn.allow_tf32 = prev
+
+
+def _raw(t):
+    """a float tensor's bits (NaN rows compare equal), any other tensor as it is"""
+    if t.is_floating_point():
+        return t.view({8: torch.int64, 4: torch.int32, 2: torch.int16}[t.element_size()])
+    return t
+
+
+def _feats(shapes, seed, grad=False):
+    return [f.to(DEV).requires_grad_(grad) for f in synth.blocky_features(shapes, seed=seed)]
+
+
+def _nyu_module(cls, ch):
+    dec = cls(enc_features=list(ch), decoder_width=0.5)
+    synth.load_random(dec, seed=11)
+    return dec.to(DEV)
+
+
+# ------------------------------------------------------------------------------------------ inference
+def nyu224(cls, n, spec):
+    def run():
+        ch, h, w = spec
+        dec = _nyu_module(cls, ch).eval()
+        with torch.no_grad():
+            return dec(_feats(synth.nyu_feature_shapes(n, h, w, ch), seed=3))
+    return run
+
+
+def kitti_no_skips(n, spec):
+    def run():
+        ch, h, w = spec
+        dec = kd.DepthWaveProgressiveDecoder(np.array(ch), use_skips=False)
+        synth.bench_kitti_params(dec)
+        with torch.no_grad():
+            return dec.to(DEV).eval()(prod._kitti_feats(n, *spec))
+    return run
+
+
+# ------------------------------------------------------------------------------------------ training
+def train(make, n, spec, shapes, loss=None):
+    """One native training step with fp32 convolutions: outputs, parameter and input-feature gradients.  With `loss`
+    (a NyuDepthLoss) the objective is that loss against a target within 30 % of the decoder's own ("disp", 0) (so the
+    signs of the differences vary); otherwise the sum of the ("disp", s) means."""
+    def run():
+        ch, h, w = spec
+        mod = make(ch)
+        synth.load_random(mod, seed=1)
+        mod = mod.to(DEV).train()
+        feats = _feats(shapes(n, h, w, ch), seed=2, grad=True)
+        out = mod(feats)
+        res = {("out",) + tuple(k): v.detach() for k, v in out.items()}
+        if loss is None:
+            total = sum(v.mean() for k, v in out.items() if k[0] == "disp")
+        else:
+            d0 = out[("disp", 0)].detach()
+            gen = torch.Generator(device="cpu").manual_seed(5)
+            target = (d0.abs() + 0.05) * (0.7 + 0.6 * torch.rand(d0.shape, generator=gen)).to(DEV)
+            total, losses = loss(out, target)
+            res.update({("loss", k): v.detach() for k, v in losses.items()})
+        total.backward()
+        res.update({("grad", k): p.grad for k, p in mod.named_parameters() if p.grad is not None})
+        res.update({("feature_grad", j): f.grad for j, f in enumerate(feats) if f.grad is not None})
+        return res
+    return run
+
+
+def _nyu(cls):
+    return lambda ch: cls(enc_features=list(ch), decoder_width=0.5)
+
+
+# ------------------------------------------------------------------------------------------ evaluation
+def _to_depth_range(disp, lo, hi):
+    """the decoder's disparities mapped affinely onto [lo, hi] (its structure, at the scale a split's depths have)"""
+    d = disp.detach()
+    return lo + (hi - lo) * (d - d.amin()) / (d.amax() - d.amin())
+
+
+def nyu_eval_edges(n, spec, batch=8):
+    """SparseDecoderWave outputs, mapped onto 1..5 m, into NyuDepthEvaluator with edges_gt (Eigen mode) in batches of
+    `batch`; then compute_errors_nyu over the whole split's prediction maps."""
+    def run():
+        ch, h, w = spec
+        split = ne.edge_split(5, n=n)
+        dec = _nyu_module(nd.SparseDecoderWave, ch).eval()
+        ev = nyu_eval.NyuDepthEvaluator(split["gt"], edges_gt=split["edges"])
+        depth = torch.empty((n,) + ev.out_shape, dtype=torch.float64, device=DEV)
+        for b in range(0, n, batch):
+            with torch.no_grad():
+                disp = dec(_feats(synth.nyu_feature_shapes(batch, h, w, ch), seed=40 + b), 0.1)[("disp", 0)]
+            ev.add(100.0 * _to_depth_range(disp, 1.0, 5.0), depth_out=depth[b:b + batch])
+        errors = nyu_eval.compute_errors_nyu(depth, ev.gt)
+        return {"sums": ev.sums, "edges_scores": ev.edges_scores, "depth": depth, "errors": errors}
+    return run
+
+
+def nyu_eval_224(n, spec):
+    def run():
+        ch, h, w = spec
+        gt = ne.edge_split(6, n=n)["gt"]
+        dec = _nyu_module(nd.DecoderWave224, ch).eval()
+        with torch.no_grad():
+            disp = dec(_feats(synth.nyu_feature_shapes(n, h, w, ch), seed=50))[("disp", 0)]
+        ev = nyu_eval.NyuDepthEvaluator(gt, use_224=True)
+        depth = torch.empty((n,) + ev.out_shape, dtype=torch.float64, device=DEV)
+        ev.add(100.0 * _to_depth_range(disp, 1.0, 5.0), depth_out=depth)
+        return {"sums": ev.sums, "depth": depth}
+    return run
+
+
+def kitti_eval_pp(n, spec):
+    """Sparse R18 decoder on the frames and their flips, disp_to_depth's scaled disparity (min 0.1, max 100 m),
+    batch_post_process_disparity, KittiDepthEvaluator with median scaling on a synthetic split at KITTI's ground-truth
+    sizes (its empty, one-valid, even-count and all-equal frames included); then compute_errors over the split's valid
+    ground truth and the depths the evaluator sampled there."""
+    def run():
+        ch, h, w = spec
+        split = oke.synthetic_split(7, n_regular=n - len(oke.SPECIAL))
+        dec = kd.SparseDepthWaveProgressiveDecoder(np.array(ch))
+        synth.bench_kitti_params(dec)
+        dec = dec.to(DEV).eval()
+        feats = prod._kitti_feats(n, *spec)
+        with torch.no_grad():
+            left = dec(feats, 0.05)[("disp", 0)][:, 0]
+            right = dec([torch.flip(f, [3]) for f in feats], 0.05)[("disp", 0)][:, 0]
+        lo, hi = 1 / 100.0, 1 / 0.1
+        pp = kitti_eval.batch_post_process_disparity(lo + (hi - lo) * left, torch.flip(lo + (hi - lo) * right, [2]))
+        ev = kitti_eval.KittiDepthEvaluator(split["gt"])
+        ev.add(pp)
+        total = int(ev.offsets[-1])
+        errors = kitti_eval.compute_errors(ev.gt[:total], ev.depth[:total])
+        return {"pp": pp, "errors": ev.errors, "ratios": ev.ratios, "counts": ev.counts, "pooled": errors}
+    return run
+
+
+WORKLOADS = {
+    "wave224_d161_x8": nyu224(nd.DecoderWave224, 8, D161_224),
+    "wave224_mnv2light_x8": nyu224(nd.DecoderWave224, 8, MNV2_224),
+    "baseline_decoder224_d161_x8": nyu224(nd.Decoder224, 8, D161_224),
+    "train_wave224_mnv2light_x8_nyuloss_ll": train(_nyu(nd.DecoderWave224), 8, MNV2_224, synth.nyu_feature_shapes,
+                                                   NyuDepthLoss(use_wavelets=True, supervise_LL=True)),
+    "train_nyu_wave_d161_640x480_x8_nyuloss": train(_nyu(nd.DecoderWave), 8, D161, synth.nyu_feature_shapes,
+                                                    NyuDepthLoss()),
+    "train_decoder_d161_640x480_x8": train(_nyu(nd.Decoder), 8, D161, synth.nyu_feature_shapes),
+    "train_decoder224_mnv2light_x8": train(_nyu(nd.Decoder224), 8, MNV2_224, synth.nyu_feature_shapes),
+    "train_wave_r50_1024x320_x8": train(lambda ch: kd.DepthWaveProgressiveDecoder(np.array(ch)), 8, R50,
+                                        synth.kitti_feature_shapes),
+    "dense_no_skips_r18_640x192_x16": kitti_no_skips(16, R18),
+    "nyu_sparse_d161_640x480_x8_thr0": prod.nyu(nd.SparseDecoderWave, 8, D161, 0.0),
+    "nyu_sparse_d161_640x480_x8_thr0.5": prod.nyu(nd.SparseDecoderWave, 8, D161, 0.5),
+    "eval_nyu_sparse_d161_x%d_edges" % EVAL_FRAMES: nyu_eval_edges(EVAL_FRAMES, D161),
+    "eval_nyu_wave224_mnv2light_x8": nyu_eval_224(8, MNV2_224),
+    "eval_kitti_sparse_r18_x%d_postprocess" % EVAL_FRAMES: kitti_eval_pp(EVAL_FRAMES, R18),
+}
+
+
+@pytest.mark.parametrize("name", list(WORKLOADS))
+def test_every_launch_meets_its_contract(name, monkeypatch):
+    run = WORKLOADS[name]
+    t0 = time.perf_counter()
+    plain = {k: _raw(v) if torch.is_tensor(v) else v for k, v in run().items()}
+    torch.cuda.synchronize()
+    t1 = time.perf_counter()
+    harness = lc.Harness(monkeypatch)
+    with harness.workload(name):
+        checked = {k: _raw(v) if torch.is_tensor(v) else v for k, v in run().items()}
+    monkeypatch.undo()
+    t2 = time.perf_counter()
+    prod._same(plain, checked, name)
+    print("%s (%.1f s plain, %.1f s checked): %s" % (name, t1 - t0, t2 - t1,
+                                                     ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
+    del plain, checked, harness
+    gc.collect()
+    torch.cuda.empty_cache()

@@ -1,16 +1,21 @@
-"""Every libwmd symbol is classified for the launch-checking harness (tests/launch_check.py): a launch whose ops entry
-point has a checker, a pack, or a size / query function.  A new entry point cannot ship without one."""
+"""Every libwmd symbol is classified for the launch-checking harness (tests/launch_check.py): a launch whose entry point
+has a checker, a pack, or a size / query function.  A new entry point cannot ship without one."""
 import inspect
 
-from wavelet_monodepth_b200 import _lib, ops
+from wavelet_monodepth_b200 import _lib, kitti_eval, nyu_eval, nyu_loss, ops
 
 import launch_check as lc
 
+ALL_SIGNATURES = {**_lib.SIGNATURES, **_lib.EVAL_SIGNATURES, **_lib.LOSS_SIGNATURES}
+
 
 def test_every_symbol_is_classified():
-    unclassified = sorted(set(_lib.SIGNATURES) - set(lc.SYMBOLS))
+    """SYMBOLS covers wmd.h, wmd_eval.h and wmd_loss.h (their bindings, which test_abi / the oracle tests hold to the
+    headers), and nothing else."""
+    assert len(ALL_SIGNATURES) == len(_lib.SIGNATURES) + len(_lib.EVAL_SIGNATURES) + len(_lib.LOSS_SIGNATURES)
+    unclassified = sorted(set(ALL_SIGNATURES) - set(lc.SYMBOLS))
     assert not unclassified, "libwmd symbols without a launch checker / pack / query classification: %s" % unclassified
-    assert not sorted(set(lc.SYMBOLS) - set(_lib.SIGNATURES))
+    assert not sorted(set(lc.SYMBOLS) - set(ALL_SIGNATURES))
 
 
 def test_launches_and_packs_name_their_wrapped_entry_points():
@@ -19,19 +24,40 @@ def test_launches_and_packs_name_their_wrapped_entry_points():
             continue
         role, entry = kind
         assert role in ("launch", "pack"), (sym, kind)
-        assert entry in (lc.CHECKED if role == "launch" else lc.PACKS), (sym, entry)
-        assert hasattr(lc.Harness, ("_check_" if role == "launch" else "_pack_") + entry), (sym, entry)
+        assert entry in (lc.ENTRIES if role == "launch" else lc.PACKS), (sym, entry)
+        assert hasattr(lc.Harness, lc.hook("_check_", entry) if role == "launch" else "_pack_" + entry), (sym, entry)
+    assert len(set(lc.ENTRIES)) == len(lc.ENTRIES)
+    assert len({lc.hook("_check_", e) for e in lc.ENTRIES}) == len(lc.ENTRIES)
+    for owner, attr in lc.ENTRY_POINTS:
+        assert callable(getattr(owner, attr)), (owner, attr)
+
+
+def _functions(module):
+    """(entry name, function) of the module's own functions and of the methods of the classes it defines"""
+    for name, fn in inspect.getmembers(module, inspect.isfunction):
+        if fn.__module__ == module.__name__:
+            yield lc.entry_name(module, name), fn
+    for _, cls in inspect.getmembers(module, inspect.isclass):
+        if cls.__module__ != module.__name__:
+            continue
+        for name, fn in vars(cls).items():
+            if inspect.isfunction(fn):
+                yield lc.entry_name(cls, name), fn
 
 
 def test_every_ops_function_that_calls_libwmd_is_wrapped():
-    """An ops function that reaches a launch or pack symbol directly is a checked entry point or a pack."""
-    wrapped = set(lc.CHECKED) | set(lc.PACKS)
-    for name, fn in inspect.getmembers(ops, inspect.isfunction):
-        if fn.__module__ != ops.__name__:
-            continue
-        src = inspect.getsource(fn)
-        used = [s for s, k in lc.SYMBOLS.items() if k != "query" and "lib.%s(" % s in src]
-        if used:
-            assert name in wrapped, (name, used)
-    for entry in wrapped:
+    """A function or method of ops, nyu_loss, nyu_eval or kitti_eval that reaches a launch or pack symbol directly is a
+    checked entry point or a pack."""
+    wrapped = set(lc.ENTRIES) | set(lc.PACKS)
+    found = set()
+    for module in (ops, nyu_loss, nyu_eval, kitti_eval):
+        for name, fn in _functions(module):
+            src = inspect.getsource(fn)
+            used = [s for s, k in lc.SYMBOLS.items() if k != "query" and ".%s(" % s in src]
+            if used:
+                assert name in wrapped, (module.__name__, name, used)
+                found.add(name)
+    # every wrapped entry point of the evaluation and loss modules calls libwmd itself
+    assert {lc.entry_name(o, a) for o, a in lc.EVAL_LOSS} <= found
+    for entry in set(lc.CHECKED) | set(lc.PACKS):
         assert callable(getattr(ops, entry)), entry

@@ -1,0 +1,249 @@
+"""The launch checkers of the evaluation and loss entry points (tests/launch_check.py) have teeth: each passes the oracle's
+own answer and raises LaunchError when one element of it is changed by the smallest step its bar must see (a loss
+gradient one ulp off, one edge pixel toggled, one a_k count off by one, one KITTI median ratio one ulp off).  CPU only:
+the checkers are called directly on CPU tensors, with stand-ins for the evaluators' state; no GPU and no libwmd."""
+import types
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import kitti_eval as oke
+from oracle import nyu_edges as ne
+from oracle import nyu_eval as one
+from oracle import nyu_loss as onl
+
+import launch_check as lc
+
+
+@pytest.fixture
+def harness():
+    """A Harness without its libwmd plumbing: the checkers only read the workload's name."""
+    saved = dict(lc.REPORT)
+    h = object.__new__(lc.Harness)
+    h.current = "teeth"
+    yield h
+    lc.REPORT.clear()
+    lc.REPORT.update(saved)
+
+
+def t(a):
+    return torch.from_numpy(np.ascontiguousarray(a))
+
+
+def ulp_up(a, index):
+    """a copy of float array a with element `index` moved one ulp away from zero"""
+    b = np.array(a, copy=True)
+    b[index] = np.nextafter(b[index], np.copysign(np.inf, b[index]), dtype=b.dtype)
+    return b
+
+
+def both(check, good, bad):
+    """check(good) passes; check(bad) raises LaunchError"""
+    check(*good)
+    with pytest.raises(lc.LaunchError):
+        check(*bad)
+
+
+# ------------------------------------------------------------------------------------------ NYUv2 training loss
+def _loss_case():
+    rng = np.random.default_rng(0)
+    n, H, W = 2, 16, 24
+    target = rng.uniform(10.0, 1000.0, (n, 1, H, W)).astype(np.float32)
+    preds = [(target[..., ::1 << s, ::1 << s] * rng.uniform(0.7, 1.3, (n, 1, H >> s, W >> s))).astype(np.float32)
+             for s in onl.SCALES]
+    means = np.array([onl.term(p[:, 0], target[:, 0]) for p in preds], np.float32)
+    signs = np.stack([onl.signs(onl.upsample(p[:, 0], H, W), target[:, 0]) for p in preds])
+    return target, preds, means, signs
+
+
+def test_loss_fwd_checker(harness):
+    target, preds, means, signs = _loss_case()
+
+    def call(means, signs):
+        a = dict(target=t(target), preds=[t(p) for p in preds], log2s=onl.SCALES, means=t(means), want_signs=True)
+        harness._check_loss_fwd(a, t(signs), None)
+    both(call, (means, signs), (ulp_up(ulp_up(means, 2), 2), signs))     # one term two ulp off
+    flipped = signs.copy()
+    flipped[1, 0, 5, 7] = -flipped[1, 0, 5, 7] if flipped[1, 0, 5, 7] else 1
+    both(call, (means, signs), (means, flipped))                          # one sign wrong
+
+
+def test_loss_bwd_checker(harness):
+    target, preds, _, signs = _loss_case()
+    n, _, H, W = target.shape
+    g = np.full(len(preds), 0.1, np.float32)
+    grads = [(np.float64(g[k]) / np.float64(n * H * W) * onl.adjoint(signs[k], p.shape[2], p.shape[3]))
+             .astype(np.float32)[:, None] for k, p in enumerate(preds)]
+
+    def call(grads):
+        a = dict(signs=t(signs), target_shape=(n, 1, H, W), preds=[t(p) for p in preds], log2s=onl.SCALES,
+                 grad_means=t(g))
+        harness._check_loss_bwd(a, [t(x) for x in grads], None)
+    bad = list(grads)
+    bad[2] = ulp_up(grads[2], (1, 0, 3, 4))                               # one gradient one ulp off
+    assert grads[2][1, 0, 3, 4] != 0
+    both(call, (grads,), (bad,))
+
+
+# ------------------------------------------------------------------------------------------ NYUv2 evaluation
+def test_nyu_evaluator_add_checker(harness):
+    split = one.synthetic_split(0, n=2)
+    disp = split["disp"][(60, 80, False)]
+    gt = one.prepare_gt(split["gt"])
+    gt_log10 = torch.log10(t(gt))
+    depth = one.predict(disp)
+    sums = one.frame_sums(depth, gt, gt_log10.numpy())
+    assert sums[:, 3].min() > 0
+
+    def call(depth_out, sums_out):
+        ev = types.SimpleNamespace(gt=t(gt), gt_log10=gt_log10, sums=t(sums_out), use_224=False, use_disparity=False,
+                                   next_frame=2)
+        pre = (0, torch.full_like(ev.sums, float("nan")))
+        harness._check_NyuDepthEvaluator_add(dict(self=ev, disp=t(disp)[:, None], depth_out=t(depth_out)), None, pre)
+    count_off = sums.copy()
+    count_off[1, 4] += 1                                                  # one a_2 count off by one
+    both(call, (depth, sums), (depth, count_off))
+    both(call, (depth, sums), (ulp_up(depth, (0, 100, 200)), sums))       # one map value one ulp off
+    rel_off = sums.copy()
+    rel_off[0, 0] *= 1 + 1e-11                                            # a sum past its 1e-12 bar
+    both(call, (depth, sums), (depth, rel_off))
+
+
+def test_compute_errors_nyu_checker(harness):
+    rng = np.random.default_rng(1)
+    gt = rng.uniform(0.5, 10.0, 5000)
+    pred = gt * rng.uniform(0.6, 1.6, 5000)
+    want = one.compute_errors_nyu(pred, gt)
+    off = want.copy()
+    off[3] += 1.0 / 5000                                                  # one a_1 count off by one
+
+    def call(out):
+        harness._check_compute_errors_nyu(dict(pred=t(pred), gt=t(gt)), t(out), None)
+    both(call, (want,), (off,))
+
+
+def _edge_case():
+    rng = np.random.default_rng(2)
+    h, w = 40, 56
+    yy, xx = np.mgrid[0:h, 0:w] / np.array([h - 1, w - 1])[:, None, None]
+    frames = []
+    for k in range(2):
+        d = 2.0 + yy + 0.5 * np.sin(6 * xx + k)
+        d[h // 4:h // 2 + 1, w // 3:2 * w // 3 + 1] += 2.0
+        frames.append((d * rng.uniform(0.97, 1.03, (h, w))).astype(np.float32))
+    pred = np.stack(frames)
+    edges_gt = np.stack([ne.step_edges(p, 0.5) for p in pred]).astype(np.float32)
+    res = [ne.dbe(edges_gt[i], pred[i]) for i in range(2)]
+    est = np.stack([r[2] for r in res])
+    assert est.sum() > 0 and np.isfinite([r[:2] for r in res]).all()
+    return pred, edges_gt, est, np.stack([r[3] for r in res]), np.array([r[:2] for r in res])
+
+
+def test_edges_frames_checker(harness):
+    pred, edges_gt, est, d_est, scores = _edge_case()
+
+    def call(est, d_est, scores):
+        a = dict(pred=t(pred.astype(np.float64)), edges_gt=t(edges_gt), scores=t(scores), low=ne.LOW, high=ne.HIGH)
+        harness._check_edges_frames(a, (t(est), t(d_est)), None)
+    toggled = est.copy()
+    toggled[1, 10, 20] = ~toggled[1, 10, 20]                              # one edge pixel toggled
+    both(call, (est, d_est, scores), (toggled, d_est, scores))
+    both(call, (est, d_est, scores), (est, ulp_up(d_est, (0, 3, 3)), scores))
+    off = scores.copy()
+    off[0, 1] *= 1 + 1e-11
+    both(call, (est, d_est, scores), (est, d_est, off))
+
+
+def test_edt_checker(harness):
+    _, _, est, d_est, _ = _edge_case()
+    feats = est.astype(np.uint8)
+    feats[1] = 0                                                          # no feature pixel: scipy's own answer
+    dist = np.stack([ne.edt(f) for f in feats != 0])
+
+    def call(dist):
+        harness._check_edt(dict(features=t(feats)), t(dist), None)
+    both(call, (dist,), (ulp_up(dist, (1, 7, 9)),))
+
+
+# ------------------------------------------------------------------------------------------ KITTI evaluation
+def _kitti_case():
+    rng = np.random.default_rng(3)
+    frames = []
+    for H, W in ((40, 120), (38, 124)):
+        lidar = rng.random((H, W)) < 0.3
+        frames.append(np.where(lidar, rng.uniform(0.0, 100.0, (H, W)), 0.0).astype(np.float32))
+    hm, wm = 40, 124
+    padded = np.zeros((2, hm, wm), np.float32)
+    for i, f in enumerate(frames):
+        padded[i, :f.shape[0], :f.shape[1]] = f
+    mask = np.zeros(padded.shape, bool)
+    for i, f in enumerate(frames):
+        mask[i, :f.shape[0], :f.shape[1]] = oke.valid_mask(f, "eigen")
+    pixels = np.flatnonzero(mask).astype(np.int32)
+    offsets = np.concatenate([[0], np.cumsum(mask.reshape(2, -1).sum(1))]).astype(np.int32)
+    ev = types.SimpleNamespace(h_max=hm, w_max=wm, hw=t(np.array([f.shape for f in frames], np.int32)),
+                               offsets=t(offsets), pixels=t(pixels), gt=t(padded.reshape(-1)[pixels]),
+                               eval_split="eigen", median_scaling=True, pred_depth_scale_factor=1.0)
+    assert offsets[1] > 10 and offsets[2] > offsets[1] + 10
+    return frames, ev
+
+
+def test_kitti_evaluator_init_checker(harness):
+    frames, ev = _kitti_case()
+
+    def call(offsets):
+        e = types.SimpleNamespace(**dict(vars(ev), offsets=t(offsets)))
+        harness._check_KittiDepthEvaluator_init(dict(self=e, gt_depths=frames, eval_split="eigen"), None, None)
+    off = ev.offsets.numpy().copy()
+    bad = off.copy()
+    bad[1] += 1                                                           # one frame's valid count off by one
+    both(call, (off,), (bad,))
+
+
+def test_kitti_evaluator_add_checker(harness):
+    frames, ev = _kitti_case()
+    rng = np.random.default_rng(4)
+    disp = (0.3 / rng.uniform(3.0, 60.0, (2, 16, 48))).astype(np.float32)
+    want = [oke.evaluate_frame(g, d) for g, d in zip(frames, disp)]
+    errors = np.stack([w[0] for w in want])
+    ratios = np.array([w[1] for w in want])
+    counts = np.array([w[2] for w in want], np.int32)
+
+    def call(errors, ratios, counts):
+        e = types.SimpleNamespace(**dict(vars(ev), errors=t(errors), ratios=t(ratios), counts=t(counts), next_frame=2))
+        pre = (0, [torch.full((2, 7), float("nan"), dtype=torch.float64), torch.full((2,), float("nan"),
+                   dtype=torch.float64), torch.zeros(2, dtype=torch.int32)])
+        harness._check_KittiDepthEvaluator_add(dict(self=e, pred_disp=t(disp)), None, pre)
+    both(call, (errors, ratios, counts), (errors, ulp_up(ratios, 1), counts))       # one median ratio one ulp off
+    c = counts.copy()
+    c[0] += 1
+    both(call, (errors, ratios, counts), (errors, ratios, c))
+    a1 = errors.copy()
+    a1[1, 4] += 1.0 / counts[1]                                           # one a1 count off by one
+    both(call, (errors, ratios, counts), (a1, ratios, counts))
+
+
+def test_post_process_checker(harness):
+    l_disp, r_disp = oke.post_process_inputs(5, n=2, h=8, w=16)
+    r = r_disp[:, :, ::-1]
+    want = oke.batch_post_process_disparity(l_disp, r)
+    off = want.copy()
+    off[1, 3, 5] *= 1 + 1e-14
+
+    def call(out):
+        harness._check_batch_post_process_disparity(dict(l_disp=t(l_disp), r_disp=t(r)), t(out), None)
+    both(call, (want,), (off,))
+
+
+def test_kitti_compute_errors_checker(harness):
+    rng = np.random.default_rng(6)
+    gt = rng.uniform(1.0, 80.0, 3000)
+    pred = gt * rng.uniform(0.6, 1.6, 3000)
+    want = np.array(oke.compute_errors(gt, pred))
+    off = want.copy()
+    off[6] -= 1.0 / 3000                                                  # one a3 count off by one
+
+    def call(out):
+        harness._check_compute_errors(dict(gt=t(gt), pred=t(pred)), t(out), None)
+    both(call, (want,), (off,))

@@ -1,10 +1,12 @@
 // Backward of the gather-GEMM convolution (training the dense decoders):
 //
-//   act_bwd    dz = dy * act'(y) from the saved post-activation output, the bias gradient sum_rows dz in a fixed order,
+//   act_bwd    dz = dy * act'(y) from the saved post-activation output, the bias gradient sum_rows dz in fp64 in a fixed
+//              order (rounded to fp32 once),
 //              and max |dz| raised into a device scalar (the fp16-pair operand form of the data-gradient GEMM needs it);
 //   wgrad      dW[tap][c][o] = sum_p A(p)[tap][c] dz(p)[o] on the tensor cores (mma.sync tf32, 3xTF32 split), A gathered
-//              exactly as the forward gathers it; the pixel reduction is split across CTAs and the partial slabs are
-//              summed in slab order by the last CTA of a tile to arrive - no float atomics, the bits do not depend on timing;
+//              exactly as the forward gathers it; the pixel reduction (fp64 sums of 32-pixel chunks) is split across CTAs
+//              and the partial slabs are summed in slab order by the last CTA of a tile to arrive - no float atomics, the
+//              bits do not depend on timing;
 //   dgrad_fold the data gradient is the forward contract itself (flipped, transposed weight, zero padding) run by the
 //              forward engine over the grid extended by the one-pixel ring; this kernel adds every ring value into the pixel
 //              the forward's pad mode read it from, sums the 2x2 children of a shift0 = 1 source into its low-resolution
@@ -35,16 +37,18 @@ static int ab_blocks(int rows) { return rows <= 0 ? 1 : (ceil_div(rows, 64) < AB
 
 __global__ void __launch_bounds__(AB_THREADS) act_bwd_kernel(const float* __restrict__ y, int ldy, const float* __restrict__ dy,
                                                              int lddy, int rows, int cout, int act, float p, float* dz,
-                                                             int lddz, float* db, float* amax, float* partial,
+                                                             int lddz, float* db, float* amax, double* partial,
                                                              unsigned* ticket, int rows_per_block) {
-  __shared__ float red[8][33];
+  // The bias gradient is summed in fp64 and rounded once: a column of 600 000 same-sign fp32 values summed in fp32 (a
+  // per-thread chain, then up to 1024 block partials in order) drifts by ~1e-5 of the sum, 170 roundings' worth.
+  __shared__ double red[8][33];
   __shared__ bool last;
   const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5;
   const int r0 = blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
   float vmax = 0.f;
   for (int cb = 0; cb < cout; cb += 32) {
     const int c = cb + lane;
-    float s = 0.f;
+    double s = 0.0;
     if (c < cout) {
       for (int r = r0 + rl; r < r1; r += 8) {
         const float g = dy[static_cast<long long>(r) * lddy + c] * act_grad(y[static_cast<long long>(r) * ldy + c], act, p);
@@ -56,7 +60,7 @@ __global__ void __launch_bounds__(AB_THREADS) act_bwd_kernel(const float* __rest
     red[rl][lane] = s;
     __syncthreads();
     if (rl == 0 && c < cout && db) {
-      float t = red[0][lane];
+      double t = red[0][lane];
 #pragma unroll
       for (int k = 1; k < 8; ++k) t += red[k][lane];
       partial[static_cast<long long>(blockIdx.x) * cout + c] = t;
@@ -77,9 +81,9 @@ __global__ void __launch_bounds__(AB_THREADS) act_bwd_kernel(const float* __rest
   if (!last) return;
   __threadfence();
   for (int c = threadIdx.x; c < cout; c += AB_THREADS) {
-    float t = 0.f;
+    double t = 0.0;
     for (int b = 0; b < static_cast<int>(gridDim.x); ++b) t += __ldcg(partial + static_cast<long long>(b) * cout + c);
-    db[c] = t;
+    db[c] = __double2float_rn(t);
   }
   if (threadIdx.x == 0) *ticket = 0u;
 }
@@ -142,7 +146,7 @@ __device__ __forceinline__ void mma_tf32(float* c, const uint32_t* a, uint32_t b
 // taps and channel blocks that read the same pixel rows run together and share them through L2.
 template <int BN>
 __global__ void __launch_bounds__(WG_THREADS) conv_wgrad_kernel(const wmd_conv_desc d, const float* __restrict__ dz, int lddz,
-                                                                float* __restrict__ dw, unsigned* counters, float* slabs,
+                                                                float* __restrict__ dw, unsigned* counters, double* slabs,
                                                                 int mt0, int ntn, long long nch) {
   using Cfg = WgCfg<BN>;
   constexpr int NT = Cfg::NT, A_LD = Cfg::A_LD, B_LD = Cfg::B_LD;
@@ -215,11 +219,12 @@ __global__ void __launch_bounds__(WG_THREADS) conv_wgrad_kernel(const wmd_conv_d
     }
   };
 
-  float acc[NT][4], sum[NT][4];
+  float acc[NT][4];
+  double sum[NT][4];
 #pragma unroll
   for (int j = 0; j < NT; ++j)
 #pragma unroll
-    for (int k = 0; k < 4; ++k) acc[j][k] = sum[j][k] = 0.f;
+    for (int k = 0; k < 4; ++k) { acc[j][k] = 0.f; sum[j][k] = 0.0; }
 
   const long long nloc = ch_end - ch_begin;
 #pragma unroll
@@ -254,8 +259,10 @@ __global__ void __launch_bounds__(WG_THREADS) conv_wgrad_kernel(const wmd_conv_d
       }
     }
     // one epoch per 32-pixel chunk: the tensor core's accumulation does not round to nearest, so each chunk's sum is
-    // added into round-to-nearest fp32 sums.  On the real operands of every layer of the R18 640x192 decoder step this
-    // keeps dW within 6.7e-7 of the largest fp64 element, against up to 1.0e-5 with 1024-pixel epochs.
+    // added into round-to-nearest sums.  On the real operands of every layer of the R18 640x192 decoder step this keeps
+    // dW within 6.7e-7 of the largest fp64 element, against up to 1.0e-5 with 1024-pixel epochs.  The sums are fp64:
+    // in fp32 a whole-tile reduction of 1200 chunks (NYU Decoder's up3 convA, 8 frames of 60 x 80) drifted to 2.55e-6
+    // of S, over the weight gradient's bar.
 #pragma unroll
     for (int j = 0; j < NT; ++j)
 #pragma unroll
@@ -275,13 +282,13 @@ __global__ void __launch_bounds__(WG_THREADS) conv_wgrad_kernel(const wmd_conv_d
 #pragma unroll
     for (int j = 0; j < NT; ++j)
 #pragma unroll
-      for (int k = 0; k < 4; ++k) store(j, k, sum[j][k]);
+      for (int k = 0; k < 4; ++k) store(j, k, __double2float_rn(sum[j][k]));
     return;
   }
   // partial slab of this split; the last split of the tile to arrive sums all of them in slab order
   constexpr int SLAB = WG_BM * BN;
   const int lidx0 = (wm + g) * BN + 2 * t;
-  float* my = slabs + (static_cast<long long>(split) * gridDim.x + tile) * SLAB;
+  double* my = slabs + (static_cast<long long>(split) * gridDim.x + tile) * SLAB;
 #pragma unroll
   for (int j = 0; j < NT; ++j)
 #pragma unroll
@@ -298,9 +305,9 @@ __global__ void __launch_bounds__(WG_THREADS) conv_wgrad_kernel(const wmd_conv_d
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int li = lidx0 + 8 * (k >> 1) * BN + j * 8 + (k & 1);
-      float v = 0.f;
+      double v = 0.0;
       for (int s = 0; s < splits; ++s) v += __ldcg(slabs + (static_cast<long long>(s) * gridDim.x + tile) * SLAB + li);
-      store(j, k, v);
+      store(j, k, __double2float_rn(v));
     }
   if (tid == 0) counters[tile] = 0u;
 }
@@ -318,7 +325,7 @@ static int launch_wgrad(const wmd_conv_desc& d, const WgPlan& p, const float* dz
     if (dev >= 0 && dev < 64) attr_done[dev] = true;
   }
   unsigned* counters = reinterpret_cast<unsigned*>(ws);
-  float* slabs = ws ? reinterpret_cast<float*>(ws + BWD_COUNTERS) : nullptr;
+  double* slabs = ws ? reinterpret_cast<double*>(ws + BWD_COUNTERS) : nullptr;
   conv_wgrad_kernel<BN><<<dim3(p.tiles, p.splits), WG_THREADS, WgCfg<BN>::SMEM, stream>>>(d, dz, lddz, dw, counters, slabs,
                                                                                          p.mt0, p.ntn, p.nch);
   return launched();
@@ -411,7 +418,7 @@ __global__ void fold_src1_kernel(const float* __restrict__ g, int ldg, int N, in
 }  // namespace wmd
 
 extern "C" size_t wmd_act_bwd_ws_bytes(int rows, int cout) {
-  return wmd::AB_HEADER + static_cast<size_t>(wmd::ab_blocks(rows)) * (cout > 0 ? cout : 0) * sizeof(float);
+  return wmd::AB_HEADER + static_cast<size_t>(wmd::ab_blocks(rows)) * (cout > 0 ? cout : 0) * sizeof(double);
 }
 
 extern "C" int wmd_act_bwd_f32(const float* y, int ldy, const float* dy, int lddy, int rows, int cout, int act,
@@ -434,7 +441,7 @@ extern "C" int wmd_act_bwd_f32(const float* y, int ldy, const float* dy, int ldd
   unsigned char* w = static_cast<unsigned char*>(ws);
   act_bwd_kernel<<<ceil_div(rows, per), AB_THREADS, 0, as_stream(stream)>>>(
       y, ldy, dy, lddy, rows, cout, act, act_param, dz, lddz, db, amax_dz,
-      w ? reinterpret_cast<float*>(w + AB_HEADER) : nullptr, reinterpret_cast<unsigned*>(w), per);
+      w ? reinterpret_cast<double*>(w + AB_HEADER) : nullptr, reinterpret_cast<unsigned*>(w), per);
   return launched();
 }
 
@@ -464,7 +471,7 @@ extern "C" size_t wmd_conv_wgrad_ws_bytes(const wmd_conv_desc* dp) {
   if (!d.x1) d.c1 = 0;
   const WgPlan p = wg_plan(d);
   if (p.splits == 1) return 0;
-  return BWD_COUNTERS + static_cast<size_t>(p.splits) * p.tiles * WG_BM * p.bn * sizeof(float);
+  return BWD_COUNTERS + static_cast<size_t>(p.splits) * p.tiles * WG_BM * p.bn * sizeof(double);
 }
 
 extern "C" int wmd_conv_wgrad_f32(const wmd_conv_desc* dp, const float* dz, int lddz, float* dw, void* ws, size_t ws_bytes,
