@@ -10,6 +10,8 @@ Public surface = the reference's (nianticlabs/wavelet-monodepth) own API for thi
                  SparseDecoderWave                                 <- NYUv2/networks/{layers,decoders/densedepth_decoder}.py
   nyu_loss       NyuDepthLoss: the NYUv2 training objective,
                  forward and backward, deterministic               <- NYUv2/train.py:279-327
+  kitti_loss     KittiDepthHintsLoss: KITTI's stereo depth-hints
+                 objective, forward and backward, deterministic    <- KITTI/trainer.py:329-560
   shard          batch sharding + the single all-gather (one process per GPU)
   ops / _lib     tensor-level wrappers over the C ABI of libwmd.so (include/wmd.h)
 

@@ -171,6 +171,16 @@ class LossTerm(Structure):
     _fields_ = [("pred", c_void_p), ("h", c_int32), ("w", c_int32), ("log2_factor", c_int32)]
 
 
+class KittiLossDesc(Structure):
+    """struct wmd_loss_kitti_desc (include/wmd_loss_kitti.h)."""
+    _fields_ = [("N", c_int32), ("H", c_int32), ("W", c_int32),
+                ("target", c_void_p), ("source", c_void_p), ("K", c_void_p), ("inv_K", c_void_p),
+                ("stereo_T", c_void_p), ("depth_hint", c_void_p), ("depth_hint_mask", c_void_p),
+                ("n_scales", c_int32), ("n_loss", c_int32), ("scale", c_int32 * 4),
+                ("disp", c_void_p * 4), ("color", c_void_p * 4), ("noise", c_void_p * 4),
+                ("min_depth", c_double), ("max_depth", c_double), ("disparity_smoothness", c_double)]
+
+
 # include/wmd_loss.h: the training-loss entry points (tests/test_oracle_nyu_loss.py checks this table against it)
 LOSS_SIGNATURES = {
     "wmd_loss_nyu_ws_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
@@ -178,6 +188,15 @@ LOSS_SIGNATURES = {
                                  c_void_p, c_void_p]),
     "wmd_loss_nyu_bwd": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(LossTerm), c_int, c_void_p, POINTER(c_void_p),
                                  c_void_p]),
+}
+# include/wmd_loss_kitti.h: KITTI's depth-hints loss (tests/test_oracle_kitti_loss.py checks this table against it)
+KITTI_LOSS_SIGNATURES = {
+    "wmd_loss_kitti_ws_bytes": (c_size_t, [POINTER(KittiLossDesc)]),
+    "wmd_loss_kitti_bwd_ws_bytes": (c_size_t, [POINTER(KittiLossDesc)]),
+    "wmd_loss_kitti_fwd": (c_int, [POINTER(KittiLossDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                   c_void_p, c_void_p]),
+    "wmd_loss_kitti_bwd": (c_int, [POINTER(KittiLossDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_size_t, POINTER(c_void_p), c_void_p]),
 }
 
 _lib = None
@@ -206,7 +225,8 @@ def load():
             except OSError:
                 continue
         lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in list(SIGNATURES.items()) + list(EVAL_SIGNATURES.items()) + list(LOSS_SIGNATURES.items()):
+    tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES)
+    for name, (res, args) in [item for table in tables for item in table.items()]:
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
