@@ -200,14 +200,8 @@ class DepthDecoder(_PackedModule):
                                lambda: ops.pack_disp_tail16(c1.weight, c1.bias, cd.weight, cd.bias))
 
     @torch.no_grad()
+    @ops._on_device
     def _native_forward(self, feats):
-        dev = next(f.device for f in feats if f.is_cuda) if any(f.is_cuda for f in feats) else None
-        if dev is not None and dev.index is not None and dev.index != torch.cuda.current_device():
-            with torch.cuda.device(dev):       # libwmd launches on the current device: make the tensors' device current
-                return self._native_forward_on_device(feats)
-        return self._native_forward_on_device(feats)
-
-    def _native_forward_on_device(self, feats):
         """upconv(i,0) / upconv(i,1) on the gather-GEMM engine, dispconv(s) on head_conv3x3, ("disp", 0) on the fused
         tail.  Operands in the fp16-pair form with tracked maxima, as in the wavelet engine."""
         _need_cuda(feats)
@@ -359,18 +353,6 @@ class _WaveDecoderBase(_PackedModule):
                                                          ops.head_tap_weight([c3p.weight, c3n.weight], [0, c], 2 * c)))
 
     # ---- native engine ------------------------------------------------------------------------
-    @torch.no_grad()
-    def _native_forward(self, feats, thresh_ratio, sparse_levels, with_masks):
-        """Runs levels 4..1 on libwmd.  sparse_levels: set of levels i executed on active lists.
-
-        Returns (outputs, counts): counts = int32 device tensor (levels, 3, N+1) with the row offsets of the compacted
-        sets S2, S4, S5 of every sparse level, sparse levels in descending order (None without sparse levels)."""
-        dev = next(f.device for f in feats if f.is_cuda) if any(f.is_cuda for f in feats) else None
-        if dev is not None and dev.index is not None and dev.index != torch.cuda.current_device():
-            with torch.cuda.device(dev):       # libwmd launches on the current device: make the tensors' device current
-                return self._native_forward_on_device(feats, thresh_ratio, sparse_levels, with_masks)
-        return self._native_forward_on_device(feats, thresh_ratio, sparse_levels, with_masks)
-
     def _empty_outputs(self, feats, sparse_levels, with_masks):
         """Outputs of an empty batch (a rank whose shard is empty: world size > batch) - right keys, N = 0."""
         dev = feats[-1].device
@@ -388,7 +370,13 @@ class _WaveDecoderBase(_PackedModule):
         counts = torch.zeros((len(sparse_levels), 3, 1), dtype=torch.int32, device=dev) if sparse_levels else None
         return out, counts
 
-    def _native_forward_on_device(self, feats, thresh_ratio, sparse_levels, with_masks):
+    @torch.no_grad()
+    @ops._on_device
+    def _native_forward(self, feats, thresh_ratio, sparse_levels, with_masks):
+        """Runs levels 4..1 on libwmd.  sparse_levels: set of levels i executed on active lists.
+
+        Returns (outputs, counts): counts = int32 device tensor (levels, 3, N+1) with the row offsets of the compacted
+        sets S2, S4, S5 of every sparse level, sparse levels in descending order (None without sparse levels)."""
         # with gated_layout the skip map of a sparse level i (feats[i-1]) may live in pinned host memory
         _need_cuda(feats, host_ok=tuple(i - 1 for i in sparse_levels) if (self.gated_layout or self.compact_skip) else ())
         out = {}
@@ -577,8 +565,7 @@ class DepthWaveProgressiveDecoder(_WaveDecoderBase):
 
     def forward(self, input_features):
         _need_cuda(input_features)
-        needs_grad = torch.is_grad_enabled() and (
-            any(p.requires_grad for p in self.parameters()) or any(f.requires_grad for f in input_features))
+        needs_grad = _needs_grad(self, input_features)
         if needs_grad and train_native.fp32_convs_requested():
             # fp32 convolutions requested: forward and backward of every convolution on libwmd
             self.outputs = train_native.kitti_forward(self, input_features)

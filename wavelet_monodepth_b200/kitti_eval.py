@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .ops import _dense, _on_device, _prof, compact
+from .ops import _dense, _launch, _on_device, compact
 
 _f64 = torch.float64
 METRICS = ("abs_rel", "sq_rel", "rmse", "rmse_log", "a1", "a2", "a3")
@@ -36,8 +36,7 @@ def compute_errors(gt, pred):
         raise _lib.WmdError("compute_errors: too many pixels")
     gt, pred = _dense(gt.reshape(-1), _f64), _dense(pred.reshape(-1), _f64)
     out = torch.empty(7, dtype=_f64, device=gt.device)
-    rc = _lib.load().wmd_eval_errors_f64(_lib.ptr(gt), _lib.ptr(pred), gt.numel(), _lib.ptr(out), _lib.stream_ptr())
-    _lib.check(rc, "wmd_eval_errors_f64")
+    _launch().wmd_eval_errors_f64(_lib.ptr(gt), _lib.ptr(pred), gt.numel(), _lib.ptr(out), _lib.stream_ptr())
     return out
 
 
@@ -53,10 +52,8 @@ def batch_post_process_disparity(l_disp, r_disp):
     out = torch.empty((n, h, w), dtype=_f64, device=lt.device)
     if out.numel() == 0:
         return out
-    with _prof("post_process_disparity", lambda: dict(n=n, h=h, w=w)):
-        rc = _lib.load().wmd_post_process_disparity(_lib.ptr(lt), _lib.ptr(rt), l64, _lib.ptr(out), n, h, w,
-                                                    _lib.stream_ptr())
-    _lib.check(rc, "wmd_post_process_disparity")
+    _launch("post_process_disparity", lambda: dict(n=n, h=h, w=w)).wmd_post_process_disparity(
+        _lib.ptr(lt), _lib.ptr(rt), l64, _lib.ptr(out), n, h, w, _lib.stream_ptr())
     return out
 
 
@@ -109,19 +106,19 @@ class KittiDepthEvaluator:
         for i, f in enumerate(frames):
             padded[i, :f.shape[0], :f.shape[1]] = f
         with torch.cuda.device(self.device):
-            lib = _lib.load()
             gt = torch.from_numpy(padded).to(self.device)
             self.hw = torch.from_numpy(sizes).to(self.device)
             mask = torch.empty(gt.shape, dtype=torch.uint8, device=self.device)
             split = _lib.EVAL_EIGEN if eval_split == "eigen" else _lib.EVAL_GT_POSITIVE
-            _lib.check(lib.wmd_eval_gt_mask(_lib.ptr(gt), _lib.ptr(self.hw), _lib.ptr(mask), n, self.h_max, self.w_max,
-                                            split, _lib.stream_ptr()), "wmd_eval_gt_mask")
+            _launch().wmd_eval_gt_mask(
+                _lib.ptr(gt), _lib.ptr(self.hw), _lib.ptr(mask), n, self.h_max, self.w_max, split, _lib.stream_ptr())
             _, pixels, self.offsets = compact(mask, want_idxmap=False)
             total = int(self.offsets[-1])                 # the split's one read-back: sizes the buffers below
             self.pixels = pixels[:max(total, 1)].clone()
             self.gt = torch.empty(max(total, 1), dtype=torch.float32, device=self.device)
-            _lib.check(lib.wmd_eval_gather_f32(_lib.ptr(gt), _lib.ptr(self.pixels), _lib.ptr(self.offsets[n:]), total,
-                                               _lib.ptr(self.gt), _lib.stream_ptr()), "wmd_eval_gather_f32")
+            _launch().wmd_eval_gather_f32(
+                _lib.ptr(gt), _lib.ptr(self.pixels), _lib.ptr(self.offsets[n:]), total, _lib.ptr(self.gt),
+                _lib.stream_ptr())
             with np.errstate(all="ignore"):
                 self.gt_log = torch.from_numpy(np.log(self.gt.cpu().numpy())).to(self.device)
             self.depth = torch.empty(max(total, 1), dtype=_f64, device=self.device)
@@ -153,13 +150,12 @@ class KittiDepthEvaluator:
             raise _lib.WmdError("pred_disp %dx%d must be no larger than every ground-truth frame (%dx%d)"
                                 % (h, w, self.h_min, self.w_min))
         f0 = self.next_frame
-        with torch.cuda.device(self.device), _prof("eval_frames", lambda: dict(n=n, h=h, w=w)):
-            rc = _lib.load().wmd_eval_frames(
+        with torch.cuda.device(self.device):
+            _launch("eval_frames", lambda: dict(n=n, h=h, w=w)).wmd_eval_frames(
                 _lib.ptr(disp), f64, n, h, w, f0, _lib.ptr(self.hw), _lib.ptr(self.pixels), _lib.ptr(self.offsets),
                 _lib.ptr(self.gt), _lib.ptr(self.gt_log), self.h_max, self.w_max, self.pred_depth_scale_factor,
                 int(self.median_scaling), _lib.ptr(self.depth), _lib.ptr(self.errors[f0:]), _lib.ptr(self.ratios[f0:]),
                 _lib.ptr(self.counts[f0:]), _lib.stream_ptr())
-        _lib.check(rc, "wmd_eval_frames")
         self.next_frame += n
         if sparse_outputs is not None:
             self._density.append(compute_density(sparse_outputs))

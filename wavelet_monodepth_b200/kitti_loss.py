@@ -16,7 +16,7 @@ import ctypes
 import torch
 
 from . import _lib
-from .ops import _dense, _on_device, _prof
+from .ops import _dense, _launch, _on_device
 
 SCALES = (0, 1, 2, 3)          # options.py: --scales default
 
@@ -40,31 +40,26 @@ def _kitti_fwd(t, scales, loss_scales, opt):
     d = _desc(t, scales, loss_scales, opt)
     n, h, w, nl = d.N, d.H, d.W, d.n_loss
     dev = t["target"].device
-    lib = _lib.load()
-    ws = torch.empty(int(lib.wmd_loss_kitti_ws_bytes(ctypes.byref(d))), dtype=torch.uint8, device=dev)
+    ws = torch.empty(int(_lib.load().wmd_loss_kitti_ws_bytes(ctypes.byref(d))), dtype=torch.uint8, device=dev)
     terms = torch.empty(1 + 3 * nl, dtype=torch.float32, device=dev)
     chint = torch.empty((n, 3, h, w), dtype=torch.float32, device=dev)
     warped = torch.empty((nl, n, 3, h, w), dtype=torch.float32, device=dev)
     idsel = torch.empty((nl, n, 1, h, w), dtype=torch.float32, device=dev)
     hpix = torch.empty((nl, n, 1, h, w), dtype=torch.float32, device=dev)
-    with _prof("loss_kitti_fwd", lambda: dict(n=n, h=h, w=w, scales=nl)):
-        rc = lib.wmd_loss_kitti_fwd(ctypes.byref(d), _lib.ptr(chint), _lib.ptr(warped), _lib.ptr(idsel),
-                                    _lib.ptr(hpix), _lib.ptr(ws), ws.numel(), _lib.ptr(terms), _lib.stream_ptr())
-    _lib.check(rc, "wmd_loss_kitti_fwd")
+    _launch("loss_kitti_fwd", lambda: dict(n=n, h=h, w=w, scales=nl)).wmd_loss_kitti_fwd(
+        ctypes.byref(d), _lib.ptr(chint), _lib.ptr(warped), _lib.ptr(idsel), _lib.ptr(hpix), _lib.ptr(ws), ws.numel(),
+        _lib.ptr(terms), _lib.stream_ptr())
     return terms, chint, warped, idsel, hpix, ws
 
 
 def _kitti_bwd(t, scales, loss_scales, opt, warped, idsel, hpix, state, grad_terms):
     d = _desc(t, scales, loss_scales, opt)
-    lib = _lib.load()
     grads = [torch.empty_like(p) for p in t["disp"]]
     ptrs = (ctypes.c_void_p * len(grads))(*[_lib.ptr(g) for g in grads])
-    ws = torch.empty(int(lib.wmd_loss_kitti_bwd_ws_bytes(ctypes.byref(d))), dtype=torch.uint8, device=warped.device)
-    with _prof("loss_kitti_bwd", lambda: dict(n=d.N, h=d.H, w=d.W, scales=d.n_loss)):
-        rc = lib.wmd_loss_kitti_bwd(ctypes.byref(d), _lib.ptr(warped), _lib.ptr(idsel), _lib.ptr(hpix),
-                                    _lib.ptr(state), _lib.ptr(grad_terms), _lib.ptr(ws), ws.numel(), ptrs,
-                                    _lib.stream_ptr())
-    _lib.check(rc, "wmd_loss_kitti_bwd")
+    ws = torch.empty(int(_lib.load().wmd_loss_kitti_bwd_ws_bytes(ctypes.byref(d))), dtype=torch.uint8, device=warped.device)
+    _launch("loss_kitti_bwd", lambda: dict(n=d.N, h=d.H, w=d.W, scales=d.n_loss)).wmd_loss_kitti_bwd(
+        ctypes.byref(d), _lib.ptr(warped), _lib.ptr(idsel), _lib.ptr(hpix), _lib.ptr(state), _lib.ptr(grad_terms),
+        _lib.ptr(ws), ws.numel(), ptrs, _lib.stream_ptr())
     return grads
 
 

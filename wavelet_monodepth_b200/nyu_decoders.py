@@ -135,8 +135,7 @@ class _NyuWaveBase(_NyuPacks):
         """Dense decoders: the cuDNN module graph for depthwise variants and for training with TF32 allowed, the native
         training forward for training with fp32 convolutions, the native engine otherwise (no_grad / inference)."""
         _need_cuda(x_blocks)
-        needs_grad = torch.is_grad_enabled() and (
-            any(p.requires_grad for p in self.parameters()) or any(f.requires_grad for f in x_blocks))
+        needs_grad = _needs_grad(self, x_blocks)
         if self._depthwise or (needs_grad and not train_native.fp32_convs_requested()):
             return self._autograd_forward(x_blocks)
         if needs_grad:
@@ -146,6 +145,7 @@ class _NyuWaveBase(_NyuPacks):
         return out
 
     @torch.no_grad()
+    @ops._on_device
     def _native_forward(self, blocks, thresh_ratio, sparse):
         """conv2/up1 and the first level dense, then the levels of _LEVELS dense or on active lists.
 
@@ -154,13 +154,6 @@ class _NyuWaveBase(_NyuPacks):
         _need_cuda(blocks)
         if self._depthwise:
             raise NotImplementedError("depthwise-separable variants only run on the differentiable cuDNN path")
-        dev = blocks[-1].device
-        if dev.index is not None and dev.index != torch.cuda.current_device():
-            with torch.cuda.device(dev):       # libwmd launches on the current device
-                return self._native_forward_on_device(blocks, thresh_ratio, sparse)
-        return self._native_forward_on_device(blocks, thresh_ratio, sparse)
-
-    def _native_forward_on_device(self, blocks, thresh_ratio, sparse):
         out = {}
         xb = blocks[-1]
         n, _, h, w = xb.shape
@@ -373,14 +366,8 @@ class _BaselineDecoder(_NyuPacks):
         return self._native_forward(blocks)
 
     @torch.no_grad()
+    @ops._on_device
     def _native_forward(self, blocks):
-        dev = blocks[-1].device
-        if dev.index is not None and dev.index != torch.cuda.current_device():
-            with torch.cuda.device(dev):       # libwmd launches on the current device
-                return self._native_forward_on_device(blocks)
-        return self._native_forward_on_device(blocks)
-
-    def _native_forward_on_device(self, blocks):
         xb = blocks[4]
         n, c, h, w = (int(v) for v in xb.shape)
         up = 32 if self._extra_stage else 16

@@ -17,7 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from .ops import _dense, _on_device, _prof
+from .ops import _dense, _launch, _on_device
 
 _f64 = torch.float64
 METRICS = ("rel", "rms", "log_10", "a1", "a2", "a3")
@@ -44,13 +44,10 @@ def compute_errors_nyu(pred, gt):
         raise _lib.WmdError("compute_errors_nyu takes float tensors of equal size")
     pred, gt = _dense(pred.reshape(-1), _f64), _dense(gt.reshape(-1), _f64)
     n = pred.numel()
-    lib = _lib.load()
-    ws = torch.empty(int(lib.wmd_eval_nyu_errors_ws_bytes(n)), dtype=torch.uint8, device=pred.device)
+    ws = torch.empty(int(_lib.load().wmd_eval_nyu_errors_ws_bytes(n)), dtype=torch.uint8, device=pred.device)
     out = torch.empty(6, dtype=_f64, device=pred.device)
-    with _prof("eval_nyu_errors", lambda: dict(n=n)):
-        rc = lib.wmd_eval_nyu_errors_f64(_lib.ptr(pred), _lib.ptr(gt), n, _lib.ptr(ws), ws.numel(), _lib.ptr(out),
-                                         _lib.stream_ptr())
-    _lib.check(rc, "wmd_eval_nyu_errors_f64")
+    _launch("eval_nyu_errors", lambda: dict(n=n)).wmd_eval_nyu_errors_f64(
+        _lib.ptr(pred), _lib.ptr(gt), n, _lib.ptr(ws), ws.numel(), _lib.ptr(out), _lib.stream_ptr())
     return out
 
 
@@ -89,11 +86,9 @@ def _gt_sums(edges_np):
 def _edt(features, out):
     """wmd_eval_edt of (n, h, w) byte feature masks into `out` (n, h, w) fp64"""
     n, h, w = (int(v) for v in features.shape)
-    lib = _lib.load()
-    ws = torch.empty(int(lib.wmd_eval_edt_ws_bytes(n, h, w)), dtype=torch.uint8, device=features.device)
-    with _prof("eval_edt", lambda: dict(n=n, h=h, w=w)):
-        rc = lib.wmd_eval_edt(_lib.ptr(features), n, h, w, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
-    _lib.check(rc, "wmd_eval_edt")
+    ws = torch.empty(int(_lib.load().wmd_eval_edt_ws_bytes(n, h, w)), dtype=torch.uint8, device=features.device)
+    _launch("eval_edt", lambda: dict(n=n, h=h, w=w)).wmd_eval_edt(
+        _lib.ptr(features), n, h, w, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
     return out
 
 
@@ -104,14 +99,11 @@ def _edges_frames(pred, edges_gt, d_gt, gt_sums, scores, low, high):
     taps, bleed = _canny_filters(h, w, dev)
     edges_est = torch.empty((n, h, w), dtype=torch.bool, device=dev)
     d_est = torch.empty((n, h, w), dtype=_f64, device=dev)
-    lib = _lib.load()
-    ws = torch.empty(int(lib.wmd_eval_edges_ws_bytes(n, h, w)), dtype=torch.uint8, device=dev)
-    with _prof("eval_edges_frames", lambda: dict(n=n, h=h, w=w)):
-        rc = lib.wmd_eval_edges_frames(
-            _lib.ptr(pred), int(pred.dtype == _f64), n, h, w, _lib.ptr(taps), _lib.ptr(bleed), float(low), float(high),
-            _lib.ptr(edges_gt), _lib.ptr(d_gt), _lib.ptr(gt_sums), _lib.ptr(edges_est), _lib.ptr(d_est),
-            _lib.ptr(scores), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
-    _lib.check(rc, "wmd_eval_edges_frames")
+    ws = torch.empty(int(_lib.load().wmd_eval_edges_ws_bytes(n, h, w)), dtype=torch.uint8, device=dev)
+    _launch("eval_edges_frames", lambda: dict(n=n, h=h, w=w)).wmd_eval_edges_frames(
+        _lib.ptr(pred), int(pred.dtype == _f64), n, h, w, _lib.ptr(taps), _lib.ptr(bleed), float(low), float(high),
+        _lib.ptr(edges_gt), _lib.ptr(d_gt), _lib.ptr(gt_sums), _lib.ptr(edges_est), _lib.ptr(d_est), _lib.ptr(scores),
+        _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
     return edges_est, d_est
 
 
@@ -247,17 +239,14 @@ class NyuDepthEvaluator:
             return
         d = d.contiguous()
         f0 = self.next_frame
-        lib = _lib.load()
         with torch.cuda.device(self.device):
             if self.edges_gt is not None and depth_out is None:
                 depth_out = torch.empty((n,) + self.out_shape, dtype=_f64, device=self.device)
-            with _prof("eval_nyu_frames", lambda: dict(n=n, h=h, w=w)):
-                ws = torch.empty(int(lib.wmd_eval_nyu_ws_bytes(n, self.mode)), dtype=torch.uint8, device=self.device)
-                rc = lib.wmd_eval_nyu_frames(
-                    _lib.ptr(d), n, h, w, self.mode, int(self.use_disparity), _lib.ptr(self.gt[f0:]),
-                    _lib.ptr(self.gt_log10[f0:]), _lib.ptr(depth_out), _lib.ptr(ws), ws.numel(),
-                    _lib.ptr(self.sums[f0:]), _lib.stream_ptr())
-            _lib.check(rc, "wmd_eval_nyu_frames")
+            ws = torch.empty(int(_lib.load().wmd_eval_nyu_ws_bytes(n, self.mode)), dtype=torch.uint8, device=self.device)
+            _launch("eval_nyu_frames", lambda: dict(n=n, h=h, w=w)).wmd_eval_nyu_frames(
+                _lib.ptr(d), n, h, w, self.mode, int(self.use_disparity), _lib.ptr(self.gt[f0:]),
+                _lib.ptr(self.gt_log10[f0:]), _lib.ptr(depth_out), _lib.ptr(ws), ws.numel(), _lib.ptr(self.sums[f0:]),
+                _lib.stream_ptr())
             if self.edges_gt is not None:
                 _edges_frames(depth_out, self.edges_gt[f0:f0 + n], self.d_gt[f0:f0 + n],
                               self.edges_gt_sums[f0:f0 + n], self.edges_scores[f0:f0 + n], EDGE_LOW, EDGE_HIGH)

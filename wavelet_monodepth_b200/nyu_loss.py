@@ -15,7 +15,7 @@ import ctypes
 import torch
 
 from . import _lib
-from .ops import _dense, _on_device, _prof
+from .ops import _dense, _launch, _on_device
 from .wavelets import DWT
 
 SCALES = (0, 1, 2, 3)          # train.py: `for scale in range(4)`
@@ -33,13 +33,11 @@ def _loss_fwd(target, preds, log2s, means, want_signs):
     """means[:] = the terms of `preds` against `target` (N, 1, H, W); returns the int8 signs (or None)."""
     n, _, h, w = (int(v) for v in target.shape)
     dev = target.device
-    lib = _lib.load()
     signs = torch.empty((len(preds), n, h, w), dtype=torch.int8, device=dev) if want_signs else None
-    ws = torch.empty(int(lib.wmd_loss_nyu_ws_bytes(n, h, w, len(preds))), dtype=torch.uint8, device=dev)
-    with _prof("loss_nyu_fwd", lambda: dict(n=n, h=h, w=w, terms=len(preds))):
-        rc = lib.wmd_loss_nyu_fwd(_lib.ptr(target), n, h, w, _terms(preds, log2s), len(preds), _lib.ptr(signs),
-                                  _lib.ptr(ws), ws.numel(), _lib.ptr(means), _lib.stream_ptr())
-    _lib.check(rc, "wmd_loss_nyu_fwd")
+    ws = torch.empty(int(_lib.load().wmd_loss_nyu_ws_bytes(n, h, w, len(preds))), dtype=torch.uint8, device=dev)
+    _launch("loss_nyu_fwd", lambda: dict(n=n, h=h, w=w, terms=len(preds))).wmd_loss_nyu_fwd(
+        _lib.ptr(target), n, h, w, _terms(preds, log2s), len(preds), _lib.ptr(signs), _lib.ptr(ws), ws.numel(),
+        _lib.ptr(means), _lib.stream_ptr())
     return signs
 
 
@@ -47,11 +45,8 @@ def _loss_bwd(signs, target_shape, preds, log2s, grad_means):
     n, _, h, w = target_shape
     grads = [torch.empty_like(p) for p in preds]
     ptrs = (ctypes.c_void_p * len(grads))(*[_lib.ptr(g) for g in grads])
-    lib = _lib.load()
-    with _prof("loss_nyu_bwd", lambda: dict(n=n, h=h, w=w, terms=len(preds))):
-        rc = lib.wmd_loss_nyu_bwd(_lib.ptr(signs), n, h, w, _terms(preds, log2s), len(preds), _lib.ptr(grad_means),
-                                  ptrs, _lib.stream_ptr())
-    _lib.check(rc, "wmd_loss_nyu_bwd")
+    _launch("loss_nyu_bwd", lambda: dict(n=n, h=h, w=w, terms=len(preds))).wmd_loss_nyu_bwd(
+        _lib.ptr(signs), n, h, w, _terms(preds, log2s), len(preds), _lib.ptr(grad_means), ptrs, _lib.stream_ptr())
     return grads
 
 

@@ -5,6 +5,8 @@ its outputs with torch, passes raw pointers to libwmd on torch's current stream
 and returns tensors.  No arithmetic happens in torch here.
 """
 import ctypes
+import functools
+import itertools
 
 import torch
 
@@ -89,30 +91,29 @@ def _single_gpu():
     return _SINGLE[0]
 
 
+def _cuda_device(a):
+    """Device of `a` if it is a CUDA tensor, or of the first CUDA tensor in it if it is a list or tuple; else None."""
+    for t in (a if isinstance(a, (list, tuple)) else (a,)):
+        if torch.is_tensor(t) and t.is_cuda:
+            return t.device
+    return None
+
+
 def _on_device(fn):
-    """Run a wrapper with its tensors' device current.
+    """Run a wrapper (or a decoder's native forward) with its tensors' device current.
 
     libwmd launches on the CUDA *current* device (it caches per-device attributes by cudaGetDevice()) and on the
     stream handed in, so both must belong to the device that owns the buffers.  The first CUDA tensor among the
-    arguments decides; a decoder living on cuda:1 therefore works while cuda:0 is the process-wide current device."""
-    import functools
+    arguments decides, looking one level into lists and tuples (a decoder's feature maps, some of which may be pinned
+    host tensors); a decoder living on cuda:1 therefore works while cuda:0 is the process-wide current device."""
 
     @functools.wraps(fn)
     def wrapper(*args, **kwargs):
         if _single_gpu():                      # one visible device: it is always the current one
             return fn(*args, **kwargs)
-        dev = None
-        for a in args:
-            if torch.is_tensor(a) and a.is_cuda:
-                dev = a.device
-                break
-        if dev is None:
-            for a in kwargs.values():
-                if torch.is_tensor(a) and a.is_cuda:
-                    dev = a.device
-                    break
-            if dev is None and isinstance(kwargs.get("device"), torch.device) and kwargs["device"].type == "cuda":
-                dev = kwargs["device"]
+        dev = next((d for d in map(_cuda_device, itertools.chain(args, kwargs.values())) if d is not None), None)
+        if dev is None and isinstance(kwargs.get("device"), torch.device) and kwargs["device"].type == "cuda":
+            dev = kwargs["device"]
         if dev is None or dev.index is None or dev.index == torch.cuda.current_device():
             return fn(*args, **kwargs)
         with torch.cuda.device(dev):
@@ -163,6 +164,28 @@ class _prof:
         return False
 
 
+class _launch:
+    """_launch(prof, info).<symbol>(*args): call the status-returning libwmd entry point <symbol>, timed as `prof` (see
+    _prof) when given, and raise WmdError naming <symbol> if it fails.  The symbol that is called is the one the error
+    names.  The library is looked up on every call, never cached."""
+    __slots__ = ("prof", "info")
+
+    def __init__(self, prof=None, info=None):
+        self.prof, self.info = prof, info
+
+    def __getattr__(self, symbol):
+        fn = getattr(_lib.load(), symbol)
+
+        def call(*args):
+            if self.prof is None:
+                rc = fn(*args)
+            else:
+                with _prof(self.prof, self.info):
+                    rc = fn(*args)
+            _lib.check(rc, symbol)
+        return call
+
+
 # --------------------------------------------------------------------------- Haar
 def _epilogue_args(epilogue, like):
     """(mode, a, b, lo, hi, out0, out1, names) of a consumer epilogue spec; see head_idwt."""
@@ -185,7 +208,6 @@ def idwt_haar(ll, hf, disp_scale=None, clamp01=False, epilogue=None):
     """ll (N,C,H,W), hf (N,C,3,H,W) -> out (N,C,2H,2W) [, disp = clamp?(out*disp_scale)] [, epilogue planes].
 
     epilogue (consumer of the last level, see head_idwt): returns the extra plane(s) after out / disp."""
-    lib = _lib.load()
     ll, hf = _dense(ll), _dense(hf)
     n, c, h, w = ll.shape
     if tuple(hf.shape) != (n, c, 3, h, w):
@@ -197,48 +219,42 @@ def idwt_haar(ll, hf, disp_scale=None, clamp01=False, epilogue=None):
     ret = (out,) + ((disp,) if disp_scale is not None else ()) + extra
     if out.numel() == 0:
         return ret if len(ret) > 1 else out
-    with _prof('idwt_haar', lambda: dict(n=n, c=c, h=h, w=w, disp=disp is not None)):
-        if mode == _lib.EPI_NONE:
-            rc = lib.wmd_idwt_haar_f32(_lib.ptr(ll), _lib.ptr(hf), _lib.ptr(out), _lib.ptr(disp),
-                                       float(disp_scale if disp_scale is not None else 1.0), int(bool(clamp01)),
-                                       n, c, h, w, _lib.stream_ptr())
-        else:
-            rc = lib.wmd_idwt_haar_epi_f32(_lib.ptr(ll), _lib.ptr(hf), _lib.ptr(out), _lib.ptr(disp),
-                                           float(disp_scale if disp_scale is not None else 1.0), int(bool(clamp01)),
-                                           mode, ea, eb, elo, ehi, _lib.ptr(e0), _lib.ptr(e1), n, c, h, w, _lib.stream_ptr())
-    _lib.check(rc, "wmd_idwt_haar_f32")
+    launch = _launch("idwt_haar", lambda: dict(n=n, c=c, h=h, w=w, disp=disp is not None))
+    scale = float(disp_scale if disp_scale is not None else 1.0)
+    if mode == _lib.EPI_NONE:
+        launch.wmd_idwt_haar_f32(_lib.ptr(ll), _lib.ptr(hf), _lib.ptr(out), _lib.ptr(disp), scale, int(bool(clamp01)),
+                                 n, c, h, w, _lib.stream_ptr())
+    else:
+        launch.wmd_idwt_haar_epi_f32(_lib.ptr(ll), _lib.ptr(hf), _lib.ptr(out), _lib.ptr(disp), scale, int(bool(clamp01)),
+                                     mode, ea, eb, elo, ehi, _lib.ptr(e0), _lib.ptr(e1), n, c, h, w, _lib.stream_ptr())
     return ret if len(ret) > 1 else out
 
 
 @_on_device
 def idwt_bilinear(ll, hf, size, disp_scale=1.0, clamp01=False, align_corners=False):
     """Fused IDWT -> disp = [clamp](out*disp_scale) -> bilinear resize to `size` (F.interpolate semantics)."""
-    lib = _lib.load()
     ll, hf = _dense(ll), _dense(hf)
     n, c, h, w = ll.shape
     full = torch.empty((n, c, int(size[0]), int(size[1])), dtype=_f32, device=ll.device)
     if full.numel() == 0:
         return full
-    with _prof('idwt_bilinear', lambda: dict(n=n, c=c, h=h, w=w, fh=int(size[0]), fw=int(size[1]))):
-        rc = lib.wmd_idwt_bilinear_f32(_lib.ptr(ll), _lib.ptr(hf), _lib.ptr(full), float(disp_scale), int(bool(clamp01)),
-                                       int(size[0]), int(size[1]), int(bool(align_corners)), n, c, h, w, _lib.stream_ptr())
-    _lib.check(rc, "wmd_idwt_bilinear_f32")
+    _launch("idwt_bilinear", lambda: dict(n=n, c=c, h=h, w=w, fh=int(size[0]), fw=int(size[1]))).wmd_idwt_bilinear_f32(
+        _lib.ptr(ll), _lib.ptr(hf), _lib.ptr(full), float(disp_scale), int(bool(clamp01)), int(size[0]), int(size[1]),
+        int(bool(align_corners)), n, c, h, w, _lib.stream_ptr())
     return full
 
 
 @_on_device
 def dwt_haar(x):
     """x (N,C,H,W) even H,W -> ll (N,C,H/2,W/2), hf (N,C,3,H/2,W/2)."""
-    lib = _lib.load()
     x = _dense(x)
     n, c, h, w = x.shape
     ll = torch.empty((n, c, h // 2, w // 2), dtype=_f32, device=x.device)
     hf = torch.empty((n, c, 3, h // 2, w // 2), dtype=_f32, device=x.device)
     if x.numel() == 0:
         return ll, hf
-    with _prof('dwt_haar', lambda: dict(n=n, c=c, h=h, w=w)):
-        rc = lib.wmd_dwt_haar_f32(_lib.ptr(x), _lib.ptr(ll), _lib.ptr(hf), n, c, h, w, _lib.stream_ptr())
-    _lib.check(rc, "wmd_dwt_haar_f32")
+    _launch("dwt_haar", lambda: dict(n=n, c=c, h=h, w=w)).wmd_dwt_haar_f32(
+        _lib.ptr(x), _lib.ptr(ll), _lib.ptr(hf), n, c, h, w, _lib.stream_ptr())
     return ll, hf
 
 
@@ -246,18 +262,14 @@ def dwt_haar(x):
 @_on_device
 def range_thresh(x, ratio, return_minmax=False):
     """Per-sample (max - min) * ratio over everything but dim 0 -> (N,) fp32 on device."""
-    lib = _lib.load()
     x = _dense(x)
     n = x.shape[0]
     per = x.numel() // max(n, 1)
     thresh = torch.empty((n,), dtype=_f32, device=x.device)
     mm = torch.empty((n, 2), dtype=_f32, device=x.device) if return_minmax else None
-    nbytes = lib.wmd_range_ws_bytes(n, per)
-    ws = _scratch.range(x.device, nbytes)
-    with _prof('range_thresh', lambda: dict(n=n, per=per)):
-        rc = lib.wmd_range_thresh_f32(_lib.ptr(x), n, per, float(ratio), _lib.ptr(thresh), _lib.ptr(mm),
-                                      _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
-    _lib.check(rc, "wmd_range_thresh_f32")
+    ws = _scratch.range(x.device, _lib.load().wmd_range_ws_bytes(n, per))
+    _launch("range_thresh", lambda: dict(n=n, per=per)).wmd_range_thresh_f32(
+        _lib.ptr(x), n, per, float(ratio), _lib.ptr(thresh), _lib.ptr(mm), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
     return (thresh, mm) if return_minmax else thresh
 
 
@@ -266,7 +278,6 @@ def level_masks(yh, thresh, n=None, h=None, w=None, device=None, want=("S0", "S1
     """yh (N,3,H,W) or (N,1,3,H,W), thresh (N,) or None (all ones; then pass n,h,w,device).
 
     Returns dict of uint8 (N,1,H,W) [S0-S2] / (N,1,2H,2W) [S3-S5] tensors."""
-    lib = _lib.load()
     if thresh is not None:
         yh = _dense(yh)
         n, h, w = yh.shape[0], yh.shape[-2], yh.shape[-1]
@@ -281,10 +292,8 @@ def level_masks(yh, thresh, n=None, h=None, w=None, device=None, want=("S0", "S1
             ptrs.append(_lib.ptr(out[k]))
         else:
             ptrs.append(None)
-    with _prof('level_masks', lambda: dict(n=n, h=h, w=w, thresh=thresh is not None)):
-        rc = lib.wmd_level_masks(_lib.ptr(yh) if thresh is not None else None, _lib.ptr(thresh), *ptrs, n, h, w,
-                                 _lib.stream_ptr())
-    _lib.check(rc, "wmd_level_masks")
+    _launch("level_masks", lambda: dict(n=n, h=h, w=w, thresh=thresh is not None)).wmd_level_masks(
+        _lib.ptr(yh) if thresh is not None else None, _lib.ptr(thresh), *ptrs, n, h, w, _lib.stream_ptr())
     return out
 
 
@@ -295,21 +304,19 @@ def compact(mask, want_idxmap=True, want_pixels=True, stream=None, ws_slot=0):
     stream: optional side stream to run on (it first waits for the current stream, which produced `mask`); then returns
     ((idxmap, pixels, offsets), event) and the consumer stream must wait for the event.  Outputs are allocated on the
     current stream.  ws_slot: workspace to use - concurrent compactions must not share one."""
-    lib = _lib.load()
     mask = _dense(mask, _u8)
     n, h, w = mask.shape[0], mask.shape[-2], mask.shape[-1]
     dev = mask.device
     idxmap = torch.empty((n, h, w), dtype=_i32, device=dev) if want_idxmap else None
     pixels = torch.empty((n * h * w,), dtype=_i32, device=dev) if want_pixels else None
     offsets = torch.empty((n + 1,), dtype=_i32, device=dev)
-    nbytes = lib.wmd_compact_ws_bytes(n, h, w)
-    ws = _scratch.compact(dev, nbytes, ws_slot)
+    ws = _scratch.compact(dev, _lib.load().wmd_compact_ws_bytes(n, h, w), ws_slot)
 
     def launch():
-        with _prof('compact_mask', lambda: dict(n=n, h=h, w=w, idxmap=idxmap is not None, pixels=pixels is not None, offsets=offsets)):
-            rc = lib.wmd_compact_mask(_lib.ptr(mask), _lib.ptr(idxmap), _lib.ptr(pixels), _lib.ptr(offsets), n, h, w,
-                                      _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
-        _lib.check(rc, "wmd_compact_mask")
+        info = lambda: dict(n=n, h=h, w=w, idxmap=idxmap is not None, pixels=pixels is not None, offsets=offsets)   # noqa: E731
+        _launch("compact_mask", info).wmd_compact_mask(
+            _lib.ptr(mask), _lib.ptr(idxmap), _lib.ptr(pixels), _lib.ptr(offsets), n, h, w, _lib.ptr(ws), ws.numel(),
+            _lib.stream_ptr())
 
     if stream is None:
         launch()
@@ -325,12 +332,10 @@ def compact(mask, want_idxmap=True, want_pixels=True, stream=None, ws_slot=0):
 @_on_device
 def gate_map(gate, idxmap=None):
     """int32 map: gate ? (idxmap or linear index) : -1, shaped like gate without the channel dim."""
-    lib = _lib.load()
     gate = _dense(gate, _u8)
     out = torch.empty((gate.shape[0], gate.shape[-2], gate.shape[-1]), dtype=_i32, device=gate.device)
-    with _prof('gate_map', lambda: dict(count=gate.numel())):
-        rc = lib.wmd_gate_map(_lib.ptr(gate), _lib.ptr(idxmap), _lib.ptr(out), gate.numel(), _lib.stream_ptr())
-    _lib.check(rc, "wmd_gate_map")
+    _launch("gate_map", lambda: dict(count=gate.numel())).wmd_gate_map(
+        _lib.ptr(gate), _lib.ptr(idxmap), _lib.ptr(out), gate.numel(), _lib.stream_ptr())
     return out
 
 
@@ -354,20 +359,16 @@ def amax_rows(x, out, mask=None):
     """out (1-element device tensor, pre-zeroed or holding a lower bound) = max(out, max |x| over the finite x; NaN and
     +-Inf are skipped): for sources no libwmd kernel produced (channels_last maps used in place).  mask: optional uint8
     tensor of one byte per row of x (contiguous); then only the marked rows count - the rows the consumer reads."""
-    lib = _lib.load()
+    info = lambda: dict(count=x.numel())   # noqa: E731
     if mask is None:
-        with _prof('amax', lambda: dict(count=x.numel())):
-            rc = lib.wmd_amax_f32(_lib.ptr(x, _f32), x.numel(), _lib.ptr(out, _f32), _lib.stream_ptr())
-        _lib.check(rc, "wmd_amax_f32")
+        _launch("amax", info).wmd_amax_f32(_lib.ptr(x, _f32), x.numel(), _lib.ptr(out, _f32), _lib.stream_ptr())
         return out
     mask = _dense(mask, _u8)
     if not x.is_contiguous() or mask.numel() != x.shape[0]:
         raise _lib.WmdError("amax_rows: contiguous rows and one mask byte per row (%d rows, %d mask bytes)"
                             % (x.shape[0], mask.numel()))
-    with _prof('amax', lambda: dict(count=x.numel())):
-        rc = lib.wmd_amax_rows_masked_f32(_lib.ptr(x, _f32), x.shape[0], x.shape[1], _lib.ptr(mask), _lib.ptr(out, _f32),
-                                          _lib.stream_ptr())
-    _lib.check(rc, "wmd_amax_rows_masked_f32")
+    _launch("amax", info).wmd_amax_rows_masked_f32(
+        _lib.ptr(x, _f32), x.shape[0], x.shape[1], _lib.ptr(mask), _lib.ptr(out, _f32), _lib.stream_ptr())
     return out
 
 
@@ -382,7 +383,6 @@ def nchw_to_rows(x, ld=None, gate=None, amax=None, amax_mask=None):
     amax: optional 1-element device tensor raised to max |x| over the pixels the consumer reads: the gate's, else those
     of amax_mask (same form as gate; it restricts only the maximum, every row is still produced), else the whole map.
     So a sparse level's skip map reports one maximum whichever way it is moved (plain, gated, list gather, in place)."""
-    lib = _lib.load()
     n, c, h, w = x.shape
     ld = pad4(c) if ld is None else ld
     on_host = not x.is_cuda
@@ -411,21 +411,20 @@ def nchw_to_rows(x, ld=None, gate=None, amax=None, amax_mask=None):
         x = _dense(x)
     rows = torch.empty((n * h * w, ld), dtype=_f32, device=dev)
     marked = _pm_count(gate)
-    with _prof('nchw_to_rows', lambda: dict(n=n, c=c, hw=h * w, ld=ld, marked=marked, host=on_host)):
-        if gate is None and amax is not None and max_mask is not None:
-            rc = lib.wmd_nchw_to_rows_masked_amax_f32(_lib.ptr(x), _lib.ptr(rows), _lib.ptr(max_mask), n, c, h * w, ld,
-                                                      _lib.ptr(amax, _f32), _lib.stream_ptr())
-        elif gate is None and amax is not None:
-            rc = lib.wmd_nchw_to_rows_amax_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.ptr(amax, _f32), _lib.stream_ptr())
-        elif gate is None:
-            rc = lib.wmd_nchw_to_rows_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.stream_ptr())
-        elif amax is not None:
-            rc = lib.wmd_nchw_to_rows_gated_amax_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
-                                                     _lib.ptr(amax, _f32), _lib.stream_ptr())
-        else:
-            rc = lib.wmd_nchw_to_rows_gated_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
-                                                _lib.stream_ptr())
-    _lib.check(rc, "wmd_nchw_to_rows_f32")
+    launch = _launch("nchw_to_rows", lambda: dict(n=n, c=c, hw=h * w, ld=ld, marked=marked, host=on_host))
+    if gate is None and amax is not None and max_mask is not None:
+        launch.wmd_nchw_to_rows_masked_amax_f32(_lib.ptr(x), _lib.ptr(rows), _lib.ptr(max_mask), n, c, h * w, ld,
+                                                _lib.ptr(amax, _f32), _lib.stream_ptr())
+    elif gate is None and amax is not None:
+        launch.wmd_nchw_to_rows_amax_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.ptr(amax, _f32), _lib.stream_ptr())
+    elif gate is None:
+        launch.wmd_nchw_to_rows_f32(_lib.ptr(x), _lib.ptr(rows), n, c, h * w, ld, _lib.stream_ptr())
+    elif amax is not None:
+        launch.wmd_nchw_to_rows_gated_amax_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
+                                               _lib.ptr(amax, _f32), _lib.stream_ptr())
+    else:
+        launch.wmd_nchw_to_rows_gated_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), _lib.ptr(gate), n, c, h * w, ld,
+                                          _lib.stream_ptr())
     return rows
 
 
@@ -438,40 +437,35 @@ def _pm_count(gate):
 
 @_on_device
 def rows_to_nchw(rows, n, c, h, w):
-    lib = _lib.load()
     rows = _dense(rows)
     out = torch.empty((n, c, h, w), dtype=_f32, device=rows.device)
-    with _prof('rows_to_nchw', lambda: dict(n=n, c=c, hw=h * w)):
-        rc = lib.wmd_rows_to_nchw_f32(_lib.ptr(rows), _lib.ptr(out), n, c, h * w, rows.shape[1], _lib.stream_ptr())
-    _lib.check(rc, "wmd_rows_to_nchw_f32")
+    _launch("rows_to_nchw", lambda: dict(n=n, c=c, hw=h * w)).wmd_rows_to_nchw_f32(
+        _lib.ptr(rows), _lib.ptr(out), n, c, h * w, rows.shape[1], _lib.stream_ptr())
     return out
 
 
 @_on_device
 def gather_rows(x_nchw, pixels, count, max_rows=None, ld=None):
     """rows[m] = x[n, :, y, x] at the listed pixels (pixels/count None = every pixel)."""
-    lib = _lib.load()
     x = _dense(x_nchw)
     n, c, h, w = x.shape
     ld = pad4(c) if ld is None else ld
     max_rows = n * h * w if max_rows is None else max_rows
     rows = torch.zeros((max(max_rows, 1), ld), dtype=_f32, device=x.device)
-    rc = lib.wmd_gather_rows_nchw_f32(_lib.ptr(x), _lib.ptr(rows), ld, c, _lib.ptr(pixels), _lib.ptr(count),
-                                      max_rows, n, h, w, _lib.stream_ptr())
-    _lib.check(rc, "wmd_gather_rows_nchw_f32")
+    _launch().wmd_gather_rows_nchw_f32(
+        _lib.ptr(x), _lib.ptr(rows), ld, c, _lib.ptr(pixels), _lib.ptr(count), max_rows, n, h, w, _lib.stream_ptr())
     return rows
 
 
 @_on_device
 def gather_rows_list(x, pixels, count, ld=None, stream=None, amax=None):
-    """Compact rows of the listed pixels of an NCHW map: rows[m] = x[n, :, y, x] for pixels[m] (wmd_gather_rows_list_f32).
+    """Compact rows of the listed pixels of an NCHW map: rows[m] = x[n, :, y, x] for pixels[m] (wmd_gather_rows_list_amax_f32).
 
     x: (N,C,H,W) CUDA tensor or PINNED HOST tensor (read in place over PCIe: only the listed pixels cross the bus).
     pixels / count: list + device count from `compact`.  Returns rows (N*H*W capacity, ld); rows past *count are
     uninitialised.  stream: optional side stream to run the gather on (it first waits for the current stream, which
     produced `pixels` / `count`).  Then returns (rows, event): the consumer stream must wait for `event`.  The output is
     allocated on the current stream, whose later work is what reads it."""
-    lib = _lib.load()
     n, c, h, w = x.shape
     ld = pad4(c) if ld is None else ld
     on_host = not x.is_cuda
@@ -484,11 +478,10 @@ def gather_rows_list(x, pixels, count, ld=None, stream=None, amax=None):
     rows = torch.empty((max(n * h * w, 1), ld), dtype=_f32, device=dev)
 
     def launch():
-        with _prof('gather_rows_list', lambda: dict(c=c, ld=ld, count=count, max_rows=n * h * w, host=on_host)):
-            rc = lib.wmd_gather_rows_list_amax_f32(_lib.host_ptr(x, _f32), _lib.ptr(rows), ld, c, _lib.ptr(pixels, _i32),
-                                                   _lib.ptr(count, _i32), n * h * w, n, h, w, _lib.ptr(amax, _f32),
-                                                   _lib.stream_ptr())
-        _lib.check(rc, "wmd_gather_rows_list_f32")
+        info = lambda: dict(c=c, ld=ld, count=count, max_rows=n * h * w, host=on_host)   # noqa: E731
+        _launch("gather_rows_list", info).wmd_gather_rows_list_amax_f32(
+            _lib.host_ptr(x, _f32), _lib.ptr(rows), ld, c, _lib.ptr(pixels, _i32), _lib.ptr(count, _i32), n * h * w, n,
+            h, w, _lib.ptr(amax, _f32), _lib.stream_ptr())
 
     if stream is None:
         launch()
@@ -504,14 +497,13 @@ def gather_rows_list(x, pixels, count, ld=None, stream=None, amax=None):
 @_on_device
 def scatter_rows(rows, c, pixels, count, n, h, w, max_rows=None, out=None):
     """Dense (N,C,H,W), zero except at the listed pixels where it takes rows[m, :c]."""
-    lib = _lib.load()
     rows = _dense(rows)
     if out is None:
         out = torch.zeros((n, c, h, w), dtype=_f32, device=rows.device)
     max_rows = min(rows.shape[0], n * h * w) if max_rows is None else max_rows
-    rc = lib.wmd_scatter_rows_nchw_f32(_lib.ptr(rows), rows.shape[1], c, _lib.ptr(pixels), _lib.ptr(count),
-                                       max_rows, _lib.ptr(out), n, h, w, _lib.stream_ptr())
-    _lib.check(rc, "wmd_scatter_rows_nchw_f32")
+    _launch().wmd_scatter_rows_nchw_f32(
+        _lib.ptr(rows), rows.shape[1], c, _lib.ptr(pixels), _lib.ptr(count), max_rows, _lib.ptr(out), n, h, w,
+        _lib.stream_ptr())
     return out
 
 
@@ -569,18 +561,16 @@ def pack_weight(weight, c1=0, kind=None, precision="f16x3"):
     if kind == "tc":
         nfl = lib.wmd_conv_tc_weight_floats(cout, c0, c1, taps)
         packed = torch.empty((nfl,), dtype=_f32, device=wt.device)
-        rc = lib.wmd_pack_conv_weight_tc_f32(_lib.ptr(wt), _lib.ptr(packed), cout, c0, c1, taps, _lib.stream_ptr())
-        _lib.check(rc, "wmd_pack_conv_weight_tc_f32")
+        _launch().wmd_pack_conv_weight_tc_f32(_lib.ptr(wt), _lib.ptr(packed), cout, c0, c1, taps, _lib.stream_ptr())
         packed16 = None
         if precision == "f16x3":
             packed16 = torch.empty((lib.wmd_conv_tc16_weight_bytes(cout, c0, c1, taps),), dtype=_u8, device=wt.device)
-            rc = lib.wmd_pack_conv_weight_tc16_f32(_lib.ptr(wt), _lib.ptr(packed16), cout, c0, c1, taps, _lib.stream_ptr())
-            _lib.check(rc, "wmd_pack_conv_weight_tc16_f32")
+            _launch().wmd_pack_conv_weight_tc16_f32(
+                _lib.ptr(wt), _lib.ptr(packed16), cout, c0, c1, taps, _lib.stream_ptr())
         return PackedW(packed, "tc", taps, c0, c1, cout, packed16)
     ldw = pad4(cout)
     packed = torch.empty((taps * cin, ldw), dtype=_f32, device=wt.device)
-    rc = lib.wmd_pack_conv_weight_f32(_lib.ptr(wt), _lib.ptr(packed), cout, cin, taps, ldw, _lib.stream_ptr())
-    _lib.check(rc, "wmd_pack_conv_weight_f32")
+    _launch().wmd_pack_conv_weight_f32(_lib.ptr(wt), _lib.ptr(packed), cout, cin, taps, ldw, _lib.stream_ptr())
     return PackedW(packed, "simt", taps, c0, c1, cout)
 
 
@@ -597,7 +587,6 @@ def conv_rows(x0, c0, wpacked, bias, cout, n, h, w, taps=9, pad=PAD_REFLECT, act
     x0: rows (R0, ld0); x1: optional dense rows (N*H*W, ld1); wpacked: PackedW from pack_weight(weight, c1).
     Returns y rows (max_rows, pad4(cout)).
     """
-    lib = _lib.load()
     dev = x0.device
     total = n * h * w
     max_rows = total if max_rows is None else int(max_rows)
@@ -636,14 +625,11 @@ def conv_rows(x0, c0, wpacked, bias, cout, n, h, w, taps=9, pad=PAD_REFLECT, act
     if wpacked.kind == "tc":
         ws = None
         if splits != 1:
-            ws = _scratch.splitk(dev, lib.wmd_conv_tc_splitk_ws_bytes(max_rows, out.shape[1], splits))
-        with _prof('conv_rows_tc', info):
-            rc = lib.wmd_conv_rows_tc_splitk_f32(ctypes.byref(d), splits, _lib.ptr(ws), ws.numel() * 4 if ws is not None else 0,
-                                                 _lib.stream_ptr())
+            ws = _scratch.splitk(dev, _lib.load().wmd_conv_tc_splitk_ws_bytes(max_rows, out.shape[1], splits))
+        _launch("conv_rows_tc", info).wmd_conv_rows_tc_splitk_f32(
+            ctypes.byref(d), splits, _lib.ptr(ws), ws.numel() * 4 if ws is not None else 0, _lib.stream_ptr())
     else:
-        with _prof('conv_rows', info):
-            rc = lib.wmd_conv_rows_f32(ctypes.byref(d), _lib.stream_ptr())
-    _lib.check(rc, "wmd_conv_rows_%sf32" % ("tc_" if wpacked.kind == "tc" else ""))
+        _launch("conv_rows", info).wmd_conv_rows_f32(ctypes.byref(d), _lib.stream_ptr())
     return out
 
 
@@ -654,18 +640,16 @@ def act_backward(y, dy, cout, act, act_param=0.0, want_bias=True, amax=None):
 
     Returns (dz rows (R, pad4(cout)), db (cout,) summed over the rows in a fixed order, or None).  amax: optional
     1-element device tensor raised to max |dz|."""
-    lib = _lib.load()
     y, dy = _dense(y), _dense(dy)
     rows = y.shape[0]
     dev = y.device
     dz = torch.empty((rows, pad4(cout)), dtype=_f32, device=dev)
     db = torch.empty((cout,), dtype=_f32, device=dev) if want_bias else None
-    ws = _scratch.bwd(dev, lib.wmd_act_bwd_ws_bytes(rows, cout)) if want_bias else None
-    with _prof('act_bwd', lambda: dict(rows=rows, cout=cout, act=act)):
-        rc = lib.wmd_act_bwd_f32(_lib.ptr(y), y.shape[1], _lib.ptr(dy), dy.shape[1], rows, cout, act, float(act_param),
-                                 _lib.ptr(dz), dz.shape[1], _lib.ptr(db), _lib.ptr(amax, _f32), _lib.ptr(ws),
-                                 ws.numel() if ws is not None else 0, _lib.stream_ptr())
-    _lib.check(rc, "wmd_act_bwd_f32")
+    ws = _scratch.bwd(dev, _lib.load().wmd_act_bwd_ws_bytes(rows, cout)) if want_bias else None
+    _launch("act_bwd", lambda: dict(rows=rows, cout=cout, act=act)).wmd_act_bwd_f32(
+        _lib.ptr(y), y.shape[1], _lib.ptr(dy), dy.shape[1], rows, cout, act, float(act_param), _lib.ptr(dz),
+        dz.shape[1], _lib.ptr(db), _lib.ptr(amax, _f32), _lib.ptr(ws), ws.numel() if ws is not None else 0,
+        _lib.stream_ptr())
     return dz, db
 
 
@@ -683,17 +667,15 @@ def _bwd_desc(x0, c0, cout, n, h, w, taps, pad, map0, shift0, x1, c1):
 def conv_wgrad(x0, c0, dz, cout, n, h, w, taps=9, pad=PAD_REFLECT, map0=None, shift0=0, x1=None, c1=0):
     """Weight gradient (cout, c0 + c1, k, k) of a dense gather-GEMM convolution (wmd_conv_wgrad_f32): the sources are
     the forward's (x0 / map0 / shift0 rows, dense x1 rows), dz the rows of the pre-activation gradient."""
-    lib = _lib.load()
     dz = _dense(dz)
     k = 3 if taps == 9 else 1
     dw = torch.empty((cout, c0 + c1, k, k), dtype=_f32, device=dz.device)
     d = _bwd_desc(x0, c0, cout, n, h, w, taps, pad, map0, shift0, x1, c1)
-    nbytes = lib.wmd_conv_wgrad_ws_bytes(ctypes.byref(d))
+    nbytes = _lib.load().wmd_conv_wgrad_ws_bytes(ctypes.byref(d))
     ws = _scratch.bwd(dz.device, nbytes) if nbytes else None
-    with _prof('conv_wgrad', lambda: dict(n=n, h=h, w=w, taps=taps, c0=c0, c1=c1, cout=cout)):
-        rc = lib.wmd_conv_wgrad_f32(ctypes.byref(d), _lib.ptr(dz), dz.shape[1], _lib.ptr(dw), _lib.ptr(ws),
-                                    ws.numel() if ws is not None else 0, _lib.stream_ptr())
-    _lib.check(rc, "wmd_conv_wgrad_f32")
+    _launch("conv_wgrad", lambda: dict(n=n, h=h, w=w, taps=taps, c0=c0, c1=c1, cout=cout)).wmd_conv_wgrad_f32(
+        ctypes.byref(d), _lib.ptr(dz), dz.shape[1], _lib.ptr(dw), _lib.ptr(ws), ws.numel() if ws is not None else 0,
+        _lib.stream_ptr())
     return dw
 
 
@@ -720,7 +702,6 @@ def conv_dgrad(dz, cout, wt_packed, c0, n, h, w, taps=9, pad=PAD_REFLECT, shift0
     launch on dz; 3x3 layers run the forward contract over the grid extended by one pixel on each side under zero padding
     (map0 = ring_map into the dz rows), then wmd_conv_dgrad_fold_f32 folds the ring by the pad mode, sums the 2x2 children of
     a shift0 = 1 source and writes the source-1 columns to NCHW.  amax: max |dz| (device scalar) for the fp16-pair form."""
-    lib = _lib.load()
     cin = c0 + c1
     if taps == 1:
         if shift0 or c1:
@@ -733,10 +714,9 @@ def conv_dgrad(dz, cout, wt_packed, c0, n, h, w, taps=9, pad=PAD_REFLECT, shift0
     dx0 = torch.empty((n * (h >> shift0) * (w >> shift0), pad4(c0)), dtype=_f32, device=dz.device)
     c1w = c1 if want_x1 else 0
     dx1 = torch.empty((n, c1, h, w), dtype=_f32, device=dz.device) if c1w else None
-    with _prof('conv_dgrad_fold', lambda: dict(n=n, h=h, w=w, c0=c0, c1=c1w, shift0=shift0)):
-        rc = lib.wmd_conv_dgrad_fold_f32(_lib.ptr(g), g.shape[1], n, h, w, pad, c0, shift0, _lib.ptr(dx0), dx0.shape[1], c1w,
-                                         _lib.ptr(dx1), _lib.stream_ptr())
-    _lib.check(rc, "wmd_conv_dgrad_fold_f32")
+    _launch("conv_dgrad_fold", lambda: dict(n=n, h=h, w=w, c0=c0, c1=c1w, shift0=shift0)).wmd_conv_dgrad_fold_f32(
+        _lib.ptr(g), g.shape[1], n, h, w, pad, c0, shift0, _lib.ptr(dx0), dx0.shape[1], c1w, _lib.ptr(dx1),
+        _lib.stream_ptr())
     return dx0, dx1
 
 
@@ -747,18 +727,17 @@ def head_mlp_supported(c, n1):
 @_on_device
 def pack_head_mlp(w1, b1, wz):
     """(n1, c, 1, 1) 1x1 weight, (n1,) bias, (nz, n1, 1, 1) tap-product weight -> packed image for head_mlp."""
-    lib = _lib.load()
     w1, wz = _dense(w1.detach()), _dense(wz.detach())
     n1, c, nz = int(w1.shape[0]), int(w1.shape[1]), int(wz.shape[0])
     if int(wz.shape[1]) != n1:
         raise _lib.WmdError("pack_head_mlp: wz expects %d inputs, w1 produces %d" % (wz.shape[1], n1))
-    nfl = lib.wmd_head_mlp_weight_floats(c, n1)
+    nfl = _lib.load().wmd_head_mlp_weight_floats(c, n1)
     if nfl == 0:
         raise _lib.WmdError("head_mlp: unsupported shape c=%d n1=%d" % (c, n1))
     packed = torch.empty((nfl,), dtype=_f32, device=w1.device)
-    rc = lib.wmd_pack_head_mlp_f32(_lib.ptr(w1), _lib.ptr(wz), _lib.ptr(_dense(b1.detach()) if b1 is not None else None),
-                                   c, n1, nz, _lib.ptr(packed), _lib.stream_ptr())
-    _lib.check(rc, "wmd_pack_head_mlp_f32")
+    _launch().wmd_pack_head_mlp_f32(
+        _lib.ptr(w1), _lib.ptr(wz), _lib.ptr(_dense(b1.detach()) if b1 is not None else None), c, n1, nz,
+        _lib.ptr(packed), _lib.stream_ptr())
     return packed
 
 
@@ -766,7 +745,6 @@ def pack_head_mlp(w1, b1, wz):
 def pack_disp_tail16(w1, b1, w2, b2):
     """upconv(0,1)'s (16, 16, 3, 3) weight and bias, dispconv(0)'s (cout <= 4, 16, 3, 3) weight and bias -> the packed
     image of disp_tail16 (wmd_pack_disp_tail16_f32)."""
-    lib = _lib.load()
     w1, w2 = _dense(w1.detach()), _dense(w2.detach())
     cout = int(w2.shape[0])
     if tuple(w1.shape) != (16, 16, 3, 3) or tuple(w2.shape[1:]) != (16, 3, 3) or not 1 <= cout <= 4:
@@ -775,9 +753,8 @@ def pack_disp_tail16(w1, b1, w2, b2):
     packed = torch.empty((_lib.DISP_TAIL16_PACKED_FLOATS,), dtype=_f32, device=w1.device)
     b1 = _dense(b1.detach()) if b1 is not None else None
     b2 = _dense(b2.detach()) if b2 is not None else None
-    rc = lib.wmd_pack_disp_tail16_f32(_lib.ptr(w1), _lib.ptr(b1), _lib.ptr(w2), _lib.ptr(b2), cout, _lib.ptr(packed),
-                                      _lib.stream_ptr())
-    _lib.check(rc, "wmd_pack_disp_tail16_f32")
+    _launch().wmd_pack_disp_tail16_f32(
+        _lib.ptr(w1), _lib.ptr(b1), _lib.ptr(w2), _lib.ptr(b2), cout, _lib.ptr(packed), _lib.stream_ptr())
     return packed
 
 
@@ -785,28 +762,23 @@ def pack_disp_tail16(w1, b1, w2, b2):
 def disp_tail16(x, packed, cout, n, h, w, out=None):
     """("disp", 0) of the baseline KITTI decoder from upconv(0,0)'s rows x (N*h*w, ld >= 16) at half resolution:
     sigmoid(dispconv(0)(ELU(upconv(0,1)(up2(x))))) -> (N, cout, 2h, 2w); see wmd_disp_tail16_f32."""
-    lib = _lib.load()
     if out is None:
         out = torch.empty((n, cout, 2 * h, 2 * w), dtype=_f32, device=x.device)
     if n == 0:
         return out
-    with _prof('disp_tail16', lambda: dict(n=n, h=h, w=w, cout=cout)):
-        rc = lib.wmd_disp_tail16_f32(_lib.ptr(x, _f32), x.shape[1], _lib.ptr(packed, _f32), cout, _lib.ptr(out, _f32), n, h, w,
-                                     _lib.stream_ptr())
-    _lib.check(rc, "wmd_disp_tail16_f32")
+    _launch("disp_tail16", lambda: dict(n=n, h=h, w=w, cout=cout)).wmd_disp_tail16_f32(
+        _lib.ptr(x, _f32), x.shape[1], _lib.ptr(packed, _f32), cout, _lib.ptr(out, _f32), n, h, w, _lib.stream_ptr())
     return out
 
 
 @_on_device
 def head_mlp(x, c, packed, n1, slope=0.1, count=None, max_rows=None, nz=54):
     """z (max_rows, 56) = Wz . lrelu(W1 . x + b1) on pixel-major rows x (R, ld >= c); see wmd_head_mlp_f32."""
-    lib = _lib.load()
     max_rows = x.shape[0] if max_rows is None else int(max_rows)
     z = torch.empty((max(max_rows, 1), 56), dtype=_f32, device=x.device)
-    with _prof('head_mlp', lambda: dict(c=c, n1=n1, nz=nz, count=count, max_rows=max_rows)):
-        rc = lib.wmd_head_mlp_f32(_lib.ptr(x, _f32), x.shape[1], c, _lib.ptr(packed, _f32), n1, float(slope),
-                                  _lib.ptr(count, _i32), max_rows, _lib.ptr(z), 56, _lib.stream_ptr())
-    _lib.check(rc, "wmd_head_mlp_f32")
+    _launch("head_mlp", lambda: dict(c=c, n1=n1, nz=nz, count=count, max_rows=max_rows)).wmd_head_mlp_f32(
+        _lib.ptr(x, _f32), x.shape[1], c, _lib.ptr(packed, _f32), n1, float(slope), _lib.ptr(count, _i32), max_rows,
+        _lib.ptr(z), 56, _lib.stream_ptr())
     return z
 
 
@@ -816,7 +788,6 @@ def head_conv3x3(t, c, off_a, wa, ba, n, h, w, cout, scale=1.0, act=ACT_NONE, pa
     """3x3 stage of the coefficient heads -> dense (N,cout,H,W); see wmd_head_conv3x3_f32.
 
     wa/wb: packed (9*c, cout) exactly (no padding: use pack_head_weight)."""
-    lib = _lib.load()
     dev = t.device
     total = n * h * w
     max_rows = total if max_rows is None else int(max_rows)
@@ -830,21 +801,18 @@ def head_conv3x3(t, c, off_a, wa, ba, n, h, w, cout, scale=1.0, act=ACT_NONE, pa
     d.cout, d.pad_mode, d.act, d.scale = cout, pad, act, float(scale)
     d.pixels, d.count, d.max_rows = _lib.ptr(pixels, _i32), _lib.ptr(count, _i32), max_rows
     d.out = _lib.ptr(out, _f32)
-    with _prof('head_conv3x3', lambda: dict(n=n, h=h, w=w, c=c, cout=cout, dual=off_b >= 0, count=count, max_rows=max_rows)):
-        rc = lib.wmd_head_conv3x3_f32(ctypes.byref(d), _lib.stream_ptr())
-    _lib.check(rc, "wmd_head_conv3x3_f32")
+    info = lambda: dict(n=n, h=h, w=w, c=c, cout=cout, dual=off_b >= 0, count=count, max_rows=max_rows)   # noqa: E731
+    _launch("head_conv3x3", info).wmd_head_conv3x3_f32(ctypes.byref(d), _lib.stream_ptr())
     return out
 
 
 @_on_device
 def pack_head_weight(weight):
     """(cout<=4, c, 3, 3) -> (9*c, cout) contiguous, the layout wmd_head_conv3x3_f32 stages in shared memory."""
-    lib = _lib.load()
     wt = _dense(weight.detach())
     cout, cin = wt.shape[0], wt.shape[1]
     packed = torch.empty((9 * cin, cout), dtype=_f32, device=wt.device)
-    rc = lib.wmd_pack_conv_weight_f32(_lib.ptr(wt), _lib.ptr(packed), cout, cin, 9, cout, _lib.stream_ptr())
-    _lib.check(rc, "wmd_pack_conv_weight_f32")
+    _launch().wmd_pack_conv_weight_f32(_lib.ptr(wt), _lib.ptr(packed), cout, cin, 9, cout, _lib.stream_ptr())
     return packed
 
 
@@ -869,18 +837,17 @@ def head_gather(z, groups, bias, n, h, w, cout, scale=1.0, act=ACT_NONE, dual=Fa
     """Sum the nine per-tap products of z (rows x >= 9*groups) around every output pixel -> dense (N,cout,H,W).
 
     col0: first column of z that belongs to this head (its nine [tap][group] blocks start there)."""
-    lib = _lib.load()
     if col0 < 0 or col0 + 9 * groups > z.shape[1]:
         raise _lib.WmdError("head_gather: columns %d..%d do not fit rows of %d" % (col0, col0 + 9 * groups, z.shape[1]))
     total = n * h * w
     max_rows = total if max_rows is None else int(max_rows)
     if out is None:
         out = (torch.zeros if pixels is not None else torch.empty)((n, cout, h, w), dtype=_f32, device=z.device)
-    with _prof('head_gather', lambda: dict(n=n, h=h, w=w, groups=groups, cout=cout, count=count, max_rows=max_rows)):
-        rc = lib.wmd_head_gather_f32(_lib.ptr(z, _f32) + 4 * col0, z.shape[1], groups, _lib.ptr(idxmap, _i32), _lib.ptr(bias, _f32),
-                                     float(scale), act, int(bool(dual)), pad, _lib.ptr(pixels, _i32), _lib.ptr(count, _i32),
-                                     max_rows, _lib.ptr(out, _f32), cout, n, h, w, _lib.stream_ptr())
-    _lib.check(rc, "wmd_head_gather_f32")
+    info = lambda: dict(n=n, h=h, w=w, groups=groups, cout=cout, count=count, max_rows=max_rows)   # noqa: E731
+    _launch("head_gather", info).wmd_head_gather_f32(
+        _lib.ptr(z, _f32) + 4 * col0, z.shape[1], groups, _lib.ptr(idxmap, _i32), _lib.ptr(bias, _f32), float(scale),
+        act, int(bool(dual)), pad, _lib.ptr(pixels, _i32), _lib.ptr(count, _i32), max_rows, _lib.ptr(out, _f32), cout,
+        n, h, w, _lib.stream_ptr())
     return out
 
 
@@ -894,7 +861,6 @@ def head_idwt(z, bias, yl, scale, disp_scale, idxmap=None, mask=None, pad=PAD_RE
     thresh (N,) if thresh_ratio is not None, plus the epilogue's planes).
     epilogue: None | ("disp_to_depth", min_depth, max_depth) -> "scaled_disp", "depth" (KITTI/layers.py:16-25)
                    | ("div_clamp", div, lo, hi)  (lo/hi None = no clamp) -> "depth" (NYUv2/utils.py:219,229)."""
-    lib = _lib.load()
     yl = _dense(yl)
     n, _, h, w = yl.shape
     dev = yl.device
@@ -919,10 +885,10 @@ def head_idwt(z, bias, yl, scale, disp_scale, idxmap=None, mask=None, pad=PAD_RE
     if thresh_ratio is not None:
         res["thresh"] = torch.empty((n,), dtype=_f32, device=dev)
         d.thresh, d.thresh_ratio = _lib.ptr(res["thresh"]), float(thresh_ratio)
-        ws = _scratch.range(dev, lib.wmd_head_idwt_ws_bytes(n, h, w))
+        ws = _scratch.range(dev, _lib.load().wmd_head_idwt_ws_bytes(n, h, w))
     if n == 0:
         return res
-    with _prof('head_idwt', lambda: dict(n=n, h=h, w=w, mask=mask, epi=d.epi_mode, thresh=thresh_ratio is not None)):
-        rc = lib.wmd_head_idwt_f32(ctypes.byref(d), _lib.ptr(ws), ws.numel() if ws is not None else 0, _lib.stream_ptr())
-    _lib.check(rc, "wmd_head_idwt_f32")
+    info = lambda: dict(n=n, h=h, w=w, mask=mask, epi=d.epi_mode, thresh=thresh_ratio is not None)   # noqa: E731
+    _launch("head_idwt", info).wmd_head_idwt_f32(
+        ctypes.byref(d), _lib.ptr(ws), ws.numel() if ws is not None else 0, _lib.stream_ptr())
     return res
