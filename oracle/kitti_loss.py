@@ -8,7 +8,8 @@ Two modes:
   * ``contract``: the device's fp32 rounding points (the warped colours, the three per-pixel losses before the argmin,
     the noise term, the reported terms); everything else in fp64 with the device's operation order, so the device's
     bits are expected within one fp32 ulp of this (sums differ from the device's in order only);
-  * ``fp64``: no rounding point at all, to hold the hand-written adjoint to torch autograd of the float64 reference.
+  * ``fp64``: no rounding point at all but the reference's own (its float32 mask counts: ``_count``), to hold the
+    hand-written adjoint to torch autograd of the float64 reference.
 
 ``run(...)`` returns the terms, the warped colours, the masks and (optionally) the gradient of the total with respect to
 each ("disp", s).  The adjoint is the same gather the device computes: per-centre SSIM coefficients, a 3x3 gather over
@@ -16,6 +17,8 @@ the reflected windows, the bilinear sample's derivative in its coordinates (0 wh
 coordinate exactly on the border), the projection's closed-form derivative in depth, disp_to_depth, the upsample's
 adjoint and the smoothness term with its per-frame mean.
 """
+import os
+
 import numpy as np
 
 SCALES = (0, 1, 2, 3)
@@ -31,6 +34,12 @@ f64, f32 = np.float64, np.float32
 
 def _r32(x, contract):
     return x.astype(f32).astype(f64) if contract else x
+
+
+def _count(m, contract):
+    """a masked mean's denominator, mask count + 1e-7: fp64 on the device (contract); in the reference the masks are
+    float32 even in its float64 run, so the count and its + 1e-7 are float32, where 1e-7 rounds away from a count >= 1"""
+    return m + MASK_EPS if contract else float(f32(m) + f32(MASK_EPS))
 
 
 def _axis_taps(n_in, n_out):
@@ -221,7 +230,8 @@ def smooth(disp, img):
     gx = nd[:, :, :-1] - nd[:, :, 1:]
     gy = nd[:, :-1, :] - nd[:, 1:, :]
     cx, cy = N * h * (w - 1), N * (h - 1) * w
-    val = (np.abs(gx) * ex).sum() / cx + (np.abs(gy) * ey).sum() / cy
+    with np.errstate(invalid="ignore"):       # one row or one column: the mean over no edges is NaN, as torch's is
+        val = (np.abs(gx) * ex).sum() / cx + (np.abs(gy) * ey).sum() / cy
     G = np.zeros_like(d)                                            # d val / d nd
     tx, ty = np.sign(gx) * ex / cx, np.sign(gy) * ey / cy
     G[:, :, :-1] += tx
@@ -238,7 +248,8 @@ def run(inputs, disps, noise, scales=SCALES, loss_scales=SCALES, min_depth=0.1, 
     """inputs: "target" color(0, 0) and "source" color("s", 0) (N, 3, H, W), "colors" {s: color(0, s)}, "K", "inv_K",
     "stereo_T" (N, 4, 4), "depth_hint", "depth_hint_mask" (N, 1, H, W); disps {s: (N, 1, H >> s, W >> s)};
     noise {s: (N, 1, H, W) float32 standard normals}.  Returns a dict of the terms ("reproj_loss/s", ...), "warped"
-    {s}, "color_depth_hint", "identity_selection" {s}, "depth_hint_pixels" {s} and, with grads, "grad" {s} of "loss"."""
+    {s}, "color_depth_hint", "identity_selection" {s}, "depth_hint_pixels" {s} and, with grads, "grad" {s} of "loss",
+    or of sum_k grad_terms[k] terms[k] (terms in term_keys(loss_scales) order) when grad_terms is given."""
     c = mode == "contract"
     tgt, src = inputs["target"].astype(f64), inputs["source"].astype(f64)
     N, _, H, W = tgt.shape
@@ -271,10 +282,10 @@ def run(inputs, disps, noise, scales=SCALES, loss_scales=SCALES, min_depth=0.1, 
         rm, hm = (k != 1).astype(f64), (k == 2).astype(f64)
         out["identity_selection"][s] = 1.0 - rm
         out["depth_hint_pixels"][s] = hm
-        M, Mh = rm.sum(), hm.sum()
-        t_rep = _r32(np.asarray((r * rm).sum() / (M + MASK_EPS)), c)
+        M, Mh = _count(rm.sum(), c), _count(hm.sum(), c)
+        t_rep = _r32(np.asarray((r * rm).sum() / M), c)
         diff = D - hint
-        t_hint = _r32(np.asarray((np.log(np.abs(diff) + 1.0) * hmask * hm).sum() / (Mh + MASK_EPS)), c)
+        t_hint = _r32(np.asarray((np.log(np.abs(diff) + 1.0) * hmask * hm).sum() / Mh), c)
         sm, sgrad = smooth(disps[s], inputs["colors"][s])
         loss_s = _r32(np.asarray(t_rep + t_hint + disparity_smoothness * sm / 2 ** s), c)
         out["reproj_loss/%d" % s], out["depth_hint_loss/%d" % s], out["loss/%d" % s] = t_rep, t_hint, loss_s
@@ -290,9 +301,9 @@ def run(inputs, disps, noise, scales=SCALES, loss_scales=SCALES, min_depth=0.1, 
         gl = gt[0] / len(scales) + gt[3 + 3 * i]
         g_rep, g_hint, g_sm = gl + gt[1 + 3 * i], gl + gt[2 + 3 * i], gl * disparity_smoothness / 2 ** s
         D, scaled, dix, diy, sdx, sdy, warped, rm, hm, M, Mh, diff, sgrad = per[s]
-        dx = reproj_adjoint(warped, tgt, rm * (g_rep / (M + MASK_EPS)))          # d L / d warped
+        dx = reproj_adjoint(warped, tgt, rm * (g_rep / M))          # d L / d warped
         dD = (dx * (sdx * dix[:, None] + sdy * diy[:, None])).sum(1)
-        dD = dD + (g_hint / (Mh + MASK_EPS)) * hmask * hm * np.sign(diff) / (np.abs(diff) + 1.0)
+        dD = dD + (g_hint / Mh) * hmask * hm * np.sign(diff) / (np.abs(diff) + 1.0)
         dup = dD * -((1.0 / min_depth - 1.0 / max_depth) * D * D)
         h, w = disps[s].shape[2:]
         gd = upsample_adjoint(dup, h, w) + g_sm * sgrad
@@ -300,13 +311,96 @@ def run(inputs, disps, noise, scales=SCALES, loss_scales=SCALES, min_depth=0.1, 
     return out
 
 
-# fixture cases: 2-frame batches at the two KITTI training sizes, a designed special split, and a loss_scales subset
+OPTIONS = dict(min_depth=0.1, max_depth=100.0, disparity_smoothness=1e-3)      # options.py's defaults
+
+
+def options(case):
+    """the case's min_depth, max_depth and disparity_smoothness (options.py's defaults where it sets none)"""
+    return {k: case.get(k, v) for k, v in OPTIONS.items()}
+
+
+def term_keys(loss_scales):
+    """the terms in the device's order: "loss", then per loss scale reproj_loss, depth_hint_loss and loss/s"""
+    return ["loss"] + [k % s for s in loss_scales for k in ("reproj_loss/%d", "depth_hint_loss/%d", "loss/%d")]
+
+
+def term_weights(loss_scales):
+    """a weight per term for the weighted-term gradients: 1/2 on the total, and (1 + t + 3 s) / 8 on term t of scale s
+    with the sign (-1)^(t + s), so that no two terms of a scale or scales of a term share a weight (all exact in fp32)"""
+    return (0.5,) + tuple((-1.0) ** (t + s) * (1 + t + 3 * s) / 8.0 for s in loss_scales for t in range(3))
+
+
+def _case(**kw):
+    kw.setdefault("scales", SCALES)
+    kw.setdefault("loss_scales", SCALES)
+    kw["weights"] = term_weights(kw["loss_scales"])
+    return kw
+
+
+# fixture cases: 2-frame batches at the two KITTI training sizes, a designed special split, a loss_scales subset; a
+# different camera per frame (rotated stereo transforms with y and z baselines), non-default options, odd low-resolution
+# shapes, one-pixel-thick scale-3 maps (1 row, 1 column: the smoothness has no edge in that direction) and one frame
 CASES = {
-    "r96x320": dict(seed=1000, N=2, H=96, W=320, scales=SCALES, loss_scales=SCALES),
-    "r192x640": dict(seed=2000, N=2, H=192, W=640, scales=SCALES, loss_scales=SCALES),
-    "subset": dict(seed=3000, N=2, H=96, W=320, scales=SCALES, loss_scales=(0, 2)),
-    "special": dict(seed=4000, N=2, H=64, W=96, scales=SCALES, loss_scales=SCALES, random=False, special=True),
+    "r96x320": _case(seed=1000, N=2, H=96, W=320),
+    "r192x640": _case(seed=2000, N=2, H=192, W=640),
+    "subset": _case(seed=3000, N=2, H=96, W=320, loss_scales=(0, 2)),
+    "special": _case(seed=4000, N=2, H=64, W=96, random=False, special=True),
+    "camera": _case(seed=5000, N=3, H=48, W=128, camera=True, fixture=3),
+    "options": _case(seed=6000, N=2, H=64, W=192, loss_scales=(1, 3), min_depth=0.5, max_depth=80.0,
+                     disparity_smoothness=0.1, fixture=2),
+    "odd": _case(seed=7000, N=3, H=72, W=136, camera=True, fixture=3),
+    "thin_row": _case(seed=8000, N=2, H=8, W=64, fixture=2),
+    "thin_col": _case(seed=9000, N=2, H=64, W=8, fixture=2),
+    "single": _case(seed=10000, N=1, H=64, W=192, fixture=2),
 }
+# the fixture's files under tests/golden, each well under 1 MiB: the first four cases as they were first pinned, their
+# weighted-term gradients (and weights), the cases added with those gradients (options and shapes, then cameras)
+FIXTURES = ("kitti_hints_loss.npz", "kitti_hints_loss_terms.npz", "kitti_hints_loss_shapes.npz",
+            "kitti_hints_loss_cameras.npz")
+FIRST_CASES = ("r96x320", "r192x640", "subset", "special")
+
+
+def fixture_file(key):
+    """which of FIXTURES holds fixture key `key` ("<case>/...")"""
+    case, _, rest = key.partition("/")
+    if case not in FIRST_CASES:
+        return FIXTURES[CASES[case]["fixture"]]
+    return FIXTURES[1] if rest == "weights" or rest.startswith("f64/wgrad/") else FIXTURES[0]
+
+
+def load_fixture(directory):
+    """every key of the fixture's files in `directory` as one dict; "cases" lists each file's cases in FIXTURES order"""
+    out, cases = {}, []
+    for name in FIXTURES:
+        with np.load(os.path.join(directory, name)) as f:
+            for k in f.files:
+                if k == "cases":
+                    cases += [str(c) for c in f[k]]
+                else:
+                    out[k] = f[k]
+    out["cases"] = np.array(cases)
+    return out
+
+
+def cameras(N, H, W):
+    """per-frame intrinsics as crops and rescales of KITTI's give them (focal lengths and principal points differ per
+    frame), their inverses, and stereo transforms with a rotation of 3-7 degrees about each axis and a translation with
+    x, y and z components, the signs alternating per frame: warps leave the image on all four sides, every z stays > 0"""
+    K = np.zeros((N, 4, 4), np.float32)
+    T = np.zeros((N, 4, 4), np.float32)
+    for n in range(N):
+        sg, grow = (1.0 if n % 2 == 0 else -1.0), 1.0 + 0.25 * n
+        fx, fy = 0.58 * W * (1.0 + 0.2 * n), 1.92 * H * (1.0 + 0.1 * n)
+        cx, cy = W * (0.5 + 0.04 * sg * (n + 1)), H * (0.5 - 0.06 * sg * (n + 1))
+        K[n] = [[fx, 0, cx, 0], [0, fy, cy, 0], [0, 0, 1, 0], [0, 0, 0, 1]]
+        ax, ay, az = np.radians([3.0 * sg * grow, -2.5 * sg * grow, 4.0 * sg * grow])
+        rx = np.array([[1, 0, 0], [0, np.cos(ax), -np.sin(ax)], [0, np.sin(ax), np.cos(ax)]])
+        ry = np.array([[np.cos(ay), 0, np.sin(ay)], [0, 1, 0], [-np.sin(ay), 0, np.cos(ay)]])
+        rz = np.array([[np.cos(az), -np.sin(az), 0], [np.sin(az), np.cos(az), 0], [0, 0, 1]])
+        T[n, :3, :3] = rz @ ry @ rx
+        T[n, :3, 3] = [0.1 * sg, 0.04 * sg * grow, -0.02 * sg * grow]
+        T[n, 3, 3] = 1.0
+    return K, np.linalg.pinv(K).astype(np.float32), T
 
 
 def intrinsics(N, H, W):
@@ -323,7 +417,7 @@ def make_inputs(case, seed):
     rng = np.random.default_rng(seed)
     N, H, W = case["N"], case["H"], case["W"]
     r = lambda *s: rng.random(s, dtype=np.float32)                                     # noqa: E731
-    K, inv_K, T = intrinsics(N, H, W)
+    K, inv_K, T = (cameras if case.get("camera") else intrinsics)(N, H, W)
     inp = {"target": r(N, 3, H, W), "K": K, "inv_K": inv_K, "stereo_T": T,
            "depth_hint": (1.0 + 40.0 * r(N, 1, H, W)).astype(np.float32),
            "depth_hint_mask": (r(N, 1, H, W) < 0.8).astype(np.float32)}
@@ -359,13 +453,16 @@ def draw_noise(seed, inputs, loss_scales):
 
 
 def decision_margin(inputs, disps, noise, case):
-    """the smallest relative distance, in fp64, of any argmin or grid-sample floor from its decision"""
-    out = run(inputs, disps, noise, case["scales"], case["loss_scales"], mode="fp64", grads=False)
+    """the smallest relative distance, in fp64, of any argmin or grid-sample floor from its decision (exact ties
+    excepted)"""
+    opt = options(case)
+    out = run(inputs, disps, noise, case["scales"], case["loss_scales"], mode="fp64", grads=False, **opt)
     tgt, src = inputs["target"].astype(f64), inputs["source"].astype(f64)
     N, _, H, W = tgt.shape
     worst = np.inf
     hint = inputs["depth_hint"][:, 0].astype(f64)
-    ds = [hint] + [depth_from_disp(upsample(disps[s], H, W), 0.1, 100.0)[1] for s in case["loss_scales"]]
+    ds = [hint] + [depth_from_disp(upsample(disps[s], H, W), opt["min_depth"], opt["max_depth"])[1]
+                   for s in case["loss_scales"]]
     for D in ds:
         ix, iy, _, _ = project(D, inputs["K"], inputs["inv_K"], inputs["stereo_T"])
         for v, n in ((ix, W), (iy, H)):
@@ -379,5 +476,10 @@ def decision_margin(inputs, disps, noise, case):
         r = reproj(out["warped"][s], tgt, False)
         ids = ident + (noise[s][:, 0] * NOISE_SCALE).astype(f64)
         st = np.sort(np.stack([r, ids, hl]), 0)
-        worst = min(worst, ((st[1] - st[0]) / np.maximum(np.abs(st[0]), 1e-30)).min())
+        # an exact tie does not count: r and the hint loss of a pixel whose scale and hint warps both leave the image
+        # past the same corner read the same clamped colours, and every precision decides that tie alike (first minimum)
+        gap = st[1] - st[0]
+        gap = gap[gap != 0]
+        if gap.size:
+            worst = min(worst, (gap / np.maximum(np.abs(st[0][st[1] != st[0]]), 1e-30)).min())
     return worst

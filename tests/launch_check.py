@@ -1,16 +1,16 @@
 """Launch-checking harness: every libwmd launch a workload makes, checked against the fp64 contract of its kernel.
 
 `Harness(monkeypatch)` wraps the entry points of ENTRY_POINTS, (owner, attribute) pairs whose owner is a module or a
-class: the public functions of wavelet_monodepth_b200.ops, and the evaluation and loss entry points of nyu_loss, nyu_eval
-and kitti_eval.  The decoders, train_native and wavelets call `ops.<name>` through the module, calls inside a module
-(conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows, _NyuLossFn -> _loss_fwd / _loss_bwd, NyuDepthEvaluator.add ->
-_edges_frames) resolve through its globals, and methods through their class, so wrapping the owners' attributes catches
-every call, nested ones included.
+class: the public functions of wavelet_monodepth_b200.ops, and the evaluation and loss entry points of nyu_loss, nyu_eval,
+kitti_eval and kitti_loss.  The decoders, train_native and wavelets call `ops.<name>` through the module, calls inside a
+module (conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows, _NyuLossFn -> _loss_fwd / _loss_bwd, _KittiLossFn ->
+_kitti_fwd / _kitti_bwd, NyuDepthEvaluator.add -> _edges_frames) resolve through its globals, and methods through their
+class, so wrapping the owners' attributes catches every call, nested ones included.
 
 Each call runs the original function, synchronises (compactions and list gathers run on side streams), recomputes the
 result from the call's actual inputs with the references of the kernel contract tests (conv_ref, head_ref, disp_tail_ref,
-conv_grad_ref, oracle.haar, oracle.nyu_loss, oracle.nyu_eval, oracle.nyu_edges, oracle.kitti_eval, plain torch
-restatements of the wmd.h comments: none of them uses ops or libwmd) and compares at that kernel's bar.  It also checks
+conv_grad_ref, oracle.haar, oracle.nyu_loss, oracle.nyu_eval, oracle.nyu_edges, oracle.kitti_eval, oracle.kitti_loss,
+plain torch restatements of the wmd.h comments: none of them uses ops or libwmd) and compares at that kernel's bar.  It also checks
 the preconditions a launch's contract relies on: source maxima that cover what an fp16-pair launch reads, exact amax
 outputs, index maps inside their sources, strictly increasing pixel lists, and count <= max_rows.  Pack calls record the
 plain weights behind each packed object; a pack is right when every launch that uses it is right.  State a checker needs
@@ -29,10 +29,11 @@ import torch.nn.functional as F
 
 from oracle import haar as ohaar
 from oracle import kitti_eval as oke
+from oracle import kitti_loss as okl
 from oracle import nyu_edges as ne
 from oracle import nyu_eval as one
 from oracle import nyu_loss as onl
-from wavelet_monodepth_b200 import _lib, kitti_eval, nyu_eval, nyu_loss, ops
+from wavelet_monodepth_b200 import _lib, kitti_eval, kitti_loss, nyu_eval, nyu_loss, ops
 
 import conv_grad_ref
 import conv_ref as cr
@@ -52,7 +53,8 @@ EVAL_LOSS = ((nyu_loss, "_loss_fwd"), (nyu_loss, "_loss_bwd"),
              (nyu_eval, "compute_errors_nyu"), (nyu_eval, "_edt"), (nyu_eval, "_edges_frames"),
              (nyu_eval.NyuDepthEvaluator, "add"),
              (kitti_eval, "compute_errors"), (kitti_eval, "batch_post_process_disparity"),
-             (kitti_eval.KittiDepthEvaluator, "__init__"), (kitti_eval.KittiDepthEvaluator, "add"))
+             (kitti_eval.KittiDepthEvaluator, "__init__"), (kitti_eval.KittiDepthEvaluator, "add"),
+             (kitti_loss, "_kitti_fwd"), (kitti_loss, "_kitti_bwd"))
 ENTRY_POINTS = tuple((ops, name) for name in CHECKED) + EVAL_LOSS
 
 
@@ -70,7 +72,8 @@ def hook(prefix, entry):
     return prefix + entry.replace(".__init__", ".init").strip("_").replace(".", "_")
 
 
-# every symbol of _lib.SIGNATURES, EVAL_SIGNATURES and LOSS_SIGNATURES: ("launch", entry point whose checker covers it) |
+# every symbol of _lib.SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES and KITTI_LOSS_SIGNATURES: ("launch", entry point
+# whose checker covers it) |
 # ("pack", ops entry point) | "query"
 SYMBOLS = {
     "wmd_version": "query", "wmd_status_string": "query", "wmd_last_cuda_error": "query", "wmd_launch_count": "query",
@@ -140,14 +143,20 @@ SYMBOLS = {
     "wmd_loss_nyu_ws_bytes": "query",
     "wmd_loss_nyu_fwd": ("launch", "_loss_fwd"),
     "wmd_loss_nyu_bwd": ("launch", "_loss_bwd"),
+    # include/wmd_loss_kitti.h
+    "wmd_loss_kitti_ws_bytes": "query",
+    "wmd_loss_kitti_bwd_ws_bytes": "query",
+    "wmd_loss_kitti_fwd": ("launch", "_kitti_fwd"),
+    "wmd_loss_kitti_bwd": ("launch", "_kitti_bwd"),
 }
 
 # bars of the checks this file adds on top of the contract tests' (units of 2^-24 of the element's scale)
 DWT_ULP = 8            # four roundings on each path of a one-level analysis bound the error by 4 x 2^-24 S; twice that
 ACT_BWD_ULP = 4        # dz = dy act'(y): at most three roundings (sigmoid: 1 - y, y (1 - y), the product with dy)
 # bars of the evaluation and loss checks: those of their own tests (test_gpu_nyu_loss, test_gpu_nyu_eval,
-# test_gpu_nyu_edges, test_gpu_kitti_eval)
+# test_gpu_nyu_edges, test_gpu_kitti_eval, test_gpu_kitti_loss)
 LOSS_MEAN_ULP = 1      # a loss term: the device's fp64 sum and the oracle's differ in order only, one fp32 rounding apart
+KITTI_GRAD_ULP = 1     # a KITTI loss gradient: fp64 sums rounded once, within one fp32 ulp of its scale's largest
 EVAL_REL = 1e-12       # fp64 sums of a fixed order against math.fsum / numpy's pairwise sums
 NYU_SUM_ABS = 1e-15    # per pixel: the fp64 log10's ulp, all a log_10 sum of equal depths is made of
 POST_REL = 1e-15       # batch_post_process_disparity: numpy's expression, evaluated in the same precision
@@ -802,6 +811,70 @@ class Harness:
                 _require(False, "%s: _loss_bwd term %d (%dx%d from %dx%d): %d gradients differ, worst %.3g ulp"
                          % (self.current, k, h, w, H, W, int(bad.sum()), worst))
         _record("_loss_bwd", "fp64", "bits", worst, 0, n * H * W * len(a["preds"]))
+
+    # ------------------------------------------------------------------------------------------ KITTI training loss
+    def _kitti_oracle(self, a, grads):
+        """oracle.kitti_loss.run in contract mode on the call's own inputs, noise, options and (backward) grad_terms"""
+        t, loss_scales = a["t"], tuple(a["loss_scales"])
+        inp = {k: _np(t[k]) for k in ("target", "source", "K", "inv_K", "stereo_T", "depth_hint", "depth_hint_mask")}
+        inp["colors"] = {s: _np(c) for s, c in zip(loss_scales, t["color"])}
+        disps = {s: _np(d) for s, d in zip(loss_scales, t["disp"])}
+        noise = {s: _np(z) for s, z in zip(loss_scales, t["noise"])}
+        min_depth, max_depth, smooth = a["opt"]
+        gt = _np(a["grad_terms"]) if grads else None
+        return okl.run(inp, disps, noise, tuple(a["scales"]), loss_scales, min_depth=min_depth, max_depth=max_depth,
+                       disparity_smoothness=smooth, grads=grads, grad_terms=gt)
+
+    def _kitti_masks(self, entry, o, loss_scales, idsel, hpix):
+        for i, s in enumerate(loss_scales):
+            for key, m in (("identity_selection", idsel), ("depth_hint_pixels", hpix)):
+                bad = int((_np(m[i])[:, 0] != o[key][s]).sum())
+                _require(bad == 0, "%s: %s scale %d: %d mask pixels differ from oracle.kitti_loss" % (entry, key, s, bad))
+
+    def _check_kitti_fwd(self, a, res, pre):
+        """oracle.kitti_loss.run (contract mode): color_depth_hint, the warped colours and both masks bit for bit; the
+        terms within LOSS_MEAN_ULP fp32 ulp, NaN exactly where the oracle's are"""
+        terms, chint, warped, idsel, hpix, _ = res
+        loss_scales = tuple(a["loss_scales"])
+        o = self._kitti_oracle(a, False)
+        _require(np.array_equal(_np(chint), o["color_depth_hint"].astype(np.float32), equal_nan=True),
+                 "%s: _kitti_fwd: color_depth_hint differs from oracle.kitti_loss" % self.current)
+        for i, s in enumerate(loss_scales):
+            _require(np.array_equal(_np(warped[i]), o["warped"][s].astype(np.float32), equal_nan=True),
+                     "%s: _kitti_fwd: the warped colours of scale %d differ from oracle.kitti_loss" % (self.current, s))
+        self._kitti_masks("%s: _kitti_fwd" % self.current, o, loss_scales, idsel, hpix)
+        got = _np(terms)
+        worst = 0.0
+        for k, key in enumerate(okl.term_keys(loss_scales)):
+            want = float(o[key])
+            _require(np.isnan(got[k]) == np.isnan(want), "_kitti_fwd: %s is %r, want %r" % (key, got[k], want))
+            if not np.isnan(want):
+                worst = max(worst, float(_ulps(got[k], want)))
+        n, _, H, W = a["t"]["target"].shape
+        _record("_kitti_fwd", "fp64", "ulp+masks", worst, LOSS_MEAN_ULP, n * H * W * len(loss_scales))
+        _require(worst <= LOSS_MEAN_ULP, "%s: _kitti_fwd term %.3g fp32 ulp > %d" % (self.current, worst, LOSS_MEAN_ULP))
+
+    def _check_kitti_bwd(self, a, grads, pre):
+        """oracle.kitti_loss.run (contract mode) with the call's grad_terms, on masks equal to the call's: each gradient
+        element within KITTI_GRAD_ULP fp32 ulp of its scale's largest, NaN exactly where the oracle's are"""
+        loss_scales = tuple(a["loss_scales"])
+        o = self._kitti_oracle(a, True)
+        self._kitti_masks("%s: _kitti_bwd" % self.current, o, loss_scales, a["idsel"], a["hpix"])
+        worst = 0.0
+        for i, s in enumerate(loss_scales):
+            got, want = _np(grads[i]).astype(np.float64), o["grad"][s]
+            nan = np.isnan(want)
+            _require(np.array_equal(np.isnan(got), nan), "%s: _kitti_bwd scale %d: %d NaN gradients, want %d"
+                     % (self.current, s, int(np.isnan(got).sum()), int(nan.sum())))
+            if nan.all():
+                continue
+            scale = float(np.float32(np.abs(want[~nan]).max()))
+            err = float(np.abs(got[~nan] - want[~nan]).max()) / max(scale * EPS, 1e-300)
+            worst = max(worst, err)
+            _require(err <= KITTI_GRAD_ULP, "%s: _kitti_bwd scale %d (%dx%d): %.3g fp32 ulp of the largest gradient > %d"
+                     % (self.current, s, got.shape[2], got.shape[3], err, KITTI_GRAD_ULP))
+        n, _, H, W = a["t"]["target"].shape
+        _record("_kitti_bwd", "fp64", "ulp of largest", worst, KITTI_GRAD_ULP, n * H * W * len(loss_scales))
 
     # ------------------------------------------------------------------------------------------ NYUv2 evaluation
     def _before_NyuDepthEvaluator_add(self, a):

@@ -1,8 +1,12 @@
 """GPU: KITTI's depth-hints training loss on libwmd (kitti_loss.KittiDepthHintsLoss, csrc/loss_kitti.cu).
 
-* Fixture parity: on the cases of tests/golden/kitti_hints_loss.npz the warped colours, color_depth_hint and both masks
-  equal the contract-mode oracle's, the terms are within one float32 ulp and every gradient element within one float32
-  ulp of its scale's largest (the fp64 sums differ from the oracle's in order only).
+* Fixture parity: on the cases of tests/golden/kitti_hints_loss*.npz, each with the loss built from its own options
+  (depth range, smoothness weight, loss scales) and cameras, the warped colours, color_depth_hint and both masks equal
+  the contract-mode oracle's, the terms are within one float32 ulp (NaN where the oracle's is NaN: the one-pixel-thick
+  scales' smoothness) and every gradient element within one float32 ulp of its scale's largest (the fp64 sums differ
+  from the oracle's in order only).
+* Per term: the case's weighted sum of every term back-propagated through ``losses``, against the oracle's gradient
+  with the same grad_terms, at the same bars.
 * Full size: R18 640x192 with 12 frames, the same bars; the mask pixels that differ from the fp64-mode oracle are
   counted and printed.
 * Edge cases: N = 0, a missing key, wrong shapes and dtypes, a size not divisible by 8, a NaN disparity.
@@ -25,7 +29,7 @@ from wavelet_monodepth_b200.kitti_loss import KittiDepthHintsLoss
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-FIX = np.load(os.path.join(os.path.dirname(__file__), "golden", "kitti_hints_loss.npz"))
+FIX = okl.load_fixture(os.path.join(os.path.dirname(__file__), "golden"))
 R18 = (64, 64, 128, 256, 512)
 
 
@@ -46,22 +50,34 @@ def to_dev(inp, disps, case, grad=True):
     return inputs, outputs
 
 
-def native(case, inp, disps, seed):
+def native(case, inp, disps, seed, weights=None):
+    """the loss built from the case's options; the gradient of the total, or of sum_k weights[k] losses[k] (the keys in
+    okl.term_keys order)"""
     inputs, outputs = to_dev(inp, disps, case)
-    loss = KittiDepthHintsLoss(case["H"], case["W"], case["scales"], case["loss_scales"])
+    loss = KittiDepthHintsLoss(case["H"], case["W"], case["scales"], case["loss_scales"], **okl.options(case))
     torch.manual_seed(seed)
     total, losses = loss(inputs, outputs)
-    total.backward()
+    if weights is None:
+        total.backward()
+    else:
+        sum(float(w) * losses[k] for w, k in zip(weights, okl.term_keys(case["loss_scales"]))).backward()
     grads = {s: outputs[("disp", s)].grad.cpu().numpy().astype(np.float64) for s in case["loss_scales"]}
     return losses, outputs, grads
 
 
-def check_against_oracle(case, inp, disps, seed):
+def check_against_oracle(case, inp, disps, seed, weights=None):
+    """the bars above; returns the oracle's result and the worst (term ulp, gradient ulp of the scale's largest)"""
     noise = okl.draw_noise(seed, inp, case["loss_scales"])
-    o = okl.run(inp, disps, noise, case["scales"], case["loss_scales"], mode="contract")
-    losses, outputs, grads = native(case, inp, disps, seed)
+    o = okl.run(inp, disps, noise, case["scales"], case["loss_scales"], mode="contract", grad_terms=weights,
+                **okl.options(case))
+    losses, outputs, grads = native(case, inp, disps, seed, weights)
+    worst = [0.0, 0.0]
     for k, v in losses.items():
-        assert ulps(float(v.detach()), float(o[k])) <= 1, (k, float(v.detach()), float(o[k]))
+        got, want = float(v.detach()), float(o[k])
+        assert np.isnan(got) == np.isnan(want), (k, got, want)
+        if not np.isnan(want):
+            worst[0] = max(worst[0], float(ulps(got, want)))
+            assert ulps(got, want) <= 1, (k, got, want)
     assert np.array_equal(outputs[("color_depth_hint", "s", 0)].cpu().numpy(), o["color_depth_hint"].astype(np.float32))
     for s in case["loss_scales"]:
         assert np.array_equal(outputs[("color", "s", s)].cpu().numpy(), o["warped"][s].astype(np.float32), equal_nan=True)
@@ -69,24 +85,41 @@ def check_against_oracle(case, inp, disps, seed):
             got = outputs["%s/%d" % (key, s)].cpu().numpy()[:, 0]
             assert np.array_equal(got, o[key][s]), (key, s, int((got != o[key][s]).sum()))
         want = o["grad"][s]
+        assert np.isfinite(want).all() and np.isfinite(grads[s]).all(), (s, int((~np.isfinite(grads[s])).sum()))
         scale = np.float32(np.abs(want).max())
         err = np.abs(grads[s] - want).max() / (float(scale) * 2.0 ** -24)
+        worst[1] = max(worst[1], float(err))
         assert err <= 1, (s, err)
-    return o
+    return o, worst
+
+
+def _case(name):
+    case = okl.CASES[name]
+    seed = int(FIX["%s/seed" % name])
+    return case, seed, okl.make_inputs(case, seed)
 
 
 @pytest.mark.parametrize("name", [str(c) for c in FIX["cases"]])
 def test_fixture_parity(name):
-    case = okl.CASES[name]
-    seed = int(FIX["%s/seed" % name])
-    inp, disps = okl.make_inputs(case, seed)
-    check_against_oracle(case, inp, disps, seed)
+    case, seed, (inp, disps) = _case(name)
+    _, worst = check_against_oracle(case, inp, disps, seed)
+    print("\n%s: worst term %.3g ulp, worst gradient %.3g ulp of its scale's largest" % (name, *worst))
+
+
+@pytest.mark.parametrize("name", [str(c) for c in FIX["cases"]])
+def test_weighted_terms(name):
+    """every term with its own weight (FIX's weights: distinct per term and scale, some negative): the backward reads
+    each reproj_loss/s, depth_hint_loss/s and loss/s coefficient of grad_terms where the oracle does"""
+    case, seed, (inp, disps) = _case(name)
+    w = FIX["%s/weights" % name]
+    _, worst = check_against_oracle(case, inp, disps, seed, weights=w)
+    print("\n%s weighted: worst term %.3g ulp, worst gradient %.3g ulp of its scale's largest" % (name, *worst))
 
 
 def test_full_size_r18_640x192_x12():
     case = dict(N=12, H=192, W=640, scales=okl.SCALES, loss_scales=okl.SCALES)
     inp, disps = okl.make_inputs(case, 77)
-    o = check_against_oracle(case, inp, disps, 77)
+    o, _ = check_against_oracle(case, inp, disps, 77)
     o64 = okl.run(inp, disps, okl.draw_noise(77, inp, case["loss_scales"]), mode="fp64", grads=False)
     flips = {s: int((o["identity_selection"][s] != o64["identity_selection"][s]).sum()
                     + (o["depth_hint_pixels"][s] != o64["depth_hint_pixels"][s]).sum()) for s in case["loss_scales"]}

@@ -4,9 +4,10 @@ benchmarked decoders, against the fp64 contract of its kernel (tests/launch_chec
 tests/test_gpu_production_launches.py checks the benchmarked decoders; this file checks the rest at production batch and
 image sizes, where the size-dependent parts of their kernels are: the 224-pixel wavelet decoder (its MobileNetV2-light
 pyramid's fine levels take the FMA engine) and the 224-pixel baseline decoder; native training of those two, of NYU's
-baseline Decoder, of DecoderWave with NyuDepthLoss (the loss's CTA partials and its backward's footprint gather) and of
-the KITTI R50 1024x320 wave decoder; the KITTI dense decoder without skips; the sparse NYU decoder at its threshold
-extremes; NYU evaluation with depth boundary errors on 440x592 frames (fixed CTA grids, union-find hysteresis, the
+baseline Decoder, of DecoderWave with NyuDepthLoss (the loss's CTA partials and its backward's footprint gather), of
+the KITTI R50 1024x320 wave decoder, and of KITTI's wave (R50 1024x320) and baseline (R18 640x192, 12 frames) decoders
+with KittiDepthHintsLoss (its warps, CTA partials and gathers at production sizes); the KITTI dense decoder without
+skips; the sparse NYU decoder at its threshold extremes; NYU evaluation with depth boundary errors on 440x592 frames (fixed CTA grids, union-find hysteresis, the
 exact distance transform) and in 224 mode; KITTI evaluation of post-processed disparities, whose medians are taken by
 radix select over full LiDAR frames.  Inputs are synthetic (synth, oracle.nyu_edges.edge_split,
 oracle.kitti_eval.synthetic_split).  The entry points are called through their modules, as the package's users do: a
@@ -24,8 +25,10 @@ import pytest
 import torch
 
 from oracle import kitti_eval as oke
+from oracle import kitti_loss as okl
 from oracle import nyu_edges as ne
 from wavelet_monodepth_b200 import kitti_decoders as kd, kitti_eval, nyu_decoders as nd, nyu_eval, synth
+from wavelet_monodepth_b200.kitti_loss import KittiDepthHintsLoss
 from wavelet_monodepth_b200.nyu_loss import NyuDepthLoss
 
 import launch_check as lc
@@ -120,6 +123,35 @@ def train(make, n, spec, shapes, loss=None):
     return run
 
 
+def train_kitti_loss(make, n, spec):
+    """One native training step of a KITTI decoder with KittiDepthHintsLoss on oracle.kitti_loss's synthetic stereo
+    frames (images, KITTI's intrinsics, hints); the tie-breaking noise from a seeded CPU generator, so both runs draw the
+    same.  Outputs, terms, masks, warps, parameter and input-feature gradients."""
+    def run():
+        ch, h, w = spec
+        mod = make(ch)
+        synth.load_random(mod, seed=1)
+        mod = mod.to(DEV).train()
+        feats = _feats(synth.kitti_feature_shapes(n, h, w, ch), seed=2, grad=True)
+        inp, _ = okl.make_inputs(dict(N=n, H=h, W=w, scales=okl.SCALES), 5)
+        inputs = {("color", 0, 0): inp["target"], ("color", "s", 0): inp["source"], ("K", 0): inp["K"],
+                  ("inv_K", 0): inp["inv_K"], "stereo_T": inp["stereo_T"], "depth_hint": inp["depth_hint"],
+                  "depth_hint_mask": inp["depth_hint_mask"]}
+        inputs.update({("color", 0, s): inp["colors"][s] for s in okl.SCALES if s})
+        inputs = {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in inputs.items()}
+        out = mod(feats)
+        torch.manual_seed(5)
+        total, losses = KittiDepthHintsLoss(h, w)(inputs, out)
+        res = {("out",) + tuple(k if isinstance(k, tuple) else (k,)): v.detach() for k, v in out.items()
+               if torch.is_tensor(v)}
+        res.update({("loss", k): v.detach() for k, v in losses.items()})
+        total.backward()
+        res.update({("grad", k): p.grad for k, p in mod.named_parameters() if p.grad is not None})
+        res.update({("feature_grad", j): f.grad for j, f in enumerate(feats) if f.grad is not None})
+        return res
+    return run
+
+
 def _nyu(cls):
     return lambda ch: cls(enc_features=list(ch), decoder_width=0.5)
 
@@ -200,6 +232,9 @@ WORKLOADS = {
     "train_decoder224_mnv2light_x8": train(_nyu(nd.Decoder224), 8, MNV2_224, synth.nyu_feature_shapes),
     "train_wave_r50_1024x320_x8": train(lambda ch: kd.DepthWaveProgressiveDecoder(np.array(ch)), 8, R50,
                                         synth.kitti_feature_shapes),
+    "train_wave_r50_1024x320_x8_kittiloss": train_kitti_loss(lambda ch: kd.DepthWaveProgressiveDecoder(np.array(ch)),
+                                                              8, R50),
+    "train_baseline_r18_640x192_x12_kittiloss": train_kitti_loss(lambda ch: kd.DepthDecoder(np.array(ch)), 12, R18),
     "dense_no_skips_r18_640x192_x16": kitti_no_skips(16, R18),
     "nyu_sparse_d161_640x480_x8_thr0": prod.nyu(nd.SparseDecoderWave, 8, D161, 0.0),
     "nyu_sparse_d161_640x480_x8_thr0.5": prod.nyu(nd.SparseDecoderWave, 8, D161, 0.5),

@@ -2,17 +2,19 @@
 has a checker, a pack, or a size / query function.  A new entry point cannot ship without one."""
 import inspect
 
-from wavelet_monodepth_b200 import _lib, kitti_eval, nyu_eval, nyu_loss, ops
+from wavelet_monodepth_b200 import _lib, kitti_eval, kitti_loss, nyu_eval, nyu_loss, ops
 
 import launch_check as lc
 
-ALL_SIGNATURES = {**_lib.SIGNATURES, **_lib.EVAL_SIGNATURES, **_lib.LOSS_SIGNATURES}
+TABLES = (_lib.SIGNATURES, _lib.EVAL_SIGNATURES, _lib.LOSS_SIGNATURES, _lib.KITTI_LOSS_SIGNATURES)
+ALL_SIGNATURES = {k: v for table in TABLES for k, v in table.items()}
 
 
 def test_every_symbol_is_classified():
-    """SYMBOLS covers wmd.h, wmd_eval.h and wmd_loss.h (their bindings, which test_abi / the oracle tests hold to the
-    headers), and nothing else."""
-    assert len(ALL_SIGNATURES) == len(_lib.SIGNATURES) + len(_lib.EVAL_SIGNATURES) + len(_lib.LOSS_SIGNATURES)
+    """SYMBOLS covers wmd.h, wmd_eval.h, wmd_loss.h and wmd_loss_kitti.h (their bindings, which test_abi / the oracle
+    tests hold to the headers), and nothing else."""
+    assert len(ALL_SIGNATURES) == sum(len(table) for table in TABLES)
+    assert _lib.KITTI_LOSS_SIGNATURES and set(_lib.KITTI_LOSS_SIGNATURES) <= set(ALL_SIGNATURES)
     unclassified = sorted(set(ALL_SIGNATURES) - set(lc.SYMBOLS))
     assert not unclassified, "libwmd symbols without a launch checker / pack / query classification: %s" % unclassified
     assert not sorted(set(lc.SYMBOLS) - set(ALL_SIGNATURES))
@@ -46,11 +48,11 @@ def _functions(module):
 
 
 def test_every_ops_function_that_calls_libwmd_is_wrapped():
-    """A function or method of ops, nyu_loss, nyu_eval or kitti_eval that reaches a launch or pack symbol directly is a
-    checked entry point or a pack."""
+    """A function or method of ops, nyu_loss, nyu_eval, kitti_eval or kitti_loss that reaches a launch or pack symbol
+    directly is a checked entry point or a pack."""
     wrapped = set(lc.ENTRIES) | set(lc.PACKS)
     found = set()
-    for module in (ops, nyu_loss, nyu_eval, kitti_eval):
+    for module in (ops, nyu_loss, nyu_eval, kitti_eval, kitti_loss):
         for name, fn in _functions(module):
             src = inspect.getsource(fn)
             used = [s for s, k in lc.SYMBOLS.items() if k != "query" and ".%s(" % s in src]

@@ -1,6 +1,7 @@
 """The launch checkers of the evaluation and loss entry points (tests/launch_check.py) have teeth: each passes the oracle's
 own answer and raises LaunchError when one element of it is changed by the smallest step its bar must see (a loss
-gradient one ulp off, one edge pixel toggled, one a_k count off by one, one KITTI median ratio one ulp off).  CPU only:
+gradient one ulp off, one edge pixel toggled, one a_k count off by one, one KITTI median ratio one ulp off, one KITTI
+loss mask pixel toggled).  CPU only:
 the checkers are called directly on CPU tensors, with stand-ins for the evaluators' state; no GPU and no libwmd."""
 import types
 
@@ -9,6 +10,7 @@ import pytest
 import torch
 
 from oracle import kitti_eval as oke
+from oracle import kitti_loss as okl
 from oracle import nyu_edges as ne
 from oracle import nyu_eval as one
 from oracle import nyu_loss as onl
@@ -247,3 +249,62 @@ def test_kitti_compute_errors_checker(harness):
     def call(out):
         harness._check_compute_errors(dict(gt=t(gt), pred=t(pred)), t(out), None)
     both(call, (want,), (off,))
+
+
+# ------------------------------------------------------------------------------------------ KITTI training loss
+def _kitti_loss_case():
+    """a 2-frame 32x48 case with a different camera per frame and loss scales (0, 1, 3), the call's arguments as
+    kitti_loss._kitti_fwd / _kitti_bwd receive them (CPU tensors), and the contract-mode oracle's answer"""
+    case = dict(N=2, H=32, W=48, scales=okl.SCALES, loss_scales=(0, 1, 3), camera=True)
+    inp, disps = okl.make_inputs(case, 21)
+    noise = okl.draw_noise(21, inp, case["loss_scales"])
+    ls, opt = case["loss_scales"], (0.5, 80.0, 0.1)
+    tt = {k: t(inp[k]) for k in ("target", "source", "K", "inv_K", "stereo_T", "depth_hint", "depth_hint_mask")}
+    tt.update(color=[t(inp["colors"][s]) for s in ls], disp=[t(disps[s]) for s in ls], noise=[t(noise[s]) for s in ls])
+    gt = np.array(okl.term_weights(ls), np.float32)
+    o = okl.run(inp, disps, noise, okl.SCALES, ls, min_depth=0.5, max_depth=80.0, disparity_smoothness=0.1,
+                grad_terms=gt)
+    a = dict(t=tt, scales=okl.SCALES, loss_scales=ls, opt=opt)
+    return a, o, gt
+
+
+def test_kitti_fwd_checker(harness):
+    a, o, _ = _kitti_loss_case()
+    ls = a["loss_scales"]
+    terms = np.array([o[k] for k in okl.term_keys(ls)], np.float32)
+    masks = [np.stack([o[key][s] for s in ls])[:, :, None].astype(np.float32)
+             for key in ("identity_selection", "depth_hint_pixels")]
+    assert masks[1].sum() > 0 and masks[0].sum() > 0
+    warped = np.stack([o["warped"][s] for s in ls]).astype(np.float32)
+
+    def call(terms, idsel, hpix):
+        res = (t(terms), t(o["color_depth_hint"].astype(np.float32)), t(warped), t(idsel), t(hpix), None)
+        harness._check_kitti_fwd(a, res, None)
+    both(call, (terms, *masks), (ulp_up(ulp_up(terms, 5), 5), *masks))     # one term two ulp off
+    for k in (0, 1):
+        toggled = [m.copy() for m in masks]
+        toggled[k][1, 1, 0, 7, 9] = 1 - toggled[k][1, 1, 0, 7, 9]        # one mask pixel toggled
+        both(call, (terms, *masks), (terms, *toggled))
+
+
+def test_kitti_bwd_checker(harness):
+    a, o, gt = _kitti_loss_case()
+    ls = a["loss_scales"]
+    idsel, hpix = (t(np.stack([o[key][s] for s in ls])[:, :, None].astype(np.float32))
+                   for key in ("identity_selection", "depth_hint_pixels"))
+    grads = [o["grad"][s].astype(np.float32) for s in ls]
+    a = dict(a, grad_terms=t(gt), idsel=idsel, hpix=hpix)
+
+    def call(grads, idsel=idsel):
+        harness._check_kitti_bwd(dict(a, idsel=idsel), [t(g) for g in grads], None)
+    for i, s in enumerate(ls):
+        # the scale's largest gradient one ulp farther from the oracle's fp64 value
+        want = o["grad"][s]
+        j = np.unravel_index(np.argmax(np.abs(want)), want.shape)
+        bad = list(grads)
+        bad[i] = grads[i].copy()
+        bad[i][j] = np.nextafter(grads[i][j], np.float32(np.inf if grads[i][j] >= want[j] else -np.inf))
+        both(call, (grads,), (bad,))
+    toggled = idsel.clone()
+    toggled[0, 0, 0, 3, 4] = 1 - toggled[0, 0, 0, 3, 4]                   # one mask pixel toggled
+    both(call, (grads,), (grads, toggled))

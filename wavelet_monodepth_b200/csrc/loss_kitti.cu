@@ -457,18 +457,24 @@ __global__ void __launch_bounds__(kKT, 1) kitti_ddepth_kernel(Geo g, const float
   dup[p] = M_(dD, -M_(M_(S_(g.hi, g.lo), D), D));
 }
 
-// d smooth / d nd at low-resolution pixel (y, x) (x edges' sign e / cx, y edges' / cy, in the oracle's order)
+// d smooth / d nd at low-resolution pixel (y, x) (x edges' sign e / cx, y edges' / cy, in the oracle's order).  Only
+// edges that exist add a term: a one-column map has cx = 0 and a one-row map cy = 0, and 0 / 0 would make every
+// gradient of the scale NaN where the reference's mean over no edges contributes none.
 __device__ __forceinline__ double smooth_G(const float* d, const float* img, long long plane, int h, int w, int y, int x, double den,
                            double cx, double cy) {
   double sg, G = 0.0;
-  edge(d, img, plane, h, w, y, x, den, 0, &sg);
-  G = A_(G, D_(sg, cx));
+  if (x < w - 1) {
+    edge(d, img, plane, h, w, y, x, den, 0, &sg);
+    G = A_(G, D_(sg, cx));
+  }
   if (x > 0) {
     edge(d, img, plane, h, w, y, x - 1, den, 0, &sg);
     G = S_(G, D_(sg, cx));
   }
-  edge(d, img, plane, h, w, y, x, den, 1, &sg);
-  G = A_(G, D_(sg, cy));
+  if (y < h - 1) {
+    edge(d, img, plane, h, w, y, x, den, 1, &sg);
+    G = A_(G, D_(sg, cy));
+  }
   if (y > 0) {
     edge(d, img, plane, h, w, y - 1, x, den, 1, &sg);
     G = S_(G, D_(sg, cy));
