@@ -1,12 +1,14 @@
-"""Shared test helpers: golden-fixture loading, seeded module construction, comparison metrics."""
+"""Shared test helpers: golden-fixture loading, seeded module construction, operands, comparison metrics."""
 import glob
 import json
 import os
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 from wavelet_monodepth_b200 import synth
+from wavelet_monodepth_b200._lib import ACT_ELU, ACT_LRELU, ACT_NONE, ACT_SIGMOID, PAD_REFLECT, PAD_REPLICATE, PAD_ZERO
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 REL_TOL = 1e-4      # north_star: outputs within 1e-4 relative fp32 tolerance
@@ -25,6 +27,29 @@ def golden_names(prefix):
 
 def key_str(k):
     return k if isinstance(k, str) else "_".join(str(v) for v in k)
+
+
+def rnd(*shape, seed=0, lo=-1.0, hi=1.0):
+    rs = np.random.RandomState(seed)
+    return torch.from_numpy(rs.uniform(lo, hi, size=shape).astype(np.float32))
+
+
+def rows_of(x):
+    """(N, C, H, W) -> pixel-major rows (N*H*W, C)."""
+    return x.permute(0, 2, 3, 1).reshape(-1, x.shape[1]).contiguous()
+
+
+def close(got, want, tol=1e-12):
+    """Two fp64 restatements of one sum, in different orders: max |got - want| <= tol max(max |want|, 1)."""
+    return float((got - want).abs().max()) <= tol * max(float(want.abs().max()), 1.0)
+
+
+def torch_conv(x, wt, b, pad, act):
+    """A 3x3 convolution with the layers' padding and activation, in torch."""
+    mode = {PAD_REFLECT: "reflect", PAD_REPLICATE: "replicate", PAD_ZERO: "constant"}[pad]
+    y = F.conv2d(F.pad(x, (1, 1, 1, 1), mode=mode), wt, b)
+    return {ACT_NONE: lambda t: t, ACT_ELU: F.elu, ACT_LRELU: lambda t: F.leaky_relu(t, 0.2),
+            ACT_SIGMOID: torch.sigmoid}[act](y)
 
 
 def rel_err(a, b):
@@ -50,6 +75,12 @@ def nyu_features(meta, device="cpu"):
     if "sample" in meta:
         feats = [f[meta["sample"]:meta["sample"] + 1] for f in feats]
     return [f.to(device) for f in feats]
+
+
+def kitti_variant(want, meta, name):
+    """(constructor kwargs, the variant's arrays keyed by key_str) of one DepthDecoder variant of the KITTI fixture."""
+    prefix = name + "__"
+    return meta["variants"][name], {k[len(prefix):]: v for k, v in want.items() if k.startswith(prefix)}
 
 
 def seeded_params(module, meta):

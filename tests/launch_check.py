@@ -39,6 +39,7 @@ import conv_grad_ref
 import conv_ref as cr
 import disp_tail_ref
 import head_ref as hr
+from contract import Worst, errors
 
 _f32, _f64 = torch.float32, torch.float64
 EPS = 2.0 ** -24
@@ -161,30 +162,11 @@ EVAL_REL = 1e-12       # fp64 sums of a fixed order against math.fsum / numpy's 
 NYU_SUM_ABS = 1e-15    # per pixel: the fp64 log10's ulp, all a log_10 sum of equal depths is made of
 POST_REL = 1e-15       # batch_post_process_disparity: numpy's expression, evaluated in the same precision
 
-REPORT = {}            # (entry, engine, mode) -> [worst err, bar, launches, largest row count]
+REPORT = Worst("entry point, engine / precision, mode")     # err in the unit of the entry's bar
 
 
 def _record(entry, engine, mode, err, bar, rows):
-    r = REPORT.setdefault((entry, engine, mode), [0.0, bar, 0, 0])
-    r[0] = max(r[0], err)
-    r[2] += 1
-    r[3] = max(r[3], int(rows))
-
-
-def report_lines():
-    lines = ["worst err per (entry point, engine / precision, mode): worst (bar, launches, most rows)"]
-    for k in sorted(REPORT):
-        worst, bar, count, rows = REPORT[k]
-        lines.append("  %-28s %-8s %-18s %.2e  (bar %s, %d launches, %d rows)"
-                     % (k + (worst, "exact" if bar == 0 else "%.2g" % bar, count, rows)))
-    return lines
-
-
-def _err(got, want, s, allow=0.0):
-    """max over the elements of (|got - want| - allow) / S."""
-    if got.numel() == 0:
-        return 0.0
-    return float(((got.double() - want).abs() - allow).clamp(min=0).div(s.clamp(min=1e-300)).max())
+    REPORT.note((entry, engine, mode), err, bar=bar, rows=int(rows))
 
 
 def _i(t):
@@ -391,7 +373,7 @@ class Harness:
         if wp.kind == "tc" and a["amax_out"] is not None:
             self._check_amax_out(entry, old_amax, a["amax_out"], y)
         allow = 0.0 if a["act"] in (cr.ACT_NONE, cr.ACT_LRELU) else cr.ACT_ALLOW
-        err = _err(y, y64, s, allow + floor)
+        err = errors(y, y64, s, allow + floor)[0]
         bar = cr.BAR[engine]
         _record(entry, engine, mode, err, bar, rows)
         _require(err <= bar, "%s: conv_rows %s %s (n %d, %dx%d, c0 %d, c1 %d, cout %d, taps %d, %d rows): err/S %.3g > %.3g"
@@ -409,7 +391,7 @@ class Harness:
         want, s, floor = hr.head_mlp_ref(x, a["c"], w1, b1, wz, a["slope"], count, max_rows, floor=True)
         nz = a["nz"]
         _require(bool((z[:rows, nz:56] == 0).all()), "head_mlp: columns nz..55 are not zero")
-        err = _err(z[:rows, :nz], want, s, floor)
+        err = errors(z[:rows, :nz], want, s, floor)[0]
         bar = hr.BAR["head_mlp"]
         _record("head_mlp", "tf32x3", "-", err, bar, rows)
         _require(err <= bar, "%s: head_mlp err/S %.3g > %.3g" % (self.current, err, bar))
@@ -427,7 +409,7 @@ class Harness:
         want, s = hr.head_gather_ref(z, z.shape[1], a["col0"], groups, a["idxmap"], a["bias"], a["scale"], a["act"],
                                      a["dual"], a["pad"], a["pixels"], a["count"], max_rows, cout, n, h, w)
         allow = 0.0 if a["act"] == cr.ACT_NONE else cr.ACT_ALLOW * abs(a["scale"]) * (2 if a["dual"] else 1)
-        err = _err(self._written(out, a["pixels"], rows, cout), want, s, allow)
+        err = errors(self._written(out, a["pixels"], rows, cout), want, s, allow)[0]
         bar = hr.BAR["head_gather"]
         _record("head_gather", "fp32", "list" if a["pixels"] is not None else "dense", err, bar, rows)
         _require(err <= bar, "%s: head_gather err/S %.3g > %.3g" % (self.current, err, bar))
@@ -444,7 +426,7 @@ class Harness:
         want, s = hr.head_conv3x3_ref(t, t.shape[1], c, a["off_a"], a["off_b"], wa, a["ba"], wb, a["bb"], cout, a["scale"],
                                       a["act"], a["pad"], a["idxmap"], a["pixels"], a["count"], max_rows, n, h, w)
         allow = 0.0 if a["act"] == cr.ACT_NONE else cr.ACT_ALLOW * abs(a["scale"]) * (2 if dual else 1)
-        err = _err(self._written(out, a["pixels"], rows, cout), want, s, allow)
+        err = errors(self._written(out, a["pixels"], rows, cout), want, s, allow)[0]
         bar = hr.BAR["head_conv3x3"]
         _record("head_conv3x3", "fp32", "list" if a["pixels"] is not None else "dense", err, bar, rows)
         _require(err <= bar, "%s: head_conv3x3 (c %d, cout %d) err/S %.3g > %.3g" % (self.current, c, cout, err, bar))
@@ -456,8 +438,9 @@ class Harness:
         ref = hr.head_idwt_ref(z, a["col0"], a["idxmap"], a["mask"], a["bias"], a["scale"], a["pad"], yl, a["disp_scale"],
                                a["clamp01"], n, h, w)
         al = cr.ACT_ALLOW * abs(a["scale"])
-        err = max(_err(res["yh"], ref["yh"], ref["s_yh"], 2 * al), _err(res["out"], ref["out"], ref["s_out"], 3 * al),
-                  _err(res["disp"], ref["disp"], ref["s_disp"], 3 * al * abs(a["disp_scale"])))
+        err = max(errors(res["yh"], ref["yh"], ref["s_yh"], 2 * al)[0],
+                  errors(res["out"], ref["out"], ref["s_out"], 3 * al)[0],
+                  errors(res["disp"], ref["disp"], ref["s_disp"], 3 * al * abs(a["disp_scale"]))[0])
         if a["mask"] is not None:
             off = (a["mask"].reshape(n, 1, h, w) == 0).expand(-1, 3, -1, -1)
             _require(bool((res["yh"][off] == 0).all()), "head_idwt: coefficients outside the wavelet mask are not zero")
@@ -518,7 +501,7 @@ class Harness:
         x64 = x.detach().double()
         rl, rh = ohaar.DWTForward(J=1, wave="haar", mode="zero").to(x.device).double()(x64)
         sc = 0.5 * F.avg_pool2d(x64.abs(), 2) * 4
-        err = max(_err(ll, rl, sc), _err(hf, rh[0], sc.unsqueeze(2).expand_as(rh[0])))
+        err = max(errors(ll, rl, sc)[0], errors(hf, rh[0], sc.unsqueeze(2).expand_as(rh[0]))[0])
         bar = DWT_ULP * EPS
         ol, oh = ohaar.DWTForward(J=1, wave="haar", mode="zero")(x.detach().float().cpu())
         exact = torch.equal(ll.cpu(), ol) and torch.equal(hf.cpu(), oh[0])
@@ -543,7 +526,7 @@ class Harness:
             return
         w1, b1, w2, b2 = self._weights(a["packed"])
         want, s, floor = disp_tail_ref.disp_tail_ref(a["x"], w1, b1, w2, b2, n, a["h"], a["w"], floor=True)
-        err = _err(out, want, s, floor)
+        err = errors(out, want, s, floor)[0]
         _record("disp_tail16", "tf32x3", "-", err, disp_tail_ref.BAR, n * a["h"] * a["w"] * 4)
         _require(err <= disp_tail_ref.BAR, "%s: disp_tail16 err/S %.3g > %.3g" % (self.current, err, disp_tail_ref.BAR))
 
@@ -703,7 +686,7 @@ class Harness:
         want = self._dz64(a["y"], a["dy"], cout, a["act"], a["act_param"])
         rows = want.shape[0]
         dz_floor, db_floor = conv_grad_ref.act_bwd_floor(a["dy"][:, :cout], rows_summed=rows)
-        err = _err(dz[:, :cout], want, want.abs().clamp(min=1e-38), dz_floor)
+        err = errors(dz[:, :cout], want, want.abs().clamp(min=1e-38), dz_floor)[0]
         bar = ACT_BWD_ULP * EPS
         _record("act_backward", "fp32", "dz", err, bar, rows)
         _require(err <= bar, "%s: act_backward dz %.3g > %.3g relative" % (self.current, err, bar))
@@ -711,7 +694,7 @@ class Harness:
             self._check_amax_out("act_backward", old_amax, a["amax"], dz[:, :cout])
         if db is not None:
             gb, sb = want.sum(0), want.abs().sum(0)
-            err = _err(db, gb, sb, db_floor)
+            err = errors(db, gb, sb, db_floor)[0]
             bar = conv_grad_ref.BARS["db"]
             _record("act_backward", "fp32", "db", err, bar, rows)
             _require(err <= bar, "%s: act_backward db err/S %.3g > %.3g" % (self.current, err, bar))
@@ -737,7 +720,7 @@ class Harness:
                                            shift0=a["shift0"])
             floor = conv_grad_ref.wgrad_floor(x0r, c0, x1r, c1, wzero, a["dz"][:, :cout], n, h, w, taps=taps,
                                               pad=a["pad"], shift0=a["shift0"])
-        err = _err(dw, *ref["w"], floor)
+        err = errors(dw, *ref["w"], floor)[0]
         bar = conv_grad_ref.BARS["dW"]
         _record("conv_wgrad", "tf32x3", "cout<=8" if cout <= 8 else "-", err, bar, n * h * w)
         _require(err <= bar, "%s: conv_wgrad (n %d, %dx%d, c0 %d, c1 %d, cout %d) err/S %.3g > %.3g"
@@ -758,14 +741,14 @@ class Harness:
         if a["amax"] is not None:           # the fp16-pair form: BAR S + F (conv_grad_ref.dgrad_floor)
             floor = conv_grad_ref.dgrad_floor(c0, c1, weight, a["dz"][:, :cout], n, h, w, _scalar(a["amax"]), taps=taps,
                                               pad=a["pad"], shift0=shift0)
-        err0 = _err(dx0[:, :c0], *ref["x0"], allow=floor["x0"])
+        err0 = errors(dx0[:, :c0], *ref["x0"], allow=floor["x0"])[0]
         _require(bool((dx0[:, c0:] == 0).all()), "conv_dgrad: dx0 pad columns are not zero")
         _record("conv_dgrad", "dx0", "taps%d" % taps, err0, conv_grad_ref.BARS["dx0"], rows0)
         _require(err0 <= conv_grad_ref.BARS["dx0"], "%s: conv_dgrad dx0 err/S %.3g > %.3g"
                  % (self.current, err0, conv_grad_ref.BARS["dx0"]))
         if dx1 is not None:
             want, s = ref["x1"]
-            err1 = _err(_nhwc(dx1), want, s, allow=floor["x1"])
+            err1 = errors(_nhwc(dx1), want, s, allow=floor["x1"])[0]
             _record("conv_dgrad", "dx1", "taps%d" % taps, err1, conv_grad_ref.BARS["dx1"], n * h * w)
             _require(err1 <= conv_grad_ref.BARS["dx1"], "%s: conv_dgrad dx1 err/S %.3g > %.3g"
                      % (self.current, err1, conv_grad_ref.BARS["dx1"]))

@@ -14,26 +14,11 @@ import torch.nn.functional as F
 from oracle import sparse_ops as osp
 
 import conv_ref as cr
-
-TOL = 1e-12
-
-
-def rnd(*shape, seed=0, lo=-1.0, hi=1.0):
-    rs = np.random.RandomState(seed)
-    return torch.from_numpy(rs.uniform(lo, hi, size=shape).astype(np.float32))
-
-
-def rows_of(x):
-    """(N, C, H, W) -> pixel-major rows (N*H*W, C)."""
-    return x.permute(0, 2, 3, 1).reshape(-1, x.shape[1]).contiguous()
+from helpers import close, rnd, rows_of
 
 
 def nchw_of(rows, n, h, w):
     return rows.reshape(n, h, w, -1).permute(0, 3, 1, 2)
-
-
-def close(got, want):
-    return float((got - want).abs().max()) <= TOL * max(float(want.abs().max()), 1.0)
 
 
 _MODE = {cr.PAD_ZERO: "constant", cr.PAD_REFLECT: "reflect", cr.PAD_REPLICATE: "replicate"}

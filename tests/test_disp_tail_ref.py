@@ -5,7 +5,7 @@ import torch
 import torch.nn.functional as F
 
 from disp_tail_ref import disp_tail_ref
-from test_conv_ref import close, rnd, rows_of
+from helpers import close, rnd, rows_of
 
 
 def _composition(x, w1, b1, w2, b2):

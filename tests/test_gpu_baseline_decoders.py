@@ -16,8 +16,8 @@ from oracle import nyu as onyu
 from wavelet_monodepth_b200 import _lib, kitti_decoders as kd, nyu_decoders as nd, synth, train_native
 from wavelet_monodepth_b200._lib import WmdError
 
-from helpers import REL_TOL, compare_outputs, key_str, kitti_features, load_golden, nyu_features, rel_err, seeded_params
-from test_oracle_baseline import kitti_variant
+from helpers import (REL_TOL, compare_outputs, key_str, kitti_features, kitti_variant, load_golden, nyu_features, rel_err,
+                     seeded_params)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"

@@ -33,7 +33,6 @@ The same-sign worst is the truncation bias of one full epoch: ~1.6e-8 x K of S f
 per epoch), so it does not grow past one epoch.  Bars: 2.4x (tf32x3), 2.9x (f16x3) and 2.3x (simt) the worst observed;
 kernels with a correction term, a slab, the bias or the epochs removed were off by 1.0e-4 S or more on some element.
 """
-import numpy as np
 import pytest
 import torch
 
@@ -41,141 +40,16 @@ from wavelet_monodepth_b200 import _lib, ops
 from wavelet_monodepth_b200._lib import ACT_ELU, ACT_LRELU, ACT_NONE, ACT_SIGMOID, PAD_REFLECT, PAD_REPLICATE, PAD_ZERO
 
 import conv_ref as cr
+from conv_launch import DEV, WORST, Layer, gather_layer, mask, operands, run, sm_count
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-
-BAR, ACT_ALLOW = cr.BAR, cr.ACT_ALLOW
-SENTINEL = -3.0e38                # never produced by these layers
-PAD_GARBAGE = 1.0e6               # padding columns of the source rows (must not be read)
 ENGINES = ["tf32x3", "f16x3", "simt"]
 DISTS = ["mixed", "same"]
-
-_WORST = {}
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
-    yield
-    if _WORST:
-        print("\nworst err per (engine, group, operands):")
-        for k in sorted(_WORST):
-            print("  %-7s %-10s %-6s %.2e  (bar %.1e, %d launches)" % (k + (_WORST[k][0], BAR[k[0]], _WORST[k][1])))
-
-
-def sm_count():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-class Layer:
-    """Geometry and index maps of one launch (index tensors on the device)."""
-
-    def __init__(self, n, h, w, c0, cout, c1=0, taps=9, pad=PAD_REFLECT, shift0=0, map0=None, map1=None, gate=None,
-                 pixels=None, count=None, max_rows=None, x0_rows=None):
-        self.n, self.h, self.w, self.c0, self.c1, self.cout, self.taps, self.pad = n, h, w, c0, c1, cout, taps, pad
-        self.shift0, self.map0, self.map1, self.gate = shift0, map0, map1, gate
-        self.pixels, self.count = pixels, count
-        total = n * h * w
-        self.max_rows = max_rows if max_rows is not None else (len(pixels) if pixels is not None else total)
-        if x0_rows is None:
-            if map0 is not None:
-                x0_rows = max(int(map0.max()) + 1, 1)
-            elif taps == 1:
-                x0_rows = total
-            else:
-                x0_rows = n * (h >> shift0) * (w >> shift0)
-        self.x0_rows = x0_rows
-        self.x1_rows = (max(int(map1.max()) + 1, 1) if map1 is not None else total) if c1 else 0
-
-    @property
-    def k(self):
-        return self.taps * (self.c0 + self.c1)
-
-    @property
-    def rows(self):
-        r = self.count if self.pixels is not None else self.n * self.h * self.w
-        return min(r, self.max_rows)
-
-
-def _uniform(shape, lo, hi, g):
-    return torch.rand(shape, generator=g, device=DEV, dtype=torch.float32) * (hi - lo) + lo
-
-
-def _source(rows, c, lo, hi, g):
-    """rows x c operand in a row buffer whose 4..7 padding columns hold PAD_GARBAGE."""
-    x = torch.full((rows, ops.pad4(c) + 4), PAD_GARBAGE, device=DEV)
-    x[:, :c] = _uniform((rows, c), lo, hi, g)
-    return x
-
-
-def operands(L, dist, seed):
-    g = torch.Generator(device=DEV)
-    g.manual_seed(seed)
-    lo = 0.0 if dist == "same" else -1.0
-    x0 = _source(L.x0_rows, L.c0, lo, 1.0, g)
-    x1 = _source(L.x1_rows, L.c1, lo, 1.0, g) if L.c1 else None
-    k = 3 if L.taps == 9 else 1
-    wlo, whi = (0.0, 2.0 / L.k) if dist == "same" else (-1.0, 1.0)
-    wt = _uniform((L.cout, L.c0 + L.c1, k, k), wlo, whi, g)
-    b = _uniform((L.cout,), lo, 1.0, g)
-    return x0, x1, wt, b
-
-
-def _bias(b, mode):
-    """None, the plain tensor, or a view `mode` floats into a fresh (256-byte aligned) allocation."""
-    if mode == "none":
-        return None
-    off = 0 if mode == "aligned" else int(mode[-1])
-    base = torch.zeros(b.numel() + 4, device=DEV)
-    base[off:off + b.numel()] = b
-    v = base[off:off + b.numel()]
-    assert v.data_ptr() % 16 == 4 * off
-    return v
-
-
-def pack(wt, c1, engine):
-    if engine == "simt":
-        return ops.pack_weight(wt, c1, kind="simt")
-    wp = ops.pack_weight(wt, c1, kind="tc", precision=engine)
-    assert wp.kind == "tc" and (engine == "tf32x3" or wp.data16 is not None)
-    return wp
-
-
-def run(L, engine, dist, group, splits=None, act=ACT_NONE, act_param=0.2, bias="aligned", seed=0, ops_in=None):
-    """One launch, checked against the reference; returns the whole output buffer."""
-    if engine == "f16x3":
-        assert splits in (None, 0, 1), "f16x3 runs whole tiles or balanced only"
-    x0, x1, wt, b = ops_in if ops_in is not None else operands(L, dist, seed)
-    bv = _bias(b, bias)
-    wp = pack(wt, L.c1, engine)
-    tc = engine != "simt"
-    out = torch.full((L.max_rows + 5, ops.pad4(L.cout) + 4), SENTINEL, device=DEV)
-    amax_out = torch.zeros(1, device=DEV) if tc else None
-    am0 = x0[:, :L.c0].abs().max().reshape(1) if engine == "f16x3" else None
-    am1 = x1[:, :L.c1].abs().max().reshape(1) if engine == "f16x3" and L.c1 else None
-    count = torch.tensor([L.count], dtype=torch.int32, device=DEV) if L.pixels is not None else None
-    ops.conv_rows(x0, L.c0, wp, bv, L.cout, L.n, L.h, L.w, taps=L.taps, pad=L.pad, act=act, act_param=act_param,
-                  map0=L.map0, shift0=L.shift0, x1=x1, c1=L.c1, gate=L.gate, pixels=L.pixels, count=count,
-                  max_rows=L.max_rows, out=out, splits=splits if tc else None, map1=L.map1, amax0=am0, amax1=am1,
-                  amax_out=amax_out)
-    rows = L.rows
-    sent = torch.tensor(SENTINEL, device=DEV)
-    assert bool((out[rows:] == sent).all()), "rows past min(count, max_rows) were written"
-    assert bool((out[:rows, L.cout:] == sent).all()), "columns past cout were written"
-    y = out[:rows, :L.cout]
-    y64, s = cr.conv_ref(x0, L.c0, wt, bv, L.n, L.h, L.w, taps=L.taps, pad=L.pad, act=act, act_param=act_param,
-                         map0=L.map0, shift0=L.shift0, x1=x1, c1=L.c1, map1=L.map1, gate=L.gate, pixels=L.pixels,
-                         count=L.count, max_rows=L.max_rows)
-    allow = 0.0 if act in (ACT_NONE, ACT_LRELU) else ACT_ALLOW
-    err = float(((y.double() - y64).abs() - allow).clamp(min=0).div(s.clamp(min=1e-300)).max()) if rows else 0.0
-    key = (engine, group, dist)
-    was = _WORST.get(key, (0.0, 0))
-    _WORST[key] = (max(was[0], err), was[1] + 1)
-    assert err <= BAR[engine], (engine, group, dist, splits, err)
-    if tc:
-        want = float(y.abs().max()) if rows else 0.0
-        assert float(amax_out) == want, ("amax_out", float(amax_out), want)
-    return out
+    yield from WORST.module_report()
 
 
 # ------------------------------------------------------------------------------------------ N tiles and channel tails
@@ -254,40 +128,6 @@ def test_balanced_cut_tiles_with_cout_tail(engine, dist):
 
 
 # ------------------------------------------------------------------------------------------ gather paths
-def _mask(shape, p, seed):
-    g = torch.Generator().manual_seed(seed)
-    return (torch.rand(shape, generator=g) < p).to(torch.uint8).to(DEV)
-
-
-def gather_layer(case):
-    if case == "shift0_compact_map0":
-        lo = _mask((2, 6, 10), 0.6, 1)
-        return Layer(2, 12, 20, 40, 64, c1=24, shift0=1, map0=cr.index_map(lo))
-    if case == "compact_map1":
-        sel = _mask((2, 10, 14), 0.5, 2)
-        return Layer(2, 10, 14, 32, 48, c1=20, map1=cr.index_map(sel))
-    if case == "gate":
-        return Layer(2, 10, 14, 36, 33, c1=8, gate=_mask((2, 10, 14), 0.5, 3))
-    if case in ("count_lt_max_rows", "max_rows_lt_count"):
-        m_in, m_out = _mask((2, 16, 24), 0.7, 4), _mask((2, 16, 24), 0.4, 5)
-        pix = cr.pixel_list(m_out)
-        p = len(pix)
-        return Layer(2, 16, 24, 48, 96, map0=cr.index_map(m_in), pixels=pix, count=p,
-                     max_rows=p + 37 if case == "count_lt_max_rows" else p - 45)
-    if case == "decoder_level":                 # sparse_upsample + sparse_conv3x3: compact half-res x0, skip, gate, list
-        s0 = _mask((1, 8, 12), 0.5, 6)
-        up = s0.repeat_interleave(2, 1).repeat_interleave(2, 2)
-        pix = cr.pixel_list(_mask((1, 16, 24), 0.5, 7) * up)
-        return Layer(1, 16, 24, 40, 64, c1=20, shift0=1, map0=cr.index_map(s0), gate=up, pixels=pix, count=len(pix))
-    if case.startswith("pad_"):
-        pad = {"pad_zero": PAD_ZERO, "pad_reflect": PAD_REFLECT, "pad_replicate": PAD_REPLICATE}[case]
-        return Layer(1, 13, 17, 24, 40, pad=pad)
-    if case.startswith("thin_"):
-        _, h, w, pad = case.split("_")
-        return Layer(2, int(h), int(w), 20, 36, c1=12, pad={"z": PAD_ZERO, "f": PAD_REFLECT, "r": PAD_REPLICATE}[pad])
-    raise KeyError(case)
-
-
 GATHER = ["shift0_compact_map0", "compact_map1", "gate", "count_lt_max_rows", "max_rows_lt_count", "decoder_level",
           "pad_zero", "pad_reflect", "pad_replicate", "thin_1_37_z", "thin_1_37_r", "thin_2_33_f", "thin_40_1_r",
           "thin_35_2_f", "thin_1_1_z"]
@@ -303,7 +143,7 @@ def test_gather_paths(case, engine, dist):
 @pytest.mark.parametrize("engine,splits", [("tf32x3", 1), ("tf32x3", 0), ("tf32x3", 2), ("f16x3", 1), ("f16x3", 0),
                                            ("simt", None)])
 def test_count_zero_writes_nothing(engine, splits):
-    pix = cr.pixel_list(_mask((1, 16, 24), 0.5, 12))
+    pix = cr.pixel_list(mask((1, 16, 24), 0.5, 12))
     run(Layer(1, 16, 24, 64, 96, pixels=pix, count=0), engine, "mixed", "gather", splits=splits, seed=12)
 
 

@@ -17,12 +17,10 @@ from wavelet_monodepth_b200 import ops
 from wavelet_monodepth_b200._lib import PAD_REFLECT, PAD_REPLICATE, PAD_ZERO
 
 import conv_ref as cr
-from test_gpu_conv_contract import Layer, _mask, operands, pack
-from test_gpu_conv_rowset import GATHER, SET, SET_ROWS, _decoder_like, distinct_rows, tc_kernels
+from conv_launch import (DEV, GATHER, SENTINEL, SET, SET_ROWS, Layer, decoder_like, dense_layer, distinct_rows, mask,
+                         operands, pack, tc_kernels, twin)
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-SENTINEL = -3.0e38
 
 # (n, h, w, c0, c1, cout, pad, shift0): one past the widest window of each kind (the gather kernel runs them), and an
 # N = 32 tile
@@ -32,21 +30,6 @@ TOO_WIDE = [
     (1, 2, 194, 40, 0, 128, PAD_REFLECT, 1),
     (2, 3, 81, 44, 0, 32, PAD_REFLECT, 0),
 ]
-
-
-def _layer(case):
-    n, h, w, c0, c1, cout, pad, shift0 = case
-    return Layer(n, h, w, c0, cout, c1=c1, pad=pad, shift0=shift0)
-
-
-def twin(L):
-    """The same launch through index maps and a gate that select every pixel: the row-set kernel's rows."""
-    total = L.n * L.h * L.w
-    src0 = L.n * (L.h >> L.shift0) * (L.w >> L.shift0)
-    return Layer(L.n, L.h, L.w, L.c0, L.cout, c1=L.c1, pad=L.pad, shift0=L.shift0,
-                 map0=torch.arange(src0, dtype=torch.int32, device=DEV),
-                 map1=torch.arange(total, dtype=torch.int32, device=DEV) if L.c1 else None,
-                 gate=torch.ones(total, dtype=torch.uint8, device=DEV))
 
 
 def _shape(x, c, values, seed):
@@ -98,7 +81,7 @@ def launch(L, splits, ops_in):
 def test_too_wide_layers_run_the_gather_kernel_and_their_twins_the_rowset_kernel():
     launches = []
     for case in TOO_WIDE:
-        L = _layer(case)
+        L = dense_layer(case)
         launches += [(L, GATHER), (twin(L), SET)]
     inputs = [_operands(L, "mixed", "uniform", 1) for L, _ in launches]
     names = tc_kernels(lambda: [launch(L, 1, x) for (L, _), x in zip(launches, inputs)], len(launches))
@@ -110,7 +93,7 @@ def test_too_wide_layers_run_the_gather_kernel_and_their_twins_the_rowset_kernel
 @pytest.mark.parametrize("splits", [1, 0])
 @pytest.mark.parametrize("case", TOO_WIDE)
 def test_rowset_slot_split_gives_the_register_splits_bits(case, splits, dist, values):
-    L = _layer(case)
+    L = dense_layer(case)
     ops_in = _operands(L, dist, values, 5 * L.w + L.c0 + L.cout)
     y_reg, am_reg = launch(L, splits, ops_in)
     y_set, am_set = launch(twin(L), splits, ops_in)
@@ -128,10 +111,10 @@ def test_per_tap_fallback_gives_the_staged_forms_bits(layer, cout, values):
     """Raster order: tiles stage their distinct rows; permuted: the tiles' rows exceed a slot and are staged per tap
     (checked on the host for the plain list).  Whole tiles: a row's sum does not depend on its tile."""
     if layer == "plain_list":
-        pix = cr.pixel_list(_mask((2, 40, 64), 0.6, 26))
+        pix = cr.pixel_list(mask((2, 40, 64), 0.6, 26))
         L = Layer(2, 40, 64, 36, cout, pad=PAD_REPLICATE, pixels=pix, count=len(pix))
     else:
-        D = _decoder_like(2, 40, 64, 23)
+        D = decoder_like(2, 40, 64, 23)
         L = Layer(D.n, D.h, D.w, D.c0, cout, c1=D.c1, shift0=D.shift0, map0=D.map0, gate=D.gate, pixels=D.pixels,
                   count=D.count)
     g = torch.Generator().manual_seed(27)

@@ -32,6 +32,8 @@ from wavelet_monodepth_b200._lib import ACT_ELU, ACT_LRELU, ACT_NONE, ACT_SIGMOI
 
 import conv_grad_ref
 import conv_ref as cr
+from contract import Worst, errors
+from conv_launch import pack
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -40,21 +42,12 @@ ENGINES = ["f16x3", "tf32x3", "simt"]
 FLT_MAX = torch.finfo(torch.float32).max
 PARITY_TOL = 1e-4                 # oracle/parity.py: the float bar of the parity statement
 
-_WORST = {}
+WORST = Worst("engine, group, ratio")
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
-    yield
-    if _WORST:
-        print("\nworst per (engine, group, ratio): err / S, err / (BAR S + F)")
-        for k in sorted(_WORST, key=lambda k: (k[0], k[1], k[2])):
-            print("  %-7s %-14s %-8s %.2e  %.3f" % (k + tuple(_WORST[k])))
-
-
-def _note(engine, group, key, e_s, e_b):
-    w = _WORST.setdefault((engine, group, str(key)), [0.0, 0.0])
-    w[0], w[1] = max(w[0], e_s), max(w[1], e_b)
+    yield from WORST.module_report()
 
 
 def _amax(x):
@@ -62,12 +55,6 @@ def _amax(x):
     out = torch.zeros(1, device=DEV)
     ops.amax_rows(x, out)
     return out
-
-
-def _pack(wt, c1, engine):
-    if engine == "simt":
-        return ops.pack_weight(wt, c1, kind="simt")
-    return ops.pack_weight(wt, c1, kind="tc", precision=engine)
 
 
 class Geo:
@@ -90,7 +77,7 @@ class Geo:
 
 def run(engine, g, x0, x1, wt, b, amax0=None, amax1=None, pad=PAD_REFLECT, act=ACT_NONE):
     """y rows (rows, cout) of one launch; f16x3 takes the given maxima, or the library's own of each source."""
-    wp = _pack(wt, g.c1, engine)
+    wp = pack(wt, g.c1, engine)
     kw = {}
     if engine == "f16x3":
         kw["amax0"] = amax0 if amax0 is not None else _amax(x0)
@@ -118,29 +105,12 @@ def reference(engine, g, x0, x1, wt, b, maxima, pad=PAD_REFLECT, act=ACT_NONE):
 
 def check(engine, y, y64, s, f, group, key, act=ACT_NONE, pre64=None):
     """Non-finite exactly where y64 is; elsewhere |y - y64| <= BAR S + F (+ the activation's own error).  The tensor-core
-    engines may also give NaN where pre64 (the fp64 pre-activation) is non-finite: their split's remainder of an Inf is
-    Inf - Inf, so the activation sees NaN where ELU / sigmoid of +-Inf is finite (wmd.h)."""
-    bad64 = ~torch.isfinite(y64)
-    bad = ~torch.isfinite(y)
-    extra = bad & ~bad64
-    if engine != "simt" and pre64 is not None:
-        may = ~torch.isfinite(pre64)
-        assert bool(torch.isnan(y[extra]).all()) and bool(may[extra].all()), \
-            "%s %s %s: %d non-finite outputs where the pre-activation is finite" % (engine, group, key,
-                                                                                  int((extra & ~may).sum()))
-        extra = torch.zeros_like(extra)
-    assert not bool(extra.any()) and torch.equal(bad64 & bad, bad64), \
-        "%s %s %s: %d non-finite outputs where the reference has %d (%d differ)" % (
-            engine, group, key, int(bad.sum()), int(bad64.sum()), int((bad ^ bad64).sum()))
-    ok = ~bad
+    engines may also give NaN where pre64 (the fp64 pre-activation) is non-finite (contract.errors)."""
+    what = "%s %s %s" % (engine, group, key)
     allow = 0.0 if act in (ACT_NONE, ACT_LRELU) else cr.ACT_ALLOW
-    d = ((y.double() - y64).abs() - allow).clamp(min=0)[ok]
-    s, f = s[ok], f[ok]
-    bound = BAR[engine] * s + f
-    e_s = float((d / s.clamp(min=1e-300)).max()) if d.numel() else 0.0
-    e_b = float((d / bound).max()) if d.numel() else 0.0
-    _note(engine, group, key, e_s, e_b)
-    assert e_b <= 1.0, "%s %s %s: err / (BAR S + F) = %.3g (err / S = %.3g)" % (engine, group, key, e_b, e_s)
+    e_s, e_b = errors(y, y64, s, allow, floor=f, bar=BAR[engine], pre=pre64 if engine != "simt" else None, what=what)
+    WORST.note((engine, group, str(key)), e_s, e_b)
+    assert e_b <= 1.0, "%s: err / (BAR S + F) = %.3g (err / S = %.3g)" % (what, e_b, e_s)
 
 
 def _rand(shape, gen, lo=-1.0, hi=1.0):
@@ -385,11 +355,9 @@ def test_backward_data_gradient_with_dz_over_decades(layer, act, _fp32_convs):
     bars = conv_grad_ref.BARS
 
     def held(what, got, want, s, f, bar):
-        d = (got.double() - want).abs()
-        e_s = float((d / s.clamp(min=1e-300)).max())
-        e_b = float((d / (bar * s + f)).max())
-        _note("f16x3" if what.startswith("dx") else what, "bwd/" + ("sigmoid" if act == ACT_SIGMOID else "elu"),
-              name + ":" + what, e_s, e_b)
+        e_s, e_b = errors(got, want, s, floor=f, bar=bar, what=name + ":" + what)
+        WORST.note(("f16x3" if what.startswith("dx") else what, "bwd/" + ("sigmoid" if act == ACT_SIGMOID else "elu"),
+                    name + ":" + what), e_s, e_b)
         assert e_b <= 1.0, "%s %s: err / (BAR S + F) = %.3g (err / S = %.3g)" % (name, what, e_b, e_s)
 
     held("dx0", x0d.grad[:, :c0], *ref["x0"], floor["x0"], bars["dx0"])

@@ -9,61 +9,26 @@ pixel list in raster order (distinct rows staged) and randomly permuted (most ti
 same rows.  Every launch is also checked against the fp64 contract reference (tests/conv_ref.py) at the bars of
 test_gpu_conv_contract.py, with amax_out == max |y| and no writes outside [0, rows) x [0, cout).
 """
-import numpy as np
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
-from wavelet_monodepth_b200 import kitti_decoders as kd
-from wavelet_monodepth_b200 import ops, synth
 from wavelet_monodepth_b200._lib import PAD_REFLECT, PAD_REPLICATE, PAD_ZERO
 
 import conv_ref as cr
-from test_gpu_conv_contract import Layer, _mask, gather_layer, operands, run
+from conv_launch import (DEV, FLAGSHIP_DENSE, GATHER, SET, SET_ROWS, WIN, WORST, Layer, decoder_like, distinct_rows,
+                         flagship_tc_kernels, gather_layer, mask, operands, run, tc_kernels)
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-WIN, SET, GATHER = "conv_rows_tc_kernel_window", "conv_rows_tc_kernel_rowset", "conv_rows_tc_kernel"
-SET_ROWS = 480
 
 
-def tc_kernels(fn, launches):
-    """Names (window / row set / gather) of the tensor-core conv kernels fn launches, in launch order.  A short profiling
-    session can come back without some kernel records; it is taken again until it holds all `launches`.  (The window
-    tests' helper of the same name counts the row-set kernel as a gather kernel, by design of its name test.)"""
-    for _ in range(3):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        evs = sorted((e for e in prof.events()
-                      if e.device_type == torch.autograd.DeviceType.CUDA and GATHER in e.name),
-                     key=lambda e: e.time_range.start)
-        if len(evs) >= launches:
-            break
-    return [WIN if WIN in e.name else (SET if SET in e.name else GATHER) for e in evs]
+@pytest.fixture(scope="module", autouse=True)
+def _report():
+    yield from WORST.module_report()
 
 
 def _pixels(cells, w, h):
     """Flat pixel indices of (image, y, x) cells, ascending."""
     return torch.tensor(sorted(n * h * w + y * w + x for n, y, x in cells), dtype=torch.int32, device=DEV)
-
-
-def distinct_rows(pix, h, w, pad):
-    """Distinct source rows (shift 0, no map) that the nine taps of these pixels read: the row-set size of their tile."""
-    rows = set()
-    for p in pix.tolist():
-        n, y, x = p // (h * w), (p // w) % h, p % w
-        for dy in (-1, 0, 1):
-            for dx in (-1, 0, 1):
-                qy, qx = y + dy, x + dx
-                if pad == PAD_ZERO and not (0 <= qy < h and 0 <= qx < w):
-                    continue
-                if pad == PAD_REFLECT:
-                    qy, qx = abs(qy) if qy < h else 2 * h - 2 - qy, abs(qx) if qx < w else 2 * w - 2 - qx
-                qy, qx = min(max(qy, 0), h - 1), min(max(qx, 0), w - 1)
-                rows.add((n * h + qy) * w + qx)
-    return len(rows)
 
 
 def capacity_layer(extra):
@@ -80,7 +45,7 @@ def capacity_layer(extra):
 
 def straddle_layer():
     """A pixel list over two images whose second tile holds the end of image 0 and the start of image 1."""
-    m = _mask((2, 16, 24), 0.5, 21)
+    m = mask((2, 16, 24), 0.5, 21)
     pix = cr.pixel_list(m)
     assert int(m[0].sum()) % 128 != 0
     return Layer(2, 16, 24, 40, 96, c1=12, pixels=pix, count=len(pix))
@@ -93,7 +58,7 @@ def gated_pad_layer(pad):
 
 def scattered_layer():
     """A sparse list over a large image: a tile's rows span more than the bitmap (4096 rows), every tap is staged."""
-    pix = cr.pixel_list(_mask((1, 160, 160), 0.01, 22))
+    pix = cr.pixel_list(mask((1, 160, 160), 0.01, 22))
     return Layer(1, 160, 160, 32, 48, pixels=pix, count=len(pix))
 
 
@@ -107,7 +72,7 @@ def rowset_layer(case):
     if case == "scattered":
         return scattered_layer()
     if case == "count_zero":
-        return Layer(1, 16, 24, 64, 96, pixels=cr.pixel_list(_mask((1, 16, 24), 0.5, 12)), count=0)
+        return Layer(1, 16, 24, 64, 96, pixels=cr.pixel_list(mask((1, 16, 24), 0.5, 12)), count=0)
     if case.startswith("gated_"):
         return gated_pad_layer({"gated_zero": PAD_ZERO, "gated_reflect": PAD_REFLECT,
                                 "gated_replicate": PAD_REPLICATE}[case])
@@ -135,26 +100,17 @@ def test_rowset_balanced_meets_the_contract(case, engine, dist):
     run(rowset_layer(case), engine, dist, "gather", splits=0, seed=31)
 
 
-def _decoder_like(n, h, w, seed):
-    """sparse_upsample + sparse_conv3x3 of a decoder level: compact half-resolution x0, full-resolution skip x1, the
-    upsample mask as gate, the level's pixel list."""
-    s0 = _mask((n, h // 2, w // 2), 0.5, seed)
-    up = s0.repeat_interleave(2, 1).repeat_interleave(2, 2)
-    pix = cr.pixel_list(_mask((n, h, w), 0.6, seed + 1) * up)
-    return Layer(n, h, w, 40, 64, c1=24, shift0=1, map0=cr.index_map(s0), gate=up, pixels=pix, count=len(pix))
-
-
 @pytest.mark.parametrize("engine", ["f16x3", "tf32x3"])
 @pytest.mark.parametrize("layer", ["decoder_level", "compact_map1", "plain_list"])
 def test_permuted_pixel_list_gives_the_same_rows(layer, engine):
     if layer == "decoder_level":
-        L = _decoder_like(2, 40, 64, 23)
+        L = decoder_like(2, 40, 64, 23)
     elif layer == "compact_map1":
-        sel = _mask((2, 40, 64), 0.5, 24)
-        pix = cr.pixel_list(_mask((2, 40, 64), 0.4, 25))
+        sel = mask((2, 40, 64), 0.5, 24)
+        pix = cr.pixel_list(mask((2, 40, 64), 0.4, 25))
         L = Layer(2, 40, 64, 32, 48, c1=20, map1=cr.index_map(sel), pixels=pix, count=len(pix))
     else:
-        pix = cr.pixel_list(_mask((2, 40, 64), 0.3, 26))
+        pix = cr.pixel_list(mask((2, 40, 64), 0.3, 26))
         L = Layer(2, 40, 64, 36, 80, pad=PAD_REPLICATE, pixels=pix, count=len(pix))
     g = torch.Generator().manual_seed(27)
     perm = torch.randperm(L.count, generator=g).to(DEV)
@@ -184,22 +140,7 @@ def test_sparse_3x3_launches_run_the_rowset_kernel():
 
 
 def test_flagship_decoder_runs_its_sparse_3x3_launches_in_the_rowset_kernel():
-    mod = kd.SparseDepthWaveProgressiveDecoder(np.array(synth.RESNET50_CH))
-    synth.bench_kitti_params(mod)
-    mod = mod.to(DEV).eval()
-    feats = [f.to(DEV) for f in synth.bench_kitti_features(2, 320, 1024, synth.RESNET50_CH)]
-    mod(feats, 0.05)
-    prof = ops.Profiler()
-    ops.set_profiler(prof)
-    try:
-        mod(feats, 0.05)
-        torch.cuda.synchronize()
-    finally:
-        ops.set_profiler(None)
-    tc = [info for name, _, info in prof.results() if name == "conv_rows_tc"]
-    names = tc_kernels(lambda: mod(feats, 0.05), len(tc))
-    shapes = [(info["taps"], info["c0"], info["c1"], info["cout"]) for info in tc]
-    dense = ((9, 2048, 0, 256), (9, 256, 1024, 256))
-    want = [WIN if s in dense else (SET if s[0] == 9 else GATHER) for s in shapes]
+    shapes, names = flagship_tc_kernels()
+    want = [WIN if s in FLAGSHIP_DENSE else (SET if s[0] == 9 else GATHER) for s in shapes]
     assert want.count(SET) == 6, shapes
     assert names == want, list(zip(shapes, names))

@@ -12,8 +12,7 @@ import torch.nn.functional as F
 from wavelet_monodepth_b200 import ops
 from wavelet_monodepth_b200._lib import ACT_ELU, ACT_LRELU, PAD_REFLECT
 
-from helpers import REL_TOL, rel_err
-from test_gpu_kernels import _torch_conv, rnd
+from helpers import REL_TOL, rel_err, rnd, torch_conv
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -30,7 +29,7 @@ def test_tc_many_tiles_per_cta_two_sources_vs_torch(splits):
     lo, skip = rnd(n, c0, h // 2, w // 2, seed=120), rnd(n, c1, h, w, seed=121)
     wt, b = rnd(cout, c0 + c1, 3, 3, seed=122, lo=-0.05, hi=0.05), rnd(cout, seed=123)
     x = torch.cat([F.interpolate(lo, scale_factor=2, mode="nearest"), skip], 1)
-    want = _torch_conv(x.to(DEV).double(), wt.to(DEV).double(), b.to(DEV).double(), PAD_REFLECT, ACT_ELU)
+    want = torch_conv(x.to(DEV).double(), wt.to(DEV).double(), b.to(DEV).double(), PAD_REFLECT, ACT_ELU)
     lo_rows, skip_rows = ops.nchw_to_rows(lo.to(DEV)), ops.nchw_to_rows(skip.to(DEV))
     wp = ops.pack_weight(wt.to(DEV), c1, kind="tc")
     outs = [ops.conv_rows(lo_rows, c0, wp, b.to(DEV), cout, n, h, w, pad=PAD_REFLECT, act=ACT_ELU, shift0=1,

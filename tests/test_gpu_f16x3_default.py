@@ -15,10 +15,14 @@ import torch
 from wavelet_monodepth_b200 import kitti_decoders as kd
 from wavelet_monodepth_b200 import _lib, ops, synth
 
-from test_gpu_conv_contract import Layer, run, sm_count
+from conv_launch import DEV, WORST, Layer, run, sm_count
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _report():
+    yield from WORST.module_report()
 
 
 def _map_and_gate(n, c, h, w, p, seed):

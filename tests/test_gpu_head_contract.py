@@ -45,9 +45,10 @@ from wavelet_monodepth_b200._lib import ACT_ELU, ACT_NONE, ACT_SIGMOID, PAD_REFL
 
 import conv_ref as cr
 import head_ref as hr
+from contract import Worst, errors
+from conv_launch import DEV, mask, sm_count, uniform
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 
 BAR, BILINEAR_ULP = hr.BAR, hr.BILINEAR_ULP
 ACT_ALLOW = cr.ACT_ALLOW          # absolute error of the kernels' expf-based sigmoid / ELU
@@ -57,29 +58,12 @@ DISTS = ["mixed", "same"]
 PADS = [PAD_ZERO, PAD_REFLECT, PAD_REPLICATE]
 ERR_SHAPE, ERR_UNSUPPORTED = -2, -5
 
-_WORST = {}
+WORST = Worst("kernel, group, operands")
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
-    yield
-    if _WORST:
-        print("\nworst err / S per (kernel, group, operands):")
-        for k in sorted(_WORST):
-            bar = BAR.get(k[0])
-            print("  %-13s %-10s %-6s %.2e  (bar %s, %d launches)"
-                  % (k + (_WORST[k][0], "%.1e" % bar if bar else "-", _WORST[k][1])))
-
-
-def _record(kernel, group, dist, err):
-    was = _WORST.get((kernel, group, dist), (0.0, 0))
-    _WORST[(kernel, group, dist)] = (max(was[0], err), was[1] + 1)
-
-
-def _err(got, want, s, allow=0.0):
-    if got.numel() == 0:
-        return 0.0
-    return float(((got.double() - want).abs() - allow).clamp(min=0).div(s.clamp(min=1e-300)).max())
+    yield from WORST.module_report()
 
 
 def _gen(seed):
@@ -88,21 +72,8 @@ def _gen(seed):
     return g
 
 
-def _uniform(shape, lo, hi, g):
-    return torch.rand(shape, generator=g, device=DEV, dtype=torch.float32) * (hi - lo) + lo
-
-
-def _mask(shape, p, seed):
-    g = torch.Generator().manual_seed(seed)
-    return (torch.rand(shape, generator=g) < p).to(torch.uint8).to(DEV)
-
-
 def _status(excinfo):
     return "status %d," % excinfo
-
-
-def sm_count():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 class Geometry:
@@ -117,14 +88,14 @@ class Geometry:
         self.map = None
         self.in_rows = total
         if form == "map":
-            self.map = cr.index_map(_mask((n, h, w), 0.7, seed + 1))
+            self.map = cr.index_map(mask((n, h, w), 0.7, seed + 1))
             self.in_rows = max(int(self.map.max()) + 1, 1)
         if form == "dense":
             self.pixels, self.count, self.max_rows = None, None, total
             self.rows = total
             self.written = torch.arange(total, device=DEV)
             return
-        self.pixels = cr.pixel_list(_mask((n, h, w), 0.5, seed + 2))
+        self.pixels = cr.pixel_list(mask((n, h, w), 0.5, seed + 2))
         n_list = len(self.pixels)
         count, max_rows = {"all": (n_list, n_list), "lt": (max(n_list - 3, 0), n_list),
                            "gt": (n_list + 5, max(n_list - 2, 0)), "zero": (0, n_list)}[counts]
@@ -156,13 +127,13 @@ def run_conv(geo, c, cout, dual, act, pad, dist, group, ld=None, off_a=0, off_b=
     ld = ld if ld is not None else max(off_a + c, off_b + c if dual else 0) + 3
     lo = 0.0 if dist == "same" else -1.0
     t = torch.full((geo.in_rows, ld), PAD_GARBAGE, device=DEV)
-    t[:, off_a:off_a + c] = _uniform((geo.in_rows, c), lo, 1.0, g)
+    t[:, off_a:off_a + c] = uniform((geo.in_rows, c), lo, 1.0, g)
     if dual:
-        t[:, off_b:off_b + c] = _uniform((geo.in_rows, c), lo, 1.0, g)
+        t[:, off_b:off_b + c] = uniform((geo.in_rows, c), lo, 1.0, g)
     wlo, whi = (0.0, 2.0 / (9 * c)) if dist == "same" else (-1.0, 1.0)
-    wa, wb = _uniform((cout, c, 3, 3), wlo, whi, g), _uniform((cout, c, 3, 3), wlo, whi, g)
-    ba = _uniform((cout,), lo, 1.0, g) if bias else None
-    bb = _uniform((cout,), lo, 1.0, g) if bias else None
+    wa, wb = uniform((cout, c, 3, 3), wlo, whi, g), uniform((cout, c, 3, 3), wlo, whi, g)
+    ba = uniform((cout,), lo, 1.0, g) if bias else None
+    bb = uniform((cout,), lo, 1.0, g) if bias else None
     out = torch.full((n, cout, h, w), SENTINEL, device=DEV)
     kw = dict(off_b=off_b, wb=ops.pack_head_weight(wb), bb=bb) if dual else {}
     ops.head_conv3x3(t, c, off_a, ops.pack_head_weight(wa), ba, n, h, w, cout, scale=scale, act=act, pad=pad,
@@ -171,8 +142,8 @@ def run_conv(geo, c, cout, dual, act, pad, dist, group, ld=None, off_a=0, off_b=
     want, s = hr.head_conv3x3_ref(t, ld, c, off_a, off_b if dual else -1, wa, ba, wb, bb, cout, scale, act, pad, geo.map,
                                   geo.pixels, geo.count, geo.max_rows, n, h, w)
     allow = 0.0 if act == ACT_NONE else ACT_ALLOW * abs(scale) * (2 if dual else 1)
-    err = _err(got, want, s, allow)
-    _record("head_conv3x3", group, dist, err)
+    err = errors(got, want, s, allow)[0]
+    WORST.note(("head_conv3x3", group, dist), err, bar=BAR["head_conv3x3"])
     assert err <= BAR["head_conv3x3"], (group, dist, err)
     return out
 
@@ -244,7 +215,7 @@ def _z_rows(rows, ldz, col0, ncols, lo, g, storage_offset=0):
     [col0, col0 + ncols), PAD_GARBAGE elsewhere."""
     base = torch.full((rows * ldz + storage_offset,), PAD_GARBAGE, device=DEV)
     z = base[storage_offset:].view(rows, ldz)
-    z[:, col0:col0 + ncols] = _uniform((rows, ncols), lo, 1.0, g)
+    z[:, col0:col0 + ncols] = uniform((rows, ncols), lo, 1.0, g)
     return z
 
 
@@ -254,7 +225,7 @@ def run_gather(geo, groups, dual, act, pad, dist, group, col0=0, ldz=None, stora
     cout = groups // 2 if dual else groups
     ldz = ldz if ldz is not None else col0 + 9 * groups + 2
     lo = 0.0 if dist == "same" else -1.0
-    b = _uniform((groups,), lo, 1.0, g) if bias else None
+    b = uniform((groups,), lo, 1.0, g) if bias else None
     if z is None:
         z = _z_rows(geo.in_rows, ldz, col0, 9 * groups, lo, g, storage_offset)
     out = torch.full((geo.n, cout, geo.h, geo.w), SENTINEL, device=DEV)
@@ -264,8 +235,8 @@ def run_gather(geo, groups, dual, act, pad, dist, group, col0=0, ldz=None, stora
     want, s = hr.head_gather_ref(z, z.shape[1], col0, groups, geo.map, b, scale, act, dual, pad, geo.pixels, geo.count,
                                  geo.max_rows, cout, geo.n, geo.h, geo.w)
     allow = 0.0 if act == ACT_NONE else ACT_ALLOW * abs(scale) * (2 if dual else 1)
-    err = _err(got, want, s, allow)
-    _record("head_gather", group, dist, err)
+    err = errors(got, want, s, allow)[0]
+    WORST.note(("head_gather", group, dist), err, bar=BAR["head_gather"])
     assert err <= BAR["head_gather"], (group, dist, err)
     return out, z
 
@@ -311,13 +282,13 @@ def test_head_gather_column_offsets_and_strides(groups, dual, pad):
 # ============================================================================================ head_idwt
 def _idwt_operands(n, h, w, form, col0, ldz, seed, dist="mixed"):
     g = _gen(seed)
-    geo_map = cr.index_map(_mask((n, h, w), 0.7, seed + 1)) if form == "map" else None
+    geo_map = cr.index_map(mask((n, h, w), 0.7, seed + 1)) if form == "map" else None
     rows = max(int(geo_map.max()) + 1, 1) if geo_map is not None else n * h * w
     lo = 0.0 if dist == "same" else -1.0
     z = _z_rows(rows, ldz, col0, 54, lo, g)
     z[:, col0:col0 + 54] *= 3.0
-    bias = _uniform((6,), -1.0, 1.0, g)
-    ll = _uniform((n, 1, h, w), 0.0, 8.0, g)
+    bias = uniform((6,), -1.0, 1.0, g)
+    ll = uniform((n, 1, h, w), 0.0, 8.0, g)
     return z, geo_map, bias, ll
 
 
@@ -325,7 +296,7 @@ def _masks(kind, n, h, w, seed):
     if kind == "none":
         return None
     if kind == "random":
-        return _mask((n, h, w), 0.4, seed)
+        return mask((n, h, w), 0.4, seed)
     return torch.full((n, h, w), 1 if kind == "ones" else 0, dtype=torch.uint8, device=DEV)
 
 
@@ -364,9 +335,9 @@ def _check_idwt(res, z, col0, idxmap, mask, bias, scale, pad, ll, disp_scale, cl
     n, _, h, w = ll.shape
     ref = hr.head_idwt_ref(z, col0, idxmap, mask, bias, scale, pad, ll, disp_scale, clamp01, n, h, w)
     a = ACT_ALLOW * abs(scale)
-    err = max(_err(res["yh"], ref["yh"], ref["s_yh"], 2 * a), _err(res["out"], ref["out"], ref["s_out"], 3 * a),
-              _err(res["disp"], ref["disp"], ref["s_disp"], 3 * a * abs(disp_scale)))
-    _record("head_idwt", group, dist, err)
+    err = max(errors(res["yh"], ref["yh"], ref["s_yh"], 2 * a)[0], errors(res["out"], ref["out"], ref["s_out"], 3 * a)[0],
+              errors(res["disp"], ref["disp"], ref["s_disp"], 3 * a * abs(disp_scale))[0])
+    WORST.note(("head_idwt", group, dist), err, bar=BAR["head_idwt"])
     if mask is not None:
         off = (mask == 0)[:, None].expand(-1, 3, -1, -1)
         assert bool((res["yh"][off] == 0).all()), "coefficients outside the wavelet mask are not exactly zero"
@@ -463,8 +434,8 @@ def test_head_idwt_epilogues(w):
 def test_idwt_haar_epilogues(w):
     """The same two epilogues on the plain IDWT (both the float2 and the scalar kernel)."""
     g = _gen(41)
-    ll = _uniform((2, 1, 6, w), 0.0, 800.0, g)
-    hf = _uniform((2, 1, 3, 6, w), -50.0, 50.0, g)
+    ll = uniform((2, 1, 6, w), 0.0, 800.0, g)
+    hf = uniform((2, 1, 3, 6, w), -50.0, 50.0, g)
     out, disp, sd, depth = ops.idwt_haar(ll, hf, disp_scale=1e-3, clamp01=True, epilogue=("disp_to_depth", 0.1, 100.0))
     o2, d2 = ops.idwt_haar(ll, hf, disp_scale=1e-3, clamp01=True)
     assert torch.equal(out, o2) and torch.equal(disp, d2)
@@ -490,10 +461,10 @@ def run_mlp(c, max_rows, count, ldx, ldz, nz, bias, slope, mag, dist, group, see
     n1 = 2 * c
     lo = 0.0 if dist == "same" else -1.0
     x = torch.full((max(max_rows, 1), ldx), PAD_GARBAGE, device=DEV)
-    x[:, :c] = _uniform((x.shape[0], c), lo, 1.0, g) * mag
-    w1 = _uniform((n1, c, 1, 1), lo, 1.0, g) * (2.0 / c if dist == "same" else 1.0)
-    b1 = _uniform((n1,), lo, 1.0, g) * mag if bias else None
-    wz = _uniform((nz, n1, 1, 1), lo, 1.0, g) * (2.0 / n1 if dist == "same" else 1.0)
+    x[:, :c] = uniform((x.shape[0], c), lo, 1.0, g) * mag
+    w1 = uniform((n1, c, 1, 1), lo, 1.0, g) * (2.0 / c if dist == "same" else 1.0)
+    b1 = uniform((n1,), lo, 1.0, g) * mag if bias else None
+    wz = uniform((nz, n1, 1, 1), lo, 1.0, g) * (2.0 / n1 if dist == "same" else 1.0)
     packed = ops.pack_head_mlp(w1, b1, wz)
     z = torch.full((max_rows + 3, ldz), SENTINEL, device=DEV)
     cnt = torch.tensor([count], dtype=torch.int32, device=DEV) if count is not None else None
@@ -506,8 +477,8 @@ def run_mlp(c, max_rows, count, ldx, ldz, nz, bias, slope, mag, dist, group, see
     assert bool((z[:rows, 56:] == SENTINEL).all()), "columns past 56 were written"
     assert bool((z[:rows, nz:56] == 0).all()), "columns nz..55 are not zero"
     want, s = hr.head_mlp_ref(x, c, w1, b1, wz, slope, count, max_rows)
-    err = _err(z[:rows, :nz], want, s)
-    _record("head_mlp", group, dist, err)
+    err = errors(z[:rows, :nz], want, s)[0]
+    WORST.note(("head_mlp", group, dist), err, bar=BAR["head_mlp"])
     assert err <= BAR["head_mlp"], (group, dist, err)
 
 
@@ -543,12 +514,12 @@ def test_head_mlp_magnitudes(c, mag, bias, slope, dist):
 # ============================================================================================ idwt_bilinear
 def _bilinear_case(n, c, h, w, size, ac, clamp01, scale, seed):
     g = _gen(seed)
-    ll = _uniform((n, c, h, w), 0.0, 8.0, g)
-    hf = _uniform((n, c, 3, h, w), -2.0, 2.0, g)
+    ll = uniform((n, c, h, w), 0.0, 8.0, g)
+    hf = uniform((n, c, 3, h, w), -2.0, 2.0, g)
     got = ops.idwt_bilinear(ll, hf, size, disp_scale=scale, clamp01=clamp01, align_corners=ac)
     _, disp = ops.idwt_haar(ll, hf, disp_scale=scale, clamp01=clamp01)
     ulps = hr.bilinear_ulps(got, disp, size, ac)
-    _record("idwt_bilinear", "ulp", "mixed", ulps)
+    WORST.note(("idwt_bilinear", "ulp", "mixed"), ulps, bar=BILINEAR_ULP)
     assert ulps <= BILINEAR_ULP, ulps
 
 

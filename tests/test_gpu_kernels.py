@@ -16,15 +16,10 @@ from wavelet_monodepth_b200 import _lib, ops, wavelets
 from wavelet_monodepth_b200._lib import (ACT_ELU, ACT_LRELU, ACT_NONE, ACT_SIGMOID, PAD_REFLECT, PAD_REPLICATE,
                                          PAD_ZERO)
 
-from helpers import REL_TOL, rel_err
+from helpers import REL_TOL, rel_err, rnd, torch_conv
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def rnd(*shape, seed=0, lo=-1.0, hi=1.0):
-    rs = np.random.RandomState(seed)
-    return torch.from_numpy(rs.uniform(lo, hi, size=shape).astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------ Haar
@@ -182,13 +177,6 @@ def kind(request):
     return request.param
 
 
-def _torch_conv(x, wt, b, pad, act):
-    mode = {PAD_REFLECT: "reflect", PAD_REPLICATE: "replicate", PAD_ZERO: "constant"}[pad]
-    y = F.conv2d(F.pad(x, (1, 1, 1, 1), mode=mode), wt, b)
-    return {ACT_NONE: lambda t: t, ACT_ELU: F.elu, ACT_LRELU: lambda t: F.leaky_relu(t, 0.2),
-            ACT_SIGMOID: torch.sigmoid}[act](y)
-
-
 @pytest.mark.parametrize("n,cin,cout,h,w,pad,act", [
     (2, 64, 32, 12, 20, PAD_REFLECT, ACT_ELU),          # thin tile config
     (1, 96, 64, 9, 11, PAD_ZERO, ACT_LRELU),            # mid
@@ -199,7 +187,7 @@ def _torch_conv(x, wt, b, pad, act):
 ])
 def test_dense_conv_rows_vs_torch(n, cin, cout, h, w, pad, act, kind):
     x, wt, b = rnd(n, cin, h, w, seed=19), rnd(cout, cin, 3, 3, seed=20, lo=-0.1, hi=0.1), rnd(cout, seed=21)
-    want = _torch_conv(x, wt, b, pad, act)
+    want = torch_conv(x, wt, b, pad, act)
     y = ops.conv_rows(ops.nchw_to_rows(x.to(DEV)), cin, ops.pack_weight(wt.to(DEV), kind=kind), b.to(DEV), cout, n, h, w,
                       pad=pad, act=act, act_param=0.2)
     got = ops.rows_to_nchw(y, n, cout, h, w)
@@ -335,7 +323,7 @@ def test_tc_split_k_vs_torch(splits):
     """Split-K work items + fixed-order reduce pass give the same convolution (and are deterministic)."""
     n, cin, cout, h, w = 2, 160, 128, 9, 13
     x, wt, b = rnd(n, cin, h, w, seed=80), rnd(cout, cin, 3, 3, seed=81, lo=-0.1, hi=0.1), rnd(cout, seed=82)
-    want = _torch_conv(x, wt, b, PAD_REFLECT, ACT_ELU)
+    want = torch_conv(x, wt, b, PAD_REFLECT, ACT_ELU)
     rows, wp = ops.nchw_to_rows(x.to(DEV)), ops.pack_weight(wt.to(DEV), kind="tc")
     y = ops.conv_rows(rows, cin, wp, b.to(DEV), cout, n, h, w, pad=PAD_REFLECT, act=ACT_ELU, splits=splits)
     assert rel_err(ops.rows_to_nchw(y, n, cout, h, w), want) <= REL_TOL

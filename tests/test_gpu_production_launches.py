@@ -18,20 +18,14 @@ import torch
 from wavelet_monodepth_b200 import kitti_decoders as kd, nyu_decoders as nd, synth
 
 import launch_check as lc
+from workloads import D161, DEV, R18, R50, kitti_feats, nyu, same
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-NYU_HEADS = ["wave1.conv.", "wave2.conv.", "wave3.conv."]       # bench.py's NYU workload: high-pass heads x4
-R50 = (synth.RESNET50_CH, 320, 1024)
-R18 = (synth.RESNET18_CH, 192, 640)
-D161 = (synth.DENSENET161_CH, 480, 640)
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
-    yield
-    if lc.REPORT:
-        print("\n" + "\n".join(lc.report_lines()))
+    yield from lc.REPORT.module_report()
 
 
 @pytest.fixture(autouse=True)
@@ -42,27 +36,12 @@ def _fp32_convs():
     torch.backends.cudnn.allow_tf32 = prev
 
 
-def _kitti_feats(n, ch, h, w, layout="nchw"):
-    host = synth.bench_kitti_features(n, h, w, ch, pin=layout == "pinned")
-    if layout == "pinned":                          # the sparse levels' skip maps stay in pinned host memory
-        return [f if k < 3 else f.to(DEV) for k, f in enumerate(host)]
-    feats = [f.to(DEV) for f in host]
-    if layout == "channels_last":
-        feats = [f.contiguous(memory_format=torch.channels_last) for f in feats]
-    return feats
-
-
-def _nyu_feats(n, ch, h, w):
-    return [f.to(DEV) for f in synth.blocky_features(synth.nyu_feature_shapes(n, h, w, ch), seed=2000,
-                                                      cell=synth.BENCH_SYNTH["cell"], texture=synth.BENCH_SYNTH["texture"])]
-
-
 def kitti_sparse(n, spec, thr, layout="nchw"):
     def run():
         dec = kd.SparseDepthWaveProgressiveDecoder(np.array(spec[0]))
         synth.bench_kitti_params(dec)
         dec = dec.to(DEV).eval()
-        return dec(_kitti_feats(n, *spec, layout=layout), thr)
+        return dec(kitti_feats(n, *spec, layout=layout), thr)
     return run
 
 
@@ -71,7 +50,7 @@ def kitti_dense(n, spec):
         dec = kd.DepthWaveProgressiveDecoder(np.array(spec[0]))
         synth.bench_kitti_params(dec)
         with torch.no_grad():
-            return dec.to(DEV).eval()(_kitti_feats(n, *spec))
+            return dec.to(DEV).eval()(kitti_feats(n, *spec))
     return run
 
 
@@ -80,21 +59,7 @@ def kitti_baseline(n, spec):
         dec = kd.DepthDecoder(np.array(spec[0]))
         synth.load_random(dec, seed=7)
         with torch.no_grad():
-            return dec.to(DEV).eval()(_kitti_feats(n, *spec))
-    return run
-
-
-def nyu(cls, n, spec, thr=None):
-    def run():
-        dec = cls(enc_features=list(spec[0]), decoder_width=0.5)
-        if cls is nd.Decoder:
-            synth.load_random(dec, seed=11)
-        else:
-            synth.load_random(dec, seed=11, gains={k: synth.BENCH_SYNTH["head_gain"] for k in NYU_HEADS}, highpass=NYU_HEADS)
-        dec = dec.to(DEV).eval()
-        feats = _nyu_feats(n, *spec)
-        with torch.no_grad():
-            return dec(feats, thr) if thr is not None else dec(feats)
+            return dec.to(DEV).eval()(kitti_feats(n, *spec))
     return run
 
 
@@ -139,16 +104,6 @@ WORKLOADS = {
 }
 
 
-def _same(a, b, name):
-    assert set(a) == set(b), (name, sorted(map(str, set(a) ^ set(b))))
-    for k in a:
-        x, y = a[k], b[k]
-        if torch.is_tensor(x):
-            assert x.shape == y.shape and x.dtype == y.dtype and torch.equal(x, y), (name, k, "differs under the harness")
-        else:
-            assert x == y, (name, k, x, y)
-
-
 @pytest.mark.parametrize("name", list(WORKLOADS))
 def test_every_launch_meets_its_contract(name, monkeypatch):
     run = WORKLOADS[name]
@@ -158,7 +113,7 @@ def test_every_launch_meets_its_contract(name, monkeypatch):
     with harness.workload(name):
         checked = run()
     monkeypatch.undo()
-    _same(plain, checked, name)
+    same(plain, checked, name)
     print("%s: %s" % (name, ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
     del plain, checked, harness
     gc.collect()

@@ -21,6 +21,7 @@ import conv_grad_ref
 import conv_ref as cr
 import disp_tail_ref
 import head_ref as hr
+from contract import Worst, errors
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -28,30 +29,20 @@ _f64 = torch.float64
 FLT_MAX = torch.finfo(torch.float32).max
 EXPS = [-126, -100, -60, 0, 60, 100, 128]      # 128: maxima up to FLT_MAX = (1 - 2^-24) 2^128
 
-_WORST = {}
+WORST = Worst("kernel, group, case")
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
-    yield
-    if _WORST:
-        print("\nworst per (kernel, group, case): err / S, err / (BAR S + F)")
-        for k in sorted(_WORST):
-            print("  %-13s %-10s %-12s %.2e  %.3f" % (k + tuple(_WORST[k])))
+    yield from WORST.module_report()
 
 
 def check(kernel, group, key, got, want, s, f, bar, allow=0.0):
-    """Finite where want is; |got - want| <= bar S + F + allow there."""
-    ok = torch.isfinite(want)
-    assert bool(torch.isfinite(got[ok]).all()), "%s %s %s: non-finite outputs where the reference is finite" % (
-        kernel, group, key)
-    d = ((got.double() - want).abs() - allow).clamp(min=0)[ok]
-    s, f = s.expand_as(want)[ok], f.expand_as(want)[ok]
-    e_s = float((d / s.clamp(min=1e-300)).max()) if d.numel() else 0.0
-    e_b = float((d / (bar * s + f)).max()) if d.numel() else 0.0
-    w = _WORST.setdefault((kernel, group, str(key)), [0.0, 0.0])
-    w[0], w[1] = max(w[0], e_s), max(w[1], e_b)
-    assert e_b <= 1.0, "%s %s %s: err / (BAR S + F) = %.3g (err / S = %.3g)" % (kernel, group, key, e_b, e_s)
+    """Non-finite exactly where want is; |got - want| <= bar S + F + allow elsewhere."""
+    what = "%s %s %s" % (kernel, group, key)
+    e_s, e_b = errors(got, want, s, allow, floor=f, bar=bar, what=what)
+    WORST.note((kernel, group, str(key)), e_s, e_b)
+    assert e_b <= 1.0, "%s: err / (BAR S + F) = %.3g (err / S = %.3g)" % (what, e_b, e_s)
 
 
 def _rand(shape, gen, e):

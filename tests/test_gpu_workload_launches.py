@@ -32,12 +32,10 @@ from wavelet_monodepth_b200.kitti_loss import KittiDepthHintsLoss
 from wavelet_monodepth_b200.nyu_loss import NyuDepthLoss
 
 import launch_check as lc
-import test_gpu_production_launches as prod
+from workloads import D161, DEV, R18, R50, kitti_feats, nyu, same
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 MNV2_LIGHT_CH = (32, 24, 32, 64, 160)
-D161, R18, R50 = prod.D161, prod.R18, prod.R50
 D161_224 = (synth.DENSENET161_CH, 224, 224)
 MNV2_224 = (MNV2_LIGHT_CH, 224, 224)
 EVAL_FRAMES = 16
@@ -45,9 +43,7 @@ EVAL_FRAMES = 16
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
-    yield
-    if lc.REPORT:
-        print("\n" + "\n".join(lc.report_lines()))
+    yield from lc.REPORT.module_report()
 
 
 @pytest.fixture(autouse=True)
@@ -91,7 +87,7 @@ def kitti_no_skips(n, spec):
         dec = kd.DepthWaveProgressiveDecoder(np.array(ch), use_skips=False)
         synth.bench_kitti_params(dec)
         with torch.no_grad():
-            return dec.to(DEV).eval()(prod._kitti_feats(n, *spec))
+            return dec.to(DEV).eval()(kitti_feats(n, *spec))
     return run
 
 
@@ -206,7 +202,7 @@ def kitti_eval_pp(n, spec):
         dec = kd.SparseDepthWaveProgressiveDecoder(np.array(ch))
         synth.bench_kitti_params(dec)
         dec = dec.to(DEV).eval()
-        feats = prod._kitti_feats(n, *spec)
+        feats = kitti_feats(n, *spec)
         with torch.no_grad():
             left = dec(feats, 0.05)[("disp", 0)][:, 0]
             right = dec([torch.flip(f, [3]) for f in feats], 0.05)[("disp", 0)][:, 0]
@@ -236,8 +232,8 @@ WORKLOADS = {
                                                               8, R50),
     "train_baseline_r18_640x192_x12_kittiloss": train_kitti_loss(lambda ch: kd.DepthDecoder(np.array(ch)), 12, R18),
     "dense_no_skips_r18_640x192_x16": kitti_no_skips(16, R18),
-    "nyu_sparse_d161_640x480_x8_thr0": prod.nyu(nd.SparseDecoderWave, 8, D161, 0.0),
-    "nyu_sparse_d161_640x480_x8_thr0.5": prod.nyu(nd.SparseDecoderWave, 8, D161, 0.5),
+    "nyu_sparse_d161_640x480_x8_thr0": nyu(nd.SparseDecoderWave, 8, D161, 0.0),
+    "nyu_sparse_d161_640x480_x8_thr0.5": nyu(nd.SparseDecoderWave, 8, D161, 0.5),
     "eval_nyu_sparse_d161_x%d_edges" % EVAL_FRAMES: nyu_eval_edges(EVAL_FRAMES, D161),
     "eval_nyu_wave224_mnv2light_x8": nyu_eval_224(8, MNV2_224),
     "eval_kitti_sparse_r18_x%d_postprocess" % EVAL_FRAMES: kitti_eval_pp(EVAL_FRAMES, R18),
@@ -256,7 +252,7 @@ def test_every_launch_meets_its_contract(name, monkeypatch):
         checked = {k: _raw(v) if torch.is_tensor(v) else v for k, v in run().items()}
     monkeypatch.undo()
     t2 = time.perf_counter()
-    prod._same(plain, checked, name)
+    same(plain, checked, name)
     print("%s (%.1f s plain, %.1f s checked): %s" % (name, t1 - t0, t2 - t1,
                                                      ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
     del plain, checked, harness

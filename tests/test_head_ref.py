@@ -12,7 +12,7 @@ from oracle import sparse_ops as osp
 
 import conv_ref as cr
 import head_ref as hr
-from test_conv_ref import close, rnd, rows_of
+from helpers import close, rnd, rows_of
 
 _MODE = {cr.PAD_ZERO: "constant", cr.PAD_REFLECT: "reflect", cr.PAD_REPLICATE: "replicate"}
 _ACT = {cr.ACT_NONE: lambda v: v, cr.ACT_ELU: F.elu, cr.ACT_SIGMOID: torch.sigmoid}

@@ -8,7 +8,7 @@ import torch
 from oracle import baseline
 from wavelet_monodepth_b200 import kitti_decoders as kd, nyu_decoders as nd
 
-from helpers import key_str, kitti_features, load_golden, nyu_features, seeded_params
+from helpers import key_str, kitti_features, kitti_variant, load_golden, nyu_features, seeded_params
 
 GOLDEN_THREADS = 8   # intra-op threads of the run that recorded the fixtures (see test_oracle_golden.py)
 
@@ -22,12 +22,6 @@ def _no_grad():
             yield
     finally:
         torch.set_num_threads(was)
-
-
-def kitti_variant(want, meta, name):
-    """(constructor kwargs, the variant's arrays keyed by key_str) of one DepthDecoder variant of the KITTI fixture."""
-    prefix = name + "__"
-    return meta["variants"][name], {k[len(prefix):]: v for k, v in want.items() if k.startswith(prefix)}
 
 
 def _exact(got, want, what):
