@@ -66,6 +66,7 @@ long long wmd_launch_count(void);
  *   the dependency's separable order (two 1/sqrt2 passes) so results are bit-equal to it.
  * Fused consumer (optional, disp may be NULL):
  *   disp  (N,C,2H,2W) = out * disp_scale, clamped to [0,1] if clamp01   (depth_decoder.py:166)
+ * The clamp propagates NaN as torch.clamp does: a NaN reconstruction gives a NaN disparity, not 0.
  */
 int wmd_idwt_haar_f32(const float* ll, const float* hf, float* out, float* disp, float disp_scale, int clamp01,
                       int N, int C, int H, int W, wmd_stream_t stream);
@@ -76,7 +77,8 @@ int wmd_idwt_haar_f32(const float* ll, const float* hf, float* out, float* disp,
  * NYUv2/utils.py:223-227, NYUv2/train.py:305-306 (align_corners=True).  The intermediate disp plane is not read
  * back from HBM.  Upsampling only, by about 1.6x per axis or more: with sy, sx = source / destination size per axis (the
  * disp plane is 2H x 2W), a 32 x 128 output tile's source patch must fit 2048 floats, (floor(32 sy) + 4) (floor(128 sx)
- * + 4) <= 2048; smaller factors (equal sizes, 1.5x) return WMD_ERR_UNSUPPORTED. */
+ * + 4) <= 2048; smaller factors (equal sizes, 1.5x) return WMD_ERR_UNSUPPORTED.  The clamp propagates NaN as
+ * torch.clamp does, so a NaN disparity spreads into the outputs that read it. */
 int wmd_idwt_bilinear_f32(const float* ll, const float* hf, float* full, float disp_scale, int clamp01, int full_h,
                           int full_w, int align_corners, int N, int C, int H, int W, wmd_stream_t stream);
 
@@ -349,7 +351,8 @@ typedef struct wmd_head_idwt_desc {
   float disp_scale;
   int32_t clamp01;
   int32_t epi_mode;          /* WMD_EPI_*: DISP_TO_DEPTH: epi_out0 = epi_a + epi_b * disp, epi_out1 = 1 / epi_out0 (nullable);
-                                DIV_CLAMP: epi_out0 = out / epi_a, clamped to [epi_lo, epi_hi] if epi_b != 0 */
+                                DIV_CLAMP: epi_out0 = out / epi_a, clamped to [epi_lo, epi_hi] if epi_b != 0.
+                                The disparity clamp and DIV_CLAMP propagate NaN as torch.clamp does */
   float epi_a, epi_b, epi_lo, epi_hi;
   float* epi_out0;
   float* epi_out1;

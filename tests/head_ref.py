@@ -21,6 +21,10 @@ _f64 = torch.float64
 # err / S bars of the head kernels and idwt_bilinear's bound (measurements and error model: tests/test_gpu_head_contract.py)
 BAR = {"head_conv3x3": 4e-7, "head_gather": 4.5e-7, "head_idwt": 4.5e-7, "head_mlp": 4e-6}
 BILINEAR_ULP = 2.5                # units of 2^-23 x the largest |disp| around the four neighbours
+# idwt_bilinear's absolute floor: |err| <= BILINEAR_ULP 2^-23 max|disp| + BILINEAR_FLOOR.  The blend is six products; one
+# that lands among the subnormals may lose up to 2^-150 beyond its relative error (sums of subnormals are exact):
+# 6 x 2^-150 = 3 x 2^-149
+BILINEAR_FLOOR = 3 * 2.0 ** -149
 
 
 def _rows(n, h, w, pixels, count, max_rows):
@@ -136,13 +140,20 @@ def head_mlp_ref(x, c, w1, b1, wz, slope, count, max_rows, floor=False):
 
 
 def bilinear_ulps(got, disp, size, align_corners):
-    """Worst |got - F.interpolate(disp)| of a bilinear resize in units of 2^-23 x the largest |disp| of the 3 x 3 window
-    around each output's top-left neighbour (a bound of the four neighbours it mixes).  disp (N, C, h, w) on got's device;
-    the interpolation runs in disp's dtype."""
+    """Worst |got - F.interpolate(disp)| of a bilinear resize in units of 2^-23 x the largest finite |disp| of the 3 x 3
+    window around each output's top-left neighbour (a bound of the four neighbours it mixes), plus BILINEAR_FLOOR /
+    BILINEAR_ULP: at most BILINEAR_ULP exactly when |err| <= BILINEAR_ULP 2^-23 max|disp| + BILINEAR_FLOOR.  disp
+    (N, C, h, w) on got's device; the interpolation runs in disp's dtype.  got must be NaN, +Inf and -Inf exactly where torch's resize is: a
+    non-finite neighbour reaches even the outputs that give it zero weight (0 x NaN, 0 x Inf)."""
     dev = got.device
     want = F.interpolate(disp, size=size, mode="bilinear", align_corners=align_corners)
+    assert got.shape == want.shape
+    g = got.to(want.dtype)
+    for what, f in (("NaN", torch.isnan), ("+Inf", lambda t: t == float("inf")), ("-Inf", lambda t: t == -float("inf"))):
+        assert torch.equal(f(g), f(want)), "bilinear: %d %s outputs where torch's resize has %d" % (
+            int(f(g).sum()), what, int(f(want).sum()))
     hs, ws = disp.shape[-2:]
-    m = F.max_pool2d(disp.abs(), 3, stride=1, padding=1)
+    m = F.max_pool2d(torch.where(torch.isfinite(disp), disp.abs(), torch.zeros_like(disp)), 3, stride=1, padding=1)
     ys, xs = torch.arange(size[0], device=dev, dtype=_f64), torch.arange(size[1], device=dev, dtype=_f64)
     if align_corners:
         fy = ys * ((hs - 1) / max(size[0] - 1, 1))
@@ -152,5 +163,7 @@ def bilinear_ulps(got, disp, size, align_corners):
         fx = ((xs + 0.5) * (ws / size[1]) - 0.5).clamp(min=0)
     y0, x0 = fy.floor().long().clamp(max=hs - 1), fx.floor().long().clamp(max=ws - 1)
     mag = m[:, :, y0][:, :, :, x0]
-    assert got.shape == want.shape
-    return float(((got.to(want.dtype) - want).abs() / (mag * 2.0 ** -23).clamp(min=1e-38)).max())
+    ok = torch.isfinite(want)
+    if not bool(ok.any()):
+        return 0.0
+    return float(((g - want).abs() / (mag * 2.0 ** -23 + BILINEAR_FLOOR / BILINEAR_ULP))[ok].max())

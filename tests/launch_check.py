@@ -38,6 +38,7 @@ from wavelet_monodepth_b200 import _lib, kitti_eval, kitti_loss, nyu_eval, nyu_l
 import conv_grad_ref
 import conv_ref as cr
 import disp_tail_ref
+import haar_ref as har
 import head_ref as hr
 from contract import Worst, errors
 
@@ -152,7 +153,6 @@ SYMBOLS = {
 }
 
 # bars of the checks this file adds on top of the contract tests' (units of 2^-24 of the element's scale)
-DWT_ULP = 8            # four roundings on each path of a one-level analysis bound the error by 4 x 2^-24 S; twice that
 ACT_BWD_ULP = 4        # dz = dy act'(y): at most three roundings (sigmoid: 1 - y, y (1 - y), the product with dy)
 # bars of the evaluation and loss checks: those of their own tests (test_gpu_nyu_loss, test_gpu_nyu_eval,
 # test_gpu_nyu_edges, test_gpu_kitti_eval, test_gpu_kitti_loss)
@@ -450,25 +450,17 @@ class Harness:
         if a["thresh_ratio"] is not None:
             o = res["out"].reshape(n, -1)
             want = (o.amax(1) - o.amin(1)) * torch.tensor(a["thresh_ratio"], dtype=_f32, device=o.device)
-            _require(torch.equal(res["thresh"], want), "head_idwt: threshold is not (max - min)(out) * ratio")
+            _require(har.same_bits(res["thresh"], want), "head_idwt: threshold is not (max - min)(out) * ratio")
         self._check_epilogue("head_idwt", a["epilogue"], res["out"], res["disp"],
                              [res[k] for k in ("scaled_disp", "depth") if k in res])
 
     def _check_epilogue(self, entry, epi, out, disp, planes):
-        """The consumer epilogue planes against the torch expressions on the kernel's own reconstruction / disparity."""
+        """The consumer epilogue planes against the torch expressions on the kernel's own reconstruction / disparity: NaN
+        exactly where they are NaN, and equal values elsewhere."""
         if epi is None:
             return
-        if epi[0] == "disp_to_depth":
-            lo, span = 1 / float(epi[2]), 1 / float(epi[1]) - 1 / float(epi[2])
-            scaled = torch.tensor(lo, dtype=_f32, device=disp.device) + torch.tensor(span, dtype=_f32, device=disp.device) * disp
-            _require(torch.equal(planes[0], scaled), "%s: scaled_disp plane" % entry)
-            if len(planes) > 1:
-                _require(torch.equal(planes[1], 1 / scaled), "%s: depth plane" % entry)
-        else:
-            v = out * (torch.tensor(1.0, dtype=_f32) / torch.tensor(float(epi[1]), dtype=_f32)).to(out.device)
-            if epi[2] is not None:
-                v = torch.clamp(v, min=float(epi[2]), max=float(epi[3]))
-            _require(torch.equal(planes[0], v), "%s: div_clamp depth plane" % entry)
+        for p, want in zip(planes, epilogue_ref(epi, out, disp)):
+            _require(har.same_values(p, want), "%s: %s epilogue plane" % (entry, epi[0]))
 
     # ------------------------------------------------------------------------------------------ Haar transforms
     def _oracle_idwt(self, ll, hf):
@@ -476,44 +468,43 @@ class Harness:
         return ohaar.DWTInverse("haar", "zero")((ll.detach().float().cpu(), [hf.detach().float().cpu()]))
 
     def _check_idwt_haar(self, a, res, pre):
+        """The reconstruction bit for bit (NaN where the oracle's is NaN), the disparity and epilogue planes by value."""
         ll, hf = a["ll"], a["hf"]
         n, c, h, w = ll.shape
         res_t = res if isinstance(res, tuple) else (res,)
         want = self._oracle_idwt(ll, hf.reshape(n, c, 3, h, w))
-        _require(torch.equal(res_t[0].cpu(), want), "idwt_haar: reconstruction differs from oracle.haar.DWTInverse")
-        scale = torch.tensor(a["disp_scale"] if a["disp_scale"] is not None else 1.0, dtype=_f32)
-        disp = want * scale
-        if a["clamp01"]:
-            disp = disp.clamp(0.0, 1.0)
+        _require(har.same_bits(res_t[0], want), "idwt_haar: reconstruction differs from oracle.haar.DWTInverse")
+        disp = har.disp(want, a["disp_scale"] if a["disp_scale"] is not None else 1.0, a["clamp01"])
         k = 1
         if a["disp_scale"] is not None:
-            _require(torch.equal(res_t[1].cpu(), disp), "idwt_haar: disparity plane")
+            _require(har.same_values(res_t[1], disp), "idwt_haar: disparity plane")
             k = 2
         if a["epilogue"] is not None:
             self._check_epilogue("idwt_haar", a["epilogue"], res_t[0], disp.to(res_t[0].device), list(res_t[k:]))
         _record("idwt_haar", "fp32", "-", 0.0, 0, n * c * h * w)
 
     def _check_dwt_haar(self, a, res, pre):
-        """One analysis level against oracle.haar in fp64: |err| <= DWT_ULP 2^-24 S, S = 1/2 the sum of the four |x|."""
+        """One analysis level against oracle.haar in fp64: |err| <= DWT_ULP 2^-24 S + DWT_FLOOR, S = 1/2 the sum of the four
+        |x| (haar_ref)."""
         x = a["x"]
         ll, hf = res
         n, c, hh, ww = x.shape
         x64 = x.detach().double()
         rl, rh = ohaar.DWTForward(J=1, wave="haar", mode="zero").to(x.device).double()(x64)
         sc = 0.5 * F.avg_pool2d(x64.abs(), 2) * 4
-        err = max(errors(ll, rl, sc)[0], errors(hf, rh[0], sc.unsqueeze(2).expand_as(rh[0]))[0])
-        bar = DWT_ULP * EPS
+        bar = har.DWT_ULP * EPS
+        e_l, f_l = errors(ll, rl, sc, floor=har.DWT_FLOOR, bar=bar)
+        e_h, f_h = errors(hf, rh[0], sc.unsqueeze(2).expand_as(rh[0]), floor=har.DWT_FLOOR, bar=bar)
         ol, oh = ohaar.DWTForward(J=1, wave="haar", mode="zero")(x.detach().float().cpu())
-        exact = torch.equal(ll.cpu(), ol) and torch.equal(hf.cpu(), oh[0])
-        _record("dwt_haar", "fp32", "exact" if exact else "bounded", err, bar, n * c * hh * ww // 4)
-        _require(err <= bar, "%s: dwt_haar err/S %.3g > %.3g" % (self.current, err, bar))
+        exact = har.same_bits(ll, ol) and har.same_bits(hf, oh[0])
+        REPORT.note(("dwt_haar", "fp32", "exact" if exact else "bounded"), max(e_l, e_h), max(f_l, f_h), bar=bar,
+                    rows=n * c * hh * ww // 4)
+        _require(max(f_l, f_h) <= 1, "%s: dwt_haar err %.3g > DWT_ULP 2^-24 S + DWT_FLOOR" % (self.current, max(f_l, f_h)))
 
     def _check_idwt_bilinear(self, a, full, pre):
         ll, hf, size, ac = a["ll"], a["hf"], a["size"], bool(a["align_corners"])
         n, c, h, w = ll.shape
-        disp = self._oracle_idwt(ll, hf.reshape(n, c, 3, h, w)) * torch.tensor(a["disp_scale"], dtype=_f32)
-        if a["clamp01"]:
-            disp = disp.clamp(0.0, 1.0)
+        disp = har.disp(self._oracle_idwt(ll, hf.reshape(n, c, 3, h, w)), a["disp_scale"], a["clamp01"])
         disp = disp.to(full.device).double()
         ulps = hr.bilinear_ulps(full, disp, size, ac)
         _record("idwt_bilinear", "fp32", "ac" if ac else "-", ulps, hr.BILINEAR_ULP, full.numel())
@@ -547,16 +538,11 @@ class Harness:
         if a["thresh"] is not None:
             yh = a["yh"]
             n, h, w = yh.shape[0], yh.shape[-2], yh.shape[-1]
-            s0 = yh.reshape(n, 3, h, w).abs().amax(1, keepdim=True) > a["thresh"].reshape(n, 1, 1, 1)
         else:
-            n, h, w = a["n"], a["h"], a["w"]
-            s0 = torch.ones((n, 1, h, w), dtype=torch.bool, device=a["device"])
-        f = s0.float()
-        s5 = f.repeat_interleave(2, 2).repeat_interleave(2, 3)
-        want = {"S0": f, "S1": F.max_pool2d(f, 3, 1, 1), "S2": F.max_pool2d(f, 5, 1, 2),
-                "S5": s5, "S4": F.max_pool2d(s5, 3, 1, 1), "S3": F.max_pool2d(s5, 5, 1, 2)}
+            yh, n, h, w = None, a["n"], a["h"], a["w"]
+        want = level_masks_ref(yh, a["thresh"], n, h, w, a["device"])
         for k, m in res.items():
-            _require(torch.equal(m, want[k].to(torch.uint8)), "level_masks: %s" % k)
+            _require(torch.equal(m, want[k]), "level_masks: %s" % k)
         _record("level_masks", "-", "-", 0.0, 0, n * h * w)
 
     def _check_compact(self, a, res, pre):
@@ -1001,6 +987,34 @@ class Harness:
         err = _rel_err(_np(out), want, "compute_errors")
         _record("compute_errors", "fp64", "-", err, EVAL_REL, a["gt"].numel())
         _require(err <= EVAL_REL, "%s: compute_errors err %.3g > %.3g" % (self.current, err, EVAL_REL))
+
+
+def epilogue_ref(epi, out, disp):
+    """The consumer epilogue planes in torch on a reconstruction and its disparity: disp_to_depth (KITTI/layers.py:16-25)
+    -> [scaled_disp, depth], div_clamp (NYUv2/utils.py:219,229) -> [depth].  torch.clamp keeps a NaN."""
+    if epi[0] == "disp_to_depth":
+        lo, span = 1 / float(epi[2]), 1 / float(epi[1]) - 1 / float(epi[2])
+        scaled = torch.tensor(lo, dtype=_f32, device=disp.device) + torch.tensor(span, dtype=_f32, device=disp.device) * disp
+        return [scaled, 1 / scaled]
+    v = out * (torch.tensor(1.0, dtype=_f32) / torch.tensor(float(epi[1]), dtype=_f32)).to(out.device)
+    if epi[2] is not None:
+        v = torch.clamp(v, min=float(epi[2]), max=float(epi[3]))
+    return [v]
+
+
+def level_masks_ref(yh, thresh, n, h, w, device):
+    """The six pixel sets of wmd_level_masks in torch, uint8 (N, 1, H, W) / (N, 1, 2H, 2W): S0 = max_band |yh| > thresh (a
+    NaN band or threshold sets no bit), S1 / S2 its 3x3 / 5x5 dilations, S5 = up2(S0), S4 / S3 up2(S0)'s 3x3 / 5x5
+    dilations; thresh None: every S0 bit set."""
+    if thresh is not None:
+        s0 = yh.reshape(n, 3, h, w).abs().amax(1, keepdim=True) > thresh.reshape(n, 1, 1, 1)
+    else:
+        s0 = torch.ones((n, 1, h, w), dtype=torch.bool, device=device)
+    f = s0.float()
+    s5 = f.repeat_interleave(2, 2).repeat_interleave(2, 3)
+    want = {"S0": f, "S1": F.max_pool2d(f, 3, 1, 1), "S2": F.max_pool2d(f, 5, 1, 2),
+            "S5": s5, "S4": F.max_pool2d(s5, 3, 1, 1), "S3": F.max_pool2d(s5, 5, 1, 2)}
+    return {k: v.to(torch.uint8) for k, v in want.items()}
 
 
 def _np(t):

@@ -215,3 +215,38 @@ def test_head_mlp_matches_matmuls(c, nz, count):
     z0, _ = hr.head_mlp_ref(x, c, w1, None, wz, 0.2, None, rows)
     pre0 = x[:, :c].double() @ w1.double()[:, :, 0, 0].T
     assert close(z0, torch.where(pre0 > 0, pre0, 0.2 * pre0) @ wz.double()[:, :, 0, 0].T)
+
+
+@pytest.mark.parametrize("ac", [False, True])
+@pytest.mark.parametrize("e", [-146, -140, -130, -127, 0])
+def test_bilinear_ulps_floor_rejects_flushed_and_doubled_outputs(e, ac):
+    """bilinear_ulps' bound BILINEAR_ULP 2^-23 max|disp| + BILINEAR_FLOOR: torch's own float32 resize of a plane of
+    subnormal (or normal) disparities, 6 x 2^-149 and up, meets it; the same output flushed to zero or doubled does not."""
+    rs = np.random.RandomState(61)
+    disp = torch.from_numpy((np.ldexp(rs.uniform(1.0, 1.5, (2, 1, 12, 20)), e) * 6).astype(np.float32))
+    size = (45, 77) if ac else (48, 80)
+    got = F.interpolate(disp, size=size, mode="bilinear", align_corners=ac)
+    d64 = disp.double()
+    assert hr.bilinear_ulps(got, d64, size, ac) <= hr.BILINEAR_ULP
+    assert hr.bilinear_ulps(torch.zeros_like(got), d64, size, ac) > hr.BILINEAR_ULP
+    assert hr.bilinear_ulps(2 * got, d64, size, ac) > hr.BILINEAR_ULP
+
+
+def test_bilinear_ulps_requires_torchs_non_finite_pattern():
+    disp = torch.rand(1, 1, 6, 8, dtype=torch.float64)
+    disp[0, 0, 2, 3] = float("nan")
+    disp[0, 0, 4, 6] = float("inf")
+    got = F.interpolate(disp, size=(24, 32), mode="bilinear", align_corners=False).float()
+    assert hr.bilinear_ulps(got, disp, (24, 32), False) <= hr.BILINEAR_ULP
+    spoiled = []
+    for v in (float("nan"), float("inf"), -float("inf")):          # a non-finite output where torch's is finite
+        g = got.clone()
+        g[0, 0, 20, 2] = v
+        spoiled.append(g)
+    for v in (0.5, -float("inf")):                                  # torch's NaN footprint made finite, or -Inf
+        g = got.clone()
+        g[torch.isnan(g)] = v
+        spoiled.append(g)
+    for g in spoiled:
+        with pytest.raises(AssertionError):
+            hr.bilinear_ulps(g, disp, (24, 32), False)

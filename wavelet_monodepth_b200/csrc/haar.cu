@@ -29,7 +29,7 @@ __device__ __forceinline__ Quad haar_synth(float ll, float lh, float hl, float h
 
 __device__ __forceinline__ float disp_of(float v, float scale, int clamp01) {
   v = __fmul_rn(v, scale);
-  return clamp01 ? fminf(fmaxf(v, 0.f), 1.f) : v;
+  return (clamp01 && v == v) ? fminf(fmaxf(v, 0.f), 1.f) : v;     // torch.clamp passes a NaN through; fmaxf would make it 0
 }
 
 // consumer epilogue of the reconstruction / its disparity plane (WMD_EPI_*, see wmd_head_idwt_desc)
@@ -48,7 +48,7 @@ __device__ __forceinline__ void epi_store(const EpiArgs& e, long long o, float r
     // torch on CUDA evaluates `t / python_scalar` as t * (1 / scalar) (one IEEE division of the scalar, then a multiply):
     // that is what the reference's `pred_y /= 100` computes where it runs (NYUv2/utils.py:219 after model.cuda())
     float v = __fmul_rn(recon, __fdiv_rn(1.f, e.a));
-    if (e.b != 0.f) v = fminf(fmaxf(v, e.lo), e.hi);
+    if (e.b != 0.f && v == v) v = fminf(fmaxf(v, e.lo), e.hi);   // NaN stays NaN, as in torch.clamp
     e.out0[o] = v;
   }
 }

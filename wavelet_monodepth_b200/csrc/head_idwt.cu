@@ -36,7 +36,7 @@ __device__ __forceinline__ void synth4(float ll, float lh, float hl, float hh, f
 
 __device__ __forceinline__ float disp_val(float v, float scale, int clamp01) {
   v = __fmul_rn(v, scale);
-  return clamp01 ? fminf(fmaxf(v, 0.f), 1.f) : v;
+  return (clamp01 && v == v) ? fminf(fmaxf(v, 0.f), 1.f) : v;     // torch.clamp passes a NaN through; fmaxf would make it 0
 }
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -50,7 +50,7 @@ __device__ __forceinline__ void epilogue(const wmd_head_idwt_desc& d, long long 
   } else if (d.epi_mode == WMD_EPI_DIV_CLAMP) {       // NYUv2/utils.py:219,229 on the reconstruction
     // torch on CUDA evaluates `t / python_scalar` as t * (1 / scalar): what the reference's `pred_y /= 100` computes
     float v = __fmul_rn(recon, __fdiv_rn(1.f, d.epi_a));
-    if (d.epi_b != 0.f) v = fminf(fmaxf(v, d.epi_lo), d.epi_hi);
+    if (d.epi_b != 0.f && v == v) v = fminf(fmaxf(v, d.epi_lo), d.epi_hi);   // NaN stays NaN, as in torch.clamp
     d.epi_out0[o] = v;
   }
 }
