@@ -199,6 +199,18 @@ KITTI_LOSS_SIGNATURES = {
                                    c_size_t, POINTER(c_void_p), c_void_p]),
 }
 
+# include/wmd_hints.h: KITTI's depth hints, the StereoSGBM matcher and the fusion (tests/test_kitti_hints_abi.py checks
+# this table against it)
+HINTS_SIGNATURES = {
+    "wmd_sgbm_ws_bytes": (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),
+    "wmd_sgbm_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p,
+                            c_size_t, c_void_p, c_void_p]),
+    "wmd_depth_hints_ws_bytes": (c_size_t, [c_int32, c_int32, c_int32]),
+    "wmd_depth_hints_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
+                                    c_int32, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
+}
+HINTS_MATCHERS = 12                       # WMD_HINTS_MATCHERS
+
 _lib = None
 
 
@@ -225,7 +237,7 @@ def load():
             except OSError:
                 continue
         lib = ctypes.CDLL(LIB_PATH)
-    tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES)
+    tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES)
     for name, (res, args) in [item for table in tables for item in table.items()]:
         fn = getattr(lib, name)
         fn.restype = res
