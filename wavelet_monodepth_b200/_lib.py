@@ -211,6 +211,24 @@ HINTS_SIGNATURES = {
 }
 HINTS_MATCHERS = 12                       # WMD_HINTS_MATCHERS
 
+
+class InputsDesc(Structure):
+    """struct wmd_inputs_desc (include/wmd_inputs.h)."""
+    _fields_ = [("N", c_int32), ("src_h", c_int32), ("src_w", c_int32), ("n_scales", c_int32),
+                ("out_h", c_int32 * 4), ("out_w", c_int32 * 4),
+                ("src", c_void_p), ("views", c_void_p), ("xtab", c_void_p * 4), ("ytab", c_void_p * 4),
+                ("xk", c_int32 * 4), ("yk", c_int32 * 4), ("jitter", c_void_p),
+                ("color", c_void_p * 4), ("color_aug", c_void_p * 4)]
+
+
+# include/wmd_inputs.h: KITTI's training inputs, the LANCZOS pyramid, colour jitter and ToTensor
+# (tests/test_kitti_inputs_oracle.py checks this table against it)
+INPUTS_SIGNATURES = {
+    "wmd_inputs_ws_bytes": (c_size_t, [POINTER(InputsDesc)]),
+    "wmd_inputs_u8": (c_int, [POINTER(InputsDesc), c_void_p, c_size_t, c_void_p]),
+}
+INPUTS_MAX_SCALES = 4                     # WMD_INPUTS_MAX_SCALES
+
 _lib = None
 
 
@@ -237,7 +255,8 @@ def load():
             except OSError:
                 continue
         lib = ctypes.CDLL(LIB_PATH)
-    tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES)
+    tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES,
+              INPUTS_SIGNATURES)
     for name, (res, args) in [item for table in tables for item in table.items()]:
         fn = getattr(lib, name)
         fn.restype = res
