@@ -229,6 +229,24 @@ INPUTS_SIGNATURES = {
 }
 INPUTS_MAX_SCALES = 4                     # WMD_INPUTS_MAX_SCALES
 
+
+class NyuInputsDesc(Structure):
+    """struct wmd_nyu_inputs_desc (include/wmd_inputs_nyu.h)."""
+    _fields_ = [("N", c_int32), ("image_h", c_int32), ("image_w", c_int32), ("depth_h", c_int32), ("depth_w", c_int32),
+                ("image_xk", c_int32), ("image_yk", c_int32), ("depth_xk", c_int32), ("depth_yk", c_int32),
+                ("image_src", c_void_p), ("depth_src", c_void_p), ("items", c_void_p), ("lut", c_void_p),
+                ("image_xtab", c_void_p), ("image_ytab", c_void_p), ("depth_xtab", c_void_p), ("depth_ytab", c_void_p),
+                ("image", c_void_p), ("depth", c_void_p)]
+
+
+# include/wmd_inputs_nyu.h: NYUv2's training inputs, the flip, channel swap, gamma, crop, resize and ToTensor
+# (tests/test_nyu_inputs_oracle.py checks this table against it)
+NYU_INPUTS_SIGNATURES = {
+    "wmd_nyu_inputs_ws_bytes": (c_size_t, [POINTER(NyuInputsDesc)]),
+    "wmd_nyu_inputs_u8": (c_int, [POINTER(NyuInputsDesc), c_void_p, c_size_t, c_void_p]),
+}
+NYU_SRC_H, NYU_SRC_W, NYU_CROP = 480, 640, 16      # WMD_NYU_SRC_H, WMD_NYU_SRC_W, WMD_NYU_CROP
+
 _lib = None
 
 
@@ -256,7 +274,7 @@ def load():
                 continue
         lib = ctypes.CDLL(LIB_PATH)
     tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES,
-              INPUTS_SIGNATURES)
+              INPUTS_SIGNATURES, NYU_INPUTS_SIGNATURES)
     for name, (res, args) in [item for table in tables for item in table.items()]:
         fn = getattr(lib, name)
         fn.restype = res

@@ -5,22 +5,16 @@
 // atomic additions commute, so the bits never depend on the schedule.  The colour ops keep Pillow's float and double
 // sub-expressions apart with explicit round-to-nearest intrinsics, so no contraction can change a value.
 #include "common.cuh"
+#include "resample8.cuh"
 #include "wmd_inputs.h"
 
 namespace wmd {
 namespace {
 
 constexpr int kT = 256;
-constexpr int kPrecisionBits = 22;
 constexpr size_t kAlign = 256;
 
 inline size_t up(size_t b) { return (b + kAlign - 1) / kAlign * kAlign; }
-
-__device__ __forceinline__ int clip8(int v) { return v < 0 ? 0 : (v > 255 ? 255 : v); }
-
-__device__ __forceinline__ int acc8(long long acc) {   // Pillow's clip8 of a 22-bit fixed-point sum
-  return clip8(static_cast<int>(acc >> kPrecisionBits));
-}
 
 // One resample pass's source and tables.  Stage 0 reads per-view sizes, flips and tables from `views`.
 struct Pass {

@@ -28,13 +28,13 @@ import random
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, pillow_tables
 from .ops import _launch
+from .pillow_tables import PRECISION_BITS
 
 KITTI_K = np.array([[0.58, 0, 0.5, 0], [0, 1.92, 0.5, 0], [0, 0, 1, 0], [0, 0, 0, 1]], dtype=np.float32)
 JITTER_RANGES = ((0.8, 1.2), (0.8, 1.2), (0.8, 1.2), (-0.1, 0.1))      # brightness, contrast, saturation, hue
 MIN_DEPTH, MAX_DEPTH = 0.1, 100.0
-PRECISION_BITS = 22
 
 VIEW_DTYPE = np.dtype([("xtab", "<u8"), ("ytab", "<u8"), ("h", "<i4"), ("w", "<i4"), ("xk", "<i4"), ("yk", "<i4"),
                        ("flip", "<i4"), ("pad", "<i4")])                 # struct wmd_inputs_view
@@ -42,40 +42,13 @@ JITTER_DTYPE = np.dtype([("order", "<i4", 4), ("factor", "<f4", 3), ("hue_shift"
 
 
 # ------------------------------------------------------------------------------------------------- host-side tables
-def _lanczos(x):
-    def sinc(t):
-        if t == 0.0:
-            return 1.0
-        t = t * math.pi
-        return math.sin(t) / t
-    return sinc(x) * sinc(x / 3) if -3.0 <= x < 3.0 else 0.0
-
-
 def lanczos_table(in_size, out_size):
     """Pillow's 8-bit LANCZOS coefficients for in_size -> out_size as (out_size, 2 + k) int32 rows of (first tap,
     taps, k coefficients); an unchanged extent is the identity, as Pillow copies the image."""
     if in_size == out_size:
         return np.stack([np.arange(out_size), np.ones(out_size, np.int64),
                          np.full(out_size, 1 << PRECISION_BITS)], 1).astype(np.int32)
-    scale = float(in_size) / out_size
-    filterscale = max(scale, 1.0)
-    support = 3.0 * filterscale
-    k = int(math.ceil(support)) * 2 + 1
-    ss = 1.0 / filterscale
-    tab = np.zeros((out_size, 2 + k), np.int32)
-    for xx in range(out_size):
-        center = (xx + 0.5) * scale
-        xmin = max(int(center - support + 0.5), 0)
-        n = min(int(center + support + 0.5), in_size) - xmin
-        w = [_lanczos((x + xmin - center + 0.5) * ss) for x in range(n)]
-        total = 0.0
-        for v in w:
-            total += v
-        if total != 0.0:
-            w = [v / total for v in w]
-        tab[xx, 0], tab[xx, 1] = xmin, n
-        tab[xx, 2:2 + n] = [int(v * (1 << PRECISION_BITS) + (-0.5 if v < 0 else 0.5)) for v in w]
-    return tab
+    return pillow_tables.table(in_size, out_size, pillow_tables.lanczos, 3.0)
 
 
 def hue_shift(hue_factor):
