@@ -247,6 +247,14 @@ NYU_INPUTS_SIGNATURES = {
 }
 NYU_SRC_H, NYU_SRC_W, NYU_CROP = 480, 640, 16      # WMD_NYU_SRC_H, WMD_NYU_SRC_W, WMD_NYU_CROP
 
+# include/wmd_gt.h: KITTI's ground-truth depths from velodyne scans (tests/test_kitti_gt_oracle.py checks this table
+# against it)
+GT_SIGNATURES = {
+    "wmd_velo_depth_ws_bytes": (c_size_t, [c_int32, c_int32, c_int32, c_longlong]),
+    "wmd_velo_depth_f64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
+                                   c_size_t, c_void_p, c_void_p]),
+}
+
 _lib = None
 
 
@@ -274,7 +282,7 @@ def load():
                 continue
         lib = ctypes.CDLL(LIB_PATH)
     tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES,
-              INPUTS_SIGNATURES, NYU_INPUTS_SIGNATURES)
+              INPUTS_SIGNATURES, NYU_INPUTS_SIGNATURES, GT_SIGNATURES)
     for name, (res, args) in [item for table in tables for item in table.items()]:
         fn = getattr(lib, name)
         fn.restype = res
