@@ -1,18 +1,22 @@
 """Launch-checking harness: every libwmd launch a workload makes, checked against the fp64 contract of its kernel.
 
 `Harness(monkeypatch)` wraps the entry points of ENTRY_POINTS, (owner, attribute) pairs whose owner is a module or a
-class: the public functions of wavelet_monodepth_b200.ops, and the evaluation and loss entry points of nyu_loss, nyu_eval,
-kitti_eval and kitti_loss.  The decoders, train_native and wavelets call `ops.<name>` through the module, calls inside a
-module (conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows, _NyuLossFn -> _loss_fwd / _loss_bwd, _KittiLossFn ->
-_kitti_fwd / _kitti_bwd, NyuDepthEvaluator.add -> _edges_frames) resolve through its globals, and methods through their
-class, so wrapping the owners' attributes catches every call, nested ones included.
+class: the public functions of wavelet_monodepth_b200.ops, the evaluation and loss entry points of nyu_loss, nyu_eval,
+kitti_eval and kitti_loss, and the data pipelines' launches (kitti_hints.stereo_sgbm and _fuse, KittiInputs._run,
+NyuInputs._run, kitti_gt.generate_depth_maps).  The decoders, train_native and wavelets call `ops.<name>` through the
+module, calls inside a module (conv_dgrad -> conv_rows, nchw_to_rows -> amax_rows, _NyuLossFn -> _loss_fwd / _loss_bwd,
+_KittiLossFn -> _kitti_fwd / _kitti_bwd, NyuDepthEvaluator.add -> _edges_frames, DepthHintGenerator -> stereo_sgbm /
+_fuse) resolve through its globals, and methods through their class, so wrapping the owners' attributes catches every
+call, nested ones included.
 
 Each call runs the original function, synchronises (compactions and list gathers run on side streams), recomputes the
 result from the call's actual inputs with the references of the kernel contract tests (conv_ref, head_ref, disp_tail_ref,
 conv_grad_ref, oracle.haar, oracle.nyu_loss, oracle.nyu_eval, oracle.nyu_edges, oracle.kitti_eval, oracle.kitti_loss,
-plain torch restatements of the wmd.h comments: none of them uses ops or libwmd) and compares at that kernel's bar.  It also checks
-the preconditions a launch's contract relies on: source maxima that cover what an fp16-pair launch reads, exact amax
-outputs, index maps inside their sources, strictly increasing pixel lists, and count <= max_rows.  Pack calls record the
+oracle.sgbm, oracle.depth_hints, oracle.kitti_inputs, oracle.nyu_inputs, oracle.kitti_gt, plain torch restatements of
+the wmd.h comments: none of them uses ops or libwmd) and compares at that kernel's bar.  It also checks the
+preconditions a launch's contract relies on: source maxima that cover what an fp16-pair launch reads, exact amax
+outputs, index maps inside their sources, strictly increasing pixel lists, count <= max_rows, views of one size per
+launch, 0 / 1 mirror flags and scan offsets that rise from 0 to the point count.  Pack calls record the
 plain weights behind each packed object; a pack is right when every launch that uses it is right.  State a checker needs
 from before the call (an evaluator's next frame and the rows the call writes) comes from the entry's `_before_` hook.
 
@@ -27,13 +31,19 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from oracle import depth_hints as odh
 from oracle import haar as ohaar
 from oracle import kitti_eval as oke
+from oracle import kitti_gt as okg
+from oracle import kitti_inputs as oki
 from oracle import kitti_loss as okl
 from oracle import nyu_edges as ne
 from oracle import nyu_eval as one
+from oracle import nyu_inputs as oni
 from oracle import nyu_loss as onl
-from wavelet_monodepth_b200 import _lib, kitti_eval, kitti_loss, nyu_eval, nyu_loss, ops
+from oracle import sgbm as osgbm
+from wavelet_monodepth_b200 import (_lib, kitti_eval, kitti_gt, kitti_hints, kitti_inputs, kitti_loss, nyu_eval, nyu_inputs,
+                                    nyu_loss, ops)
 
 import conv_grad_ref
 import conv_ref as cr
@@ -57,7 +67,10 @@ EVAL_LOSS = ((nyu_loss, "_loss_fwd"), (nyu_loss, "_loss_bwd"),
              (kitti_eval, "compute_errors"), (kitti_eval, "batch_post_process_disparity"),
              (kitti_eval.KittiDepthEvaluator, "__init__"), (kitti_eval.KittiDepthEvaluator, "add"),
              (kitti_loss, "_kitti_fwd"), (kitti_loss, "_kitti_bwd"))
-ENTRY_POINTS = tuple((ops, name) for name in CHECKED) + EVAL_LOSS
+# the depth-hint, training-input and ground-truth pipelines' entry points that launch kernels, (owner, attribute)
+PIPELINES = ((kitti_hints, "stereo_sgbm"), (kitti_hints, "_fuse"), (kitti_inputs.KittiInputs, "_run"),
+             (nyu_inputs.NyuInputs, "_run"), (kitti_gt, "generate_depth_maps"))
+ENTRY_POINTS = tuple((ops, name) for name in CHECKED) + EVAL_LOSS + PIPELINES
 
 
 def entry_name(owner, attr):
@@ -74,9 +87,8 @@ def hook(prefix, entry):
     return prefix + entry.replace(".__init__", ".init").strip("_").replace(".", "_")
 
 
-# every symbol of _lib.SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES and KITTI_LOSS_SIGNATURES: ("launch", entry point
-# whose checker covers it) |
-# ("pack", ops entry point) | "query"
+# every symbol of the tables of _lib.TABLES: ("launch", entry point whose checker covers it) | ("pack", ops entry point) |
+# "query"
 SYMBOLS = {
     "wmd_version": "query", "wmd_status_string": "query", "wmd_last_cuda_error": "query", "wmd_launch_count": "query",
     "wmd_idwt_haar_f32": ("launch", "idwt_haar"),
@@ -150,6 +162,20 @@ SYMBOLS = {
     "wmd_loss_kitti_bwd_ws_bytes": "query",
     "wmd_loss_kitti_fwd": ("launch", "_kitti_fwd"),
     "wmd_loss_kitti_bwd": ("launch", "_kitti_bwd"),
+    # include/wmd_hints.h
+    "wmd_sgbm_ws_bytes": "query",
+    "wmd_sgbm_u8": ("launch", "stereo_sgbm"),
+    "wmd_depth_hints_ws_bytes": "query",
+    "wmd_depth_hints_f32": ("launch", "_fuse"),
+    # include/wmd_inputs.h
+    "wmd_inputs_ws_bytes": "query",
+    "wmd_inputs_u8": ("launch", "KittiInputs._run"),
+    # include/wmd_inputs_nyu.h
+    "wmd_nyu_inputs_ws_bytes": "query",
+    "wmd_nyu_inputs_u8": ("launch", "NyuInputs._run"),
+    # include/wmd_gt.h
+    "wmd_velo_depth_ws_bytes": "query",
+    "wmd_velo_depth_f64": ("launch", "generate_depth_maps"),
 }
 
 # bars of the checks this file adds on top of the contract tests' (units of 2^-24 of the element's scale)
@@ -987,6 +1013,131 @@ class Harness:
         err = _rel_err(_np(out), want, "compute_errors")
         _record("compute_errors", "fp64", "-", err, EVAL_REL, a["gt"].numel())
         _require(err <= EVAL_REL, "%s: compute_errors err %.3g > %.3g" % (self.current, err, EVAL_REL))
+
+    # ------------------------------------------------------------------------------------------ KITTI depth hints
+    def _check_stereo_sgbm(self, a, out, pre):
+        """each frame equals oracle.sgbm.compute_side on the call's views and mirror flag, int16 bits, the borders the
+        matcher never writes included"""
+        left, right = _np(a["left"]), _np(a["right"])
+        n, h, w, _ = left.shape
+        _require(right.shape == left.shape, "stereo_sgbm: views of %s and %s" % (left.shape, right.shape))
+        rev = np.zeros(n, bool)
+        if a["reverse"] is not None:
+            r = np.asarray(_np(a["reverse"]) if torch.is_tensor(a["reverse"]) else a["reverse"]).reshape(-1)
+            _require(r.size == n and np.isin(r, (0, 1)).all(), "stereo_sgbm: reverse flags %s, want %d of 0 / 1"
+                     % (r.tolist(), n))
+            rev = r.astype(bool)
+        nd, bs = a["num_disparities"], a["block_size"]
+        got = _np(out)
+        _require(got.dtype == np.int16 and got.shape == (n, h, w), "stereo_sgbm: map %s %s" % (got.dtype, got.shape))
+        for i in range(n):
+            want = osgbm.compute_side(left[i], right[i], nd, bs, bool(rev[i]))
+            bad = int((got[i] != want).sum())
+            _require(bad == 0, "%s: stereo_sgbm (%d, %d) frame %d (%dx%d%s): %d disparities differ from oracle.sgbm"
+                     % (self.current, nd, bs, i, h, w, ", mirrored" if rev[i] else "", bad))
+        _record("stereo_sgbm", "int16", "nd%d/bs%d" % (nd, bs), 0.0, 0, n * h * w)
+
+    def _check_fuse(self, a, res, pre):
+        """oracle.depth_hints.fuse (contract mode) on the launch's own views and maps: depth bits and index equal; the
+        cameras are the generator's for each view's side"""
+        base, lookup, maps = _np(a["base"]), _np(a["lookup"]), _np(a["maps"])
+        n, h, w, _ = base.shape
+        _require(lookup.shape == base.shape and maps.shape == (len(osgbm.MATCHERS), n, h, w),
+                 "_fuse: views %s, %s and maps %s" % (base.shape, lookup.shape, maps.shape))
+        right = _np(a["T"])[:, 0, 3] > 0
+        for name, want in zip(("K", "inv_K", "T"), odh.cameras(h, w, right)):
+            _require(np.array_equal(_np(a[name]).view(np.uint32), want.view(np.uint32)),
+                     "_fuse: %s is not the generator's camera" % name)
+        depth, index, _ = odh.fuse(base, lookup, maps, right, mode="contract")
+        got = _np(a["depth"])
+        bad = int((got.view(np.uint32) != depth.view(np.uint32)).sum())
+        _require(bad == 0, "%s: _fuse (%d views of %dx%d): %d depths differ from oracle.depth_hints" % (self.current, n, h,
+                                                                                                        w, bad))
+        if a["index"] is not None:
+            bad = int((_np(a["index"]) != index).sum())
+            _require(bad == 0, "%s: _fuse: %d matcher indices differ from oracle.depth_hints" % (self.current, bad))
+        _record("_fuse", "fp32", "contract" + ("+index" if a["index"] is not None else ""), 0.0, 0, n * h * w)
+
+    # ------------------------------------------------------------------------------------------ training inputs
+    def _check_KittiInputs__run(self, a, out, pre):
+        """oracle.kitti_inputs.expected of each item of the call's host batch and draws: every key bit for bit (pyramid,
+        flip, jitter order and factors, cameras, stereo_T, hints); disp_hint zero for an item without a hint"""
+        fn, batch = a["self"], a["batch"]
+        frames = fn.frame_idxs
+        src, sizes = _np(batch["src"]), _np(batch["sizes"])
+        n = len(batch["side"])
+        _require(src.shape[0] == n * len(frames), "KittiInputs._run: %d views for %d items" % (src.shape[0], n))
+        flip, aug = _np(batch["do_flip"]).astype(bool), _np(batch["do_color_aug"]).astype(bool)
+        factors, order = _np(batch["factors"]), _np(batch["order"])
+        hints = fn.use_depth_hints and "s" in frames
+        _require(out["image_path"] == list(batch["image_path"]), "KittiInputs._run: image_path")
+        for k in range(n):
+            _require(aug[k] == (order[k, 0] >= 0), "KittiInputs._run: item %d do_color_aug %s with jitter order %s"
+                     % (k, aug[k], order[k].tolist()))
+            views = {}
+            for fi, f in enumerate(frames):
+                h, w = sizes[fi * n + k]
+                views[f] = src[fi * n + k, :h, :w]
+            params = (tuple(map(float, factors[k])), tuple(map(int, order[k]))) if aug[k] else None
+            hint = None
+            if hints and batch["hint_found"][k]:
+                hh, hw = _np(batch["hint_size"])[k]
+                hint = _np(batch["hint"])[k, :hh, :hw]
+            want = oki.expected(views, (aug[k], flip[k], params), batch["side"][k], hint, fn.height, fn.width,
+                                fn.scales, fn.use_depth_hints)
+            extra = set(out) - set(want) - {"image_path"}
+            _require(extra <= {"disp_hint"}, "KittiInputs._run: item %d has keys %s the reference does not" % (k, extra))
+            for key in extra:
+                _require(not _np(out[key][k]).any(), "KittiInputs._run: item %d's %s is not zero" % (k, key))
+            for key, wv in want.items():
+                _require(key in out, "KittiInputs._run: no %s" % (key,))
+                g = _np(out[key][k])
+                _require(g.dtype == wv.dtype and g.shape == wv.shape and g.tobytes() == wv.tobytes(),
+                         "%s: KittiInputs._run item %d (%dx%d views, flip %d, jitter %s): %s differs from "
+                         "oracle.kitti_inputs" % (self.current, k, *sizes[k], flip[k], params, key))
+        mode = "%dx%d" % (fn.width, fn.height) + ("+hints" if hints else "")
+        _record("KittiInputs._run", "u8/fp32", mode, 0.0, 0, len(src) * fn.height * fn.width)
+
+    def _check_NyuInputs__run(self, a, out, pre):
+        """oracle.nyu_inputs.expected of each item of the call's host batch and draws: image and depth bit for bit"""
+        fn, batch = a["self"], a["batch"]
+        image, depth, perm = _np(batch["image"]), _np(batch["depth"]), _np(batch["perm"])
+        flip, gamma = _np(batch["flip"]).astype(bool), _np(batch["gamma"])
+        for k in range(image.shape[0]):
+            p = tuple(int(v) for v in perm[k])
+            _require(p in oni.PERMS, "NyuInputs._run: item %d's channel order %s is not a permutation" % (k, p))
+            want = oni.expected(image[k], depth[k], flip[k], oni.PERMS.index(p),
+                                None if np.isnan(gamma[k]) else float(gamma[k]), fn.is_224, fn.resample)
+            for key, wv in want.items():
+                g = _np(out[key][k])
+                _require(g.dtype == wv.dtype and g.shape == wv.shape and g.tobytes() == wv.tobytes(),
+                         "%s: NyuInputs._run item %d (flip %d, perm %s, gamma %s): %s differs from oracle.nyu_inputs"
+                         % (self.current, k, flip[k], p, gamma[k], key))
+        mode = ("224" if fn.is_224 else "640") + "/" + fn.resample
+        _record("NyuInputs._run", "u8/fp32", mode, 0.0, 0, out["image"].numel())
+
+    # ------------------------------------------------------------------------------------------ KITTI ground truth
+    def _check_generate_depth_maps(self, a, depth, pre):
+        """oracle.kitti_gt.depth_map of each scan: the fp64 bits of its (H, W) map, and +0.0 everywhere past (H, W)"""
+        pts = a["points"]
+        pts = _np(pts) if torch.is_tensor(pts) else np.asarray(pts, np.float32)
+        off = np.asarray(_np(a["offsets"]) if torch.is_tensor(a["offsets"]) else a["offsets"], np.int64).reshape(-1)
+        P = np.asarray(_np(a["P"]) if torch.is_tensor(a["P"]) else a["P"], np.float64).reshape(-1, 3, 4)
+        sizes = np.asarray(_np(a["sizes"]) if torch.is_tensor(a["sizes"]) else a["sizes"], np.int64).reshape(-1, 2)
+        n = sizes.shape[0]
+        _require(off.size == n + 1 and off[0] == 0 and off[-1] == pts.shape[0] and (np.diff(off) >= 0).all(),
+                 "generate_depth_maps: offsets %s for %d scans of %d points" % (off.tolist(), n, pts.shape[0]))
+        got = _np(depth)
+        for i, (h, w) in enumerate(sizes):
+            want = okg.depth_map(pts[off[i]:off[i + 1]], P[i], int(h), int(w), bool(a["vel_depth"]))
+            bad = int((got[i, :h, :w].view(np.int64) != want.view(np.int64)).sum())
+            _require(bad == 0, "%s: generate_depth_maps frame %d (%dx%d, %d points): %d depths differ from "
+                     "oracle.kitti_gt" % (self.current, i, h, w, off[i + 1] - off[i], bad))
+            pad = got[i].copy()
+            pad[:h, :w] = 0
+            _require(not pad.view(np.int64).any(), "%s: generate_depth_maps frame %d: written past its %dx%d"
+                     % (self.current, i, h, w))
+        _record("generate_depth_maps", "fp64", "vel_depth" if a["vel_depth"] else "camera", 0.0, 0, int(off[-1]))
 
 
 def epilogue_ref(epi, out, disp):

@@ -9,25 +9,38 @@ the KITTI R50 1024x320 wave decoder, and of KITTI's wave (R50 1024x320) and base
 with KittiDepthHintsLoss (its warps, CTA partials and gathers at production sizes); the KITTI dense decoder without
 skips; the sparse NYU decoder at its threshold extremes; NYU evaluation with depth boundary errors on 440x592 frames (fixed CTA grids, union-find hysteresis, the
 exact distance transform) and in 224 mode; KITTI evaluation of post-processed disparities, whose medians are taken by
-radix select over full LiDAR frames.  Inputs are synthetic (synth, oracle.nyu_edges.edge_split,
-oracle.kitti_eval.synthetic_split).  The entry points are called through their modules, as the package's users do: a
-name imported from a module would bypass the harness's wrapper, and the completeness check would name its symbol.
+radix select over full LiDAR frames.  The data pipelines run where their outputs are used: depth hints of one 1024x320
+pair with both views in one batch (all twelve matchers and the fusion); KittiInputs on twelve items of KITTI's five raw
+sizes, flipped, jittered and with hints, driving an R18 wave decoder step with KittiDepthHintsLoss; NyuInputs' depths as
+the NyuDepthLoss target of a DecoderWave step; the ground truth of eight full velodyne scans, over the calibration
+dates' image sizes, both cameras and both depth conventions, scored by KittiDepthEvaluator.  Inputs are synthetic
+(synth, oracle.nyu_edges.edge_split, oracle.kitti_eval.synthetic_split, oracle.depth_hints.make_pair,
+oracle.kitti_inputs.synthetic_view, oracle.nyu_inputs.synthetic_image, oracle.kitti_gt.synthetic_scan).  The entry
+points are called through their modules, as the package's users do: a name imported from a module would bypass the
+harness's wrapper, and the completeness check would name its symbol.
 
 Each workload runs once plainly and once under the harness, which checks each launch at its kernel's bar and that every
 kernel launched ran inside a checked call; the two runs must agree bit for bit.  Each prints its per-entry-point call
 counts and wall times; the module prints the worst error of every (entry point, engine, mode) at the end.
 """
 import gc
+import os
+import random
 import time
 
 import numpy as np
 import pytest
 import torch
 
+from oracle import depth_hints as odh
 from oracle import kitti_eval as oke
+from oracle import kitti_gt as okg
+from oracle import kitti_inputs as oki
 from oracle import kitti_loss as okl
 from oracle import nyu_edges as ne
-from wavelet_monodepth_b200 import kitti_decoders as kd, kitti_eval, nyu_decoders as nd, nyu_eval, synth
+from oracle import nyu_inputs as oni
+from wavelet_monodepth_b200 import (kitti_decoders as kd, kitti_eval, kitti_gt, kitti_hints, kitti_inputs,
+                                    nyu_decoders as nd, nyu_eval, nyu_inputs, synth)
 from wavelet_monodepth_b200.kitti_loss import KittiDepthHintsLoss
 from wavelet_monodepth_b200.nyu_loss import NyuDepthLoss
 
@@ -39,6 +52,7 @@ MNV2_LIGHT_CH = (32, 24, 32, 64, 160)
 D161_224 = (synth.DENSENET161_CH, 224, 224)
 MNV2_224 = (MNV2_LIGHT_CH, 224, 224)
 EVAL_FRAMES = 16
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -92,10 +106,11 @@ def kitti_no_skips(n, spec):
 
 
 # ------------------------------------------------------------------------------------------ training
-def train(make, n, spec, shapes, loss=None):
+def train(make, n, spec, shapes, loss=None, inputs=None):
     """One native training step with fp32 convolutions: outputs, parameter and input-feature gradients.  With `loss`
-    (a NyuDepthLoss) the objective is that loss against a target within 30 % of the decoder's own ("disp", 0) (so the
-    signs of the differences vary); otherwise the sum of the ("disp", s) means."""
+    (a NyuDepthLoss) the objective is that loss against the "depth" of inputs(n) (a NyuInputs batch), or without
+    `inputs` against a target within 30 % of the decoder's own ("disp", 0) (so the signs of the differences vary);
+    otherwise the sum of the ("disp", s) means."""
     def run():
         ch, h, w = spec
         mod = make(ch)
@@ -107,9 +122,14 @@ def train(make, n, spec, shapes, loss=None):
         if loss is None:
             total = sum(v.mean() for k, v in out.items() if k[0] == "disp")
         else:
-            d0 = out[("disp", 0)].detach()
-            gen = torch.Generator(device="cpu").manual_seed(5)
-            target = (d0.abs() + 0.05) * (0.7 + 0.6 * torch.rand(d0.shape, generator=gen)).to(DEV)
+            if inputs is None:
+                d0 = out[("disp", 0)].detach()
+                gen = torch.Generator(device="cpu").manual_seed(5)
+                target = (d0.abs() + 0.05) * (0.7 + 0.6 * torch.rand(d0.shape, generator=gen)).to(DEV)
+            else:
+                batch = inputs(n)
+                res.update({("input", k): v for k, v in batch.items()})
+                target = batch["depth"]
             total, losses = loss(out, target)
             res.update({("loss", k): v.detach() for k, v in losses.items()})
         total.backward()
@@ -119,27 +139,56 @@ def train(make, n, spec, shapes, loss=None):
     return run
 
 
-def train_kitti_loss(make, n, spec):
-    """One native training step of a KITTI decoder with KittiDepthHintsLoss on oracle.kitti_loss's synthetic stereo
-    frames (images, KITTI's intrinsics, hints); the tie-breaking noise from a seeded CPU generator, so both runs draw the
-    same.  Outputs, terms, masks, warps, parameter and input-feature gradients."""
+def kitti_loss_inputs(n, h, w):
+    """oracle.kitti_loss's synthetic stereo frames (images, KITTI's intrinsics, hints) as a loss's inputs dict"""
+    inp, _ = okl.make_inputs(dict(N=n, H=h, W=w, scales=okl.SCALES), 5)
+    inputs = {("color", 0, 0): inp["target"], ("color", "s", 0): inp["source"], ("K", 0): inp["K"],
+              ("inv_K", 0): inp["inv_K"], "stereo_T": inp["stereo_T"], "depth_hint": inp["depth_hint"],
+              "depth_hint_mask": inp["depth_hint_mask"]}
+    inputs.update({("color", 0, s): inp["colors"][s] for s in okl.SCALES if s})
+    return {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in inputs.items()}
+
+
+def kitti_inputs_batch(n, h, w):
+    """KittiInputs on n items (frames 0 and "s") over KITTI's five raw image sizes: left and right sides, flipped and
+    not, two in three jittered, depth hints at two raw sizes and one missing"""
+    items = []
+    for i in range(n):
+        view = oki.synthetic_view(60 + i, *oki.RAW_SIZES[i % len(oki.RAW_SIZES)])
+        side = "lr"[(i // 2) % 2]
+        hint = None if i == 5 else oki.synthetic_hint(90 + i, *((320, 1024) if i % 3 else (188, 621)))
+        items.append({"views": {0: view, "s": np.ascontiguousarray(np.roll(view, 12 if side == "l" else -12, 1))},
+                      "do_color_aug": i % 3 != 0, "do_flip": i % 2 == 1,
+                      "jitter": oki.get_params(random.Random(i)) if i % 3 != 0 else None, "side": side,
+                      "image_path": "frame_%d" % i, "hint": hint})
+    return kitti_inputs.KittiInputs(h, w, [0, "s"], use_depth_hints=True)(kitti_inputs.collate(items))
+
+
+def nyu_inputs_batch(n):
+    """NyuInputs (640x480 image, 320x240 depth, bicubic) on n items: flipped and not, every channel order, gammas 0.8,
+    1.0 and 1.25, and items without a swap or gamma"""
+    items = [{"image": oni.synthetic_image(20 + i), "depth": oni.synthetic_depth(20 + i), "flip": i % 2 == 1,
+              "perm": i % 7 - 1, "gamma": None if i % 7 == 0 else (0.8, 1.0, 1.25)[i % 3]} for i in range(n)]
+    return nyu_inputs.NyuInputs(False, "bicubic")(nyu_inputs.collate(items))
+
+
+def train_kitti_loss(make, n, spec, inputs=kitti_loss_inputs):
+    """One native training step of a KITTI decoder with KittiDepthHintsLoss on inputs(n, h, w), by default
+    oracle.kitti_loss's synthetic stereo frames; the tie-breaking noise from a seeded CPU generator, so both runs draw
+    the same.  Inputs, outputs, terms, masks, warps, parameter and input-feature gradients."""
     def run():
         ch, h, w = spec
         mod = make(ch)
         synth.load_random(mod, seed=1)
         mod = mod.to(DEV).train()
         feats = _feats(synth.kitti_feature_shapes(n, h, w, ch), seed=2, grad=True)
-        inp, _ = okl.make_inputs(dict(N=n, H=h, W=w, scales=okl.SCALES), 5)
-        inputs = {("color", 0, 0): inp["target"], ("color", "s", 0): inp["source"], ("K", 0): inp["K"],
-                  ("inv_K", 0): inp["inv_K"], "stereo_T": inp["stereo_T"], "depth_hint": inp["depth_hint"],
-                  "depth_hint_mask": inp["depth_hint_mask"]}
-        inputs.update({("color", 0, s): inp["colors"][s] for s in okl.SCALES if s})
-        inputs = {k: torch.from_numpy(np.ascontiguousarray(v)).to(DEV) for k, v in inputs.items()}
+        inputs_ = inputs(n, h, w)
         out = mod(feats)
         torch.manual_seed(5)
-        total, losses = KittiDepthHintsLoss(h, w)(inputs, out)
+        total, losses = KittiDepthHintsLoss(h, w)(inputs_, out)
         res = {("out",) + tuple(k if isinstance(k, tuple) else (k,)): v.detach() for k, v in out.items()
                if torch.is_tensor(v)}
+        res.update({("input", k): v for k, v in inputs_.items()})
         res.update({("loss", k): v.detach() for k, v in losses.items()})
         total.backward()
         res.update({("grad", k): p.grad for k, p in mod.named_parameters() if p.grad is not None})
@@ -216,6 +265,45 @@ def kitti_eval_pp(n, spec):
     return run
 
 
+# ------------------------------------------------------------------------------------------ data pipelines
+def hints_pair(seed, h, w):
+    """DepthHintGenerator on one synthetic pair, its left and right views in one batch (the right one mirrored around
+    the matchers): all twelve matchers and the fusion"""
+    def run():
+        left, right = odh.make_pair(seed, h, w)
+        base = torch.from_numpy(np.stack([left, right])).to(DEV)
+        lookup = torch.from_numpy(np.stack([right, left])).to(DEV)
+        depth, index = kitti_hints.DepthHintGenerator(h, w)(base, lookup, [False, True], return_index=True)
+        return {"depth": depth, "index": index}
+    return run
+
+
+def gt_export_then_eval(n):
+    """generate_depth_maps on n full synthetic scans, one call per depth convention (vel_depth off, on), the frames
+    mixing the calibration dates' image sizes and both cameras; the maps then score seeded 640x192 disparities in
+    KittiDepthEvaluator"""
+    def run():
+        with np.load(os.path.join(GOLDEN, "kitti_gt_calib.npz")) as f:
+            calib = {k: f[k] for k in f.files}
+        dates = sorted(okg.DATES)
+        res, gts = {}, []
+        for vd in (False, True):
+            frames = [(dates[(2 * i + vd) % len(dates)], 2 + (i + vd) % 2) for i in range(n // 2)]
+            scans = [okg.synthetic_scan(300 + 10 * vd + i) for i in range(n // 2)]
+            offsets = np.concatenate([[0], np.cumsum([s.shape[0] for s in scans])])
+            P = np.stack([calib["%s/P%d" % fr] for fr in frames])
+            sizes = np.array([calib["%s/size" % d] for d, _ in frames], np.int32)
+            depth = kitti_gt.generate_depth_maps(torch.from_numpy(np.concatenate(scans)).to(DEV), offsets, P, sizes, vd)
+            res["depth", vd] = depth
+            gts += [depth[k, :h, :w] for k, (h, w) in enumerate(sizes.tolist())]
+        ev = kitti_eval.KittiDepthEvaluator(gts)
+        gen = torch.Generator(device="cpu").manual_seed(9)
+        ev.add((0.01 + 0.3 * torch.rand((n, 1, 192, 640), generator=gen)).to(DEV))
+        res.update(errors=ev.errors, ratios=ev.ratios, counts=ev.counts)
+        return res
+    return run
+
+
 WORKLOADS = {
     "wave224_d161_x8": nyu224(nd.DecoderWave224, 8, D161_224),
     "wave224_mnv2light_x8": nyu224(nd.DecoderWave224, 8, MNV2_224),
@@ -237,6 +325,12 @@ WORKLOADS = {
     "eval_nyu_sparse_d161_x%d_edges" % EVAL_FRAMES: nyu_eval_edges(EVAL_FRAMES, D161),
     "eval_nyu_wave224_mnv2light_x8": nyu_eval_224(8, MNV2_224),
     "eval_kitti_sparse_r18_x%d_postprocess" % EVAL_FRAMES: kitti_eval_pp(EVAL_FRAMES, R18),
+    "hints_320x1024_pair_both_sides": hints_pair(odh.FULL["full0"][0], 320, 1024),
+    "train_wave_r18_640x192_x12_from_kitti_inputs": train_kitti_loss(
+        lambda ch: kd.DepthWaveProgressiveDecoder(np.array(ch)), 12, R18, kitti_inputs_batch),
+    "train_nyu_wave_d161_640x480_x8_from_nyu_inputs": train(_nyu(nd.DecoderWave), 8, D161, synth.nyu_feature_shapes,
+                                                            NyuDepthLoss(), nyu_inputs_batch),
+    "gt_export_full_scans_then_eval": gt_export_then_eval(8),
 }
 
 

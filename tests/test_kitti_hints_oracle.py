@@ -22,7 +22,7 @@ HINT_SYMBOLS = {
     "wmd_sgbm_ws_bytes": "query",
     "wmd_sgbm_u8": ("launch", "stereo_sgbm"),
     "wmd_depth_hints_ws_bytes": "query",
-    "wmd_depth_hints_f32": ("launch", "DepthHintGenerator._run"),
+    "wmd_depth_hints_f32": ("launch", "_fuse"),
 }
 
 

@@ -2,19 +2,23 @@
 has a checker, a pack, or a size / query function.  A new entry point cannot ship without one."""
 import inspect
 
-from wavelet_monodepth_b200 import _lib, kitti_eval, kitti_loss, nyu_eval, nyu_loss, ops
+from wavelet_monodepth_b200 import (_lib, kitti_eval, kitti_gt, kitti_hints, kitti_inputs, kitti_loss, nyu_eval, nyu_inputs,
+                                    nyu_loss, ops)
 
 import launch_check as lc
 
-TABLES = (_lib.SIGNATURES, _lib.EVAL_SIGNATURES, _lib.LOSS_SIGNATURES, _lib.KITTI_LOSS_SIGNATURES)
+TABLES = _lib.TABLES                    # every table _lib.load() binds
 ALL_SIGNATURES = {k: v for table in TABLES for k, v in table.items()}
 
 
 def test_every_symbol_is_classified():
-    """SYMBOLS covers wmd.h, wmd_eval.h, wmd_loss.h and wmd_loss_kitti.h (their bindings, which test_abi / the oracle
-    tests hold to the headers), and nothing else."""
+    """SYMBOLS covers every table _lib.load() binds (wmd.h, wmd_eval.h, wmd_loss.h, wmd_loss_kitti.h, wmd_hints.h,
+    wmd_inputs.h, wmd_inputs_nyu.h and wmd_gt.h, which test_abi / the oracle tests hold to the headers), and nothing
+    else."""
     assert len(ALL_SIGNATURES) == sum(len(table) for table in TABLES)
-    assert _lib.KITTI_LOSS_SIGNATURES and set(_lib.KITTI_LOSS_SIGNATURES) <= set(ALL_SIGNATURES)
+    for table in (_lib.KITTI_LOSS_SIGNATURES, _lib.HINTS_SIGNATURES, _lib.INPUTS_SIGNATURES, _lib.NYU_INPUTS_SIGNATURES,
+                  _lib.GT_SIGNATURES):
+        assert table and any(t is table for t in TABLES)
     unclassified = sorted(set(ALL_SIGNATURES) - set(lc.SYMBOLS))
     assert not unclassified, "libwmd symbols without a launch checker / pack / query classification: %s" % unclassified
     assert not sorted(set(lc.SYMBOLS) - set(ALL_SIGNATURES))
@@ -48,18 +52,18 @@ def _functions(module):
 
 
 def test_every_ops_function_that_calls_libwmd_is_wrapped():
-    """A function or method of ops, nyu_loss, nyu_eval, kitti_eval or kitti_loss that reaches a launch or pack symbol
-    directly is a checked entry point or a pack."""
+    """A function or method of ops, nyu_loss, nyu_eval, kitti_eval, kitti_loss, kitti_hints, kitti_inputs, nyu_inputs or
+    kitti_gt that reaches a launch or pack symbol directly is a checked entry point or a pack."""
     wrapped = set(lc.ENTRIES) | set(lc.PACKS)
     found = set()
-    for module in (ops, nyu_loss, nyu_eval, kitti_eval, kitti_loss):
+    for module in (ops, nyu_loss, nyu_eval, kitti_eval, kitti_loss, kitti_hints, kitti_inputs, nyu_inputs, kitti_gt):
         for name, fn in _functions(module):
             src = inspect.getsource(fn)
             used = [s for s, k in lc.SYMBOLS.items() if k != "query" and ".%s(" % s in src]
             if used:
                 assert name in wrapped, (module.__name__, name, used)
                 found.add(name)
-    # every wrapped entry point of the evaluation and loss modules calls libwmd itself
-    assert {lc.entry_name(o, a) for o, a in lc.EVAL_LOSS} <= found
+    # every wrapped entry point of the evaluation, loss and pipeline modules calls libwmd itself
+    assert {lc.entry_name(o, a) for o, a in lc.EVAL_LOSS + lc.PIPELINES} <= found
     for entry in set(lc.CHECKED) | set(lc.PACKS):
         assert callable(getattr(ops, entry)), entry

@@ -1,21 +1,33 @@
-"""The launch checkers of the evaluation and loss entry points (tests/launch_check.py) have teeth: each passes the oracle's
-own answer and raises LaunchError when one element of it is changed by the smallest step its bar must see (a loss
-gradient one ulp off, one edge pixel toggled, one a_k count off by one, one KITTI median ratio one ulp off, one KITTI
-loss mask pixel toggled).  CPU only:
-the checkers are called directly on CPU tensors, with stand-ins for the evaluators' state; no GPU and no libwmd."""
+"""The launch checkers of the evaluation, loss and data-pipeline entry points (tests/launch_check.py) have teeth: each
+passes the oracle's own answer and raises LaunchError when one element of it is changed by the smallest step its bar
+must see (a loss gradient one ulp off, one edge pixel toggled, one a_k count off by one, one KITTI median ratio one ulp
+off, one KITTI loss mask pixel toggled, one SGBM disparity 1/16 px off, one fused depth one ulp off or its matcher index
+changed, one input colour element one ulp off, one hint pixel toggled, one ground-truth depth one ulp off or one empty
+ground-truth pixel given a depth).  CPU only: the checkers are called directly on CPU tensors, with stand-ins for the
+evaluators' state; no GPU and no libwmd."""
+import os
 import types
 
 import numpy as np
 import pytest
 import torch
 
+from oracle import depth_hints as odh
 from oracle import kitti_eval as oke
+from oracle import kitti_gt as okg
+from oracle import kitti_inputs as oki
 from oracle import kitti_loss as okl
 from oracle import nyu_edges as ne
 from oracle import nyu_eval as one
+from oracle import nyu_inputs as oni
 from oracle import nyu_loss as onl
+from oracle import sgbm as osgbm
+from wavelet_monodepth_b200 import kitti_inputs as ki
+from wavelet_monodepth_b200 import nyu_inputs as ni
 
+import kitti_inputs_cases as kic
 import launch_check as lc
+import nyu_inputs_cases as nic
 
 
 @pytest.fixture
@@ -308,3 +320,125 @@ def test_kitti_bwd_checker(harness):
     toggled = idsel.clone()
     toggled[0, 0, 0, 3, 4] = 1 - toggled[0, 0, 0, 3, 4]                   # one mask pixel toggled
     both(call, (grads,), (grads, toggled))
+
+
+# ------------------------------------------------------------------------------------------ KITTI depth hints
+def _hint_pair():
+    """the 64x256 pair of tests/golden/kitti_depth_hints_a.npz as one mixed batch: its left view and its mirrored right
+    view, with the twelve matchers' maps OpenCV made of each"""
+    with np.load(os.path.join(kic.GOLDEN, "kitti_depth_hints_a.npz")) as f:
+        left, right = f["a/left"], f["a/right"]
+        maps = np.stack([f["a/l/maps"], f["a/r/maps"]], 1)
+    base, lookup = np.stack([left, right]), np.stack([right, left])
+    return base, lookup, maps, [False, True]
+
+
+def test_stereo_sgbm_checker(harness):
+    base, lookup, _, right = _hint_pair()
+    want = np.stack([osgbm.compute_side(base[i], lookup[i], 96, 2, right[i]) for i in range(2)])
+    assert (want != -16).mean() > 0.3
+
+    def call(out):
+        a = dict(left=t(base), right=t(lookup), num_disparities=96, block_size=2, reverse=right, out=None)
+        harness._check_stereo_sgbm(a, t(out), None)
+    moved = want.copy()
+    moved[1, 30, 200] += 1                                                # one disparity 1/16 px off
+    both(call, (want,), (moved,))
+    border = want.copy()
+    border[0, 0, 0] = 0                                                   # one unwritten border pixel written
+    assert want[0, 0, 0] == -16
+    both(call, (want,), (border,))
+
+
+def test_fuse_checker(harness):
+    base, lookup, maps, right = _hint_pair()
+    K, inv_K, T = odh.cameras(64, 256, right)
+    depth, index, _ = odh.fuse(base, lookup, maps, right, mode="contract")
+    index = index.astype(np.int32)
+    assert depth[0, 0, 20, 100] > 0 and len(np.unique(index)) > 2
+
+    def call(depth, index):
+        a = dict(base=t(base), lookup=t(lookup), maps=t(maps), K=t(K), inv_K=t(inv_K), T=t(T), depth=t(depth),
+                 index=t(index))
+        harness._check_fuse(a, None, None)
+    both(call, (depth, index), (ulp_up(depth, (0, 0, 20, 100)), index))  # one fused depth one ulp off
+    changed = index.copy()
+    changed[1, 0, 40, 60] = (changed[1, 0, 40, 60] + 1) % 12              # one matcher index changed
+    both(call, (depth, index), (depth, changed))
+
+
+# ------------------------------------------------------------------------------------------ training inputs
+def test_kitti_inputs_checker(harness):
+    """two items of the train640 fixture (both frames, flips, jitter, hints) at 640x192"""
+    fx = kic.load("train640")
+    cfg = fx["config"]
+    items = kic.items(fx)[:2]
+    fn = ki.KittiInputs(cfg["height"], cfg["width"], cfg["frame_idxs"], cfg["scales"], cfg["use_depth_hints"])
+    batch = ki.collate(items)
+    exp = [oki.expected(it["views"], (it["do_color_aug"], it["do_flip"], it["jitter"]), it["side"], it.get("hint"),
+                        fn.height, fn.width, fn.scales, fn.use_depth_hints) for it in items]
+    keys = set(exp[0]) | set(exp[1])
+    assert ("disp_hint" in exp[0]) != ("disp_hint" in exp[1])                    # an item without a hint: zeros
+    out = {k: t(np.stack([e.get(k, np.zeros_like(exp[0].get(k, exp[1].get(k)))) for e in exp])) for k in keys}
+    out["image_path"] = list(batch["image_path"])
+    assert cfg["use_depth_hints"] and "s" in fn.frame_idxs and out["depth_hint_mask"].any()
+
+    def call(out):
+        harness._check_KittiInputs__run(dict(self=fn, batch=batch, device=None), out, None)
+    key = ("color_aug", "s", 1)
+    moved = dict(out)
+    moved[key] = t(ulp_up(out[key].numpy(), (1, 2, 30, 40)))                     # one colour element one ulp off
+    both(call, (out,), (moved,))
+    h = 0 if "disp_hint" in exp[0] else 1
+    mask = out["depth_hint_mask"].clone()
+    mask[h, 0, 50, 60] = 1 - mask[h, 0, 50, 60]                                 # one hint pixel toggled
+    both(call, (out,), (dict(out, depth_hint_mask=mask),))
+    disp = out["disp_hint"].clone()
+    disp[1 - h, 0, 5, 6] = 0.5                                                  # a hintless item's disp_hint not zero
+    both(call, (out,), (dict(out, disp_hint=disp),))
+
+
+def test_nyu_inputs_checker(harness):
+    """two items of the 224_bicubic fixture"""
+    fx = nic.load("224_bicubic")
+    cfg = fx["config"]
+    items = nic.items(fx)[:2]
+    fn = ni.NyuInputs(cfg["is_224"], cfg["resample"])
+    exp = [oni.expected(it["image"], it["depth"], it["flip"], it["perm"], it["gamma"], fn.is_224, fn.resample)
+           for it in items]
+    out = {k: np.stack([e[k] for e in exp]) for k in ("image", "depth")}
+
+    def call(image, depth):
+        harness._check_NyuInputs__run(dict(self=fn, batch=ni.collate(items), device=None),
+                                      dict(image=t(image), depth=t(depth)), None)
+    both(call, (out["image"], out["depth"]), (ulp_up(out["image"], (1, 0, 100, 50)), out["depth"]))
+    both(call, (out["image"], out["depth"]), (out["image"], ulp_up(out["depth"], (0, 0, 10, 20))))
+
+
+# ------------------------------------------------------------------------------------------ KITTI ground truth
+def test_generate_depth_maps_checker(harness):
+    """two 20000-point scans at two of the calibration dates' sizes, padded to one batch"""
+    with np.load(os.path.join(kic.GOLDEN, "kitti_gt_calib.npz")) as f:
+        frames = [("2011_09_26", 2), ("2011_09_28", 3)]
+        P = np.stack([f["%s/P%d" % (d, cam)] for d, cam in frames])
+        sizes = np.array([f["%s/size" % d] for d, _ in frames], np.int32)
+    scans = [okg.small_scan(31 + k, 20000) for k in range(2)]
+    offsets = np.array([0, scans[0].shape[0], scans[0].shape[0] + scans[1].shape[0]])
+    hm, wm = sizes.max(0)
+    depth = np.zeros((2, hm, wm))
+    for k, (h, w) in enumerate(sizes):
+        depth[k, :h, :w] = okg.depth_map(scans[k], P[k], h, w, True)
+    hit = np.argwhere(depth[1] > 0)[0]
+    assert depth[0].all() == 0 and (depth[1] > 0).sum() > 1000 and sizes[1, 0] < hm
+
+    def call(depth):
+        a = dict(points=t(np.concatenate(scans)), offsets=offsets, P=P, sizes=sizes, vel_depth=True)
+        harness._check_generate_depth_maps(a, t(depth), None)
+    both(call, (depth,), (ulp_up(depth, (1, *hit)),))                     # one depth one ulp off
+    zero = np.argwhere(depth[0] == 0)[0]
+    lit = depth.copy()
+    lit[(0, *zero)] = 1.0                                                 # one empty pixel given a depth
+    both(call, (depth,), (lit,))
+    past = depth.copy()
+    past[1, hm - 1, 0] = 1.0                                              # one pixel past frame 1's 370 rows written
+    both(call, (depth,), (past,))

@@ -255,6 +255,10 @@ GT_SIGNATURES = {
                                    c_size_t, c_void_p, c_void_p]),
 }
 
+# every table load() binds; tests/test_launch_check_table.py holds the launch-checking harness to all of them
+TABLES = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES, INPUTS_SIGNATURES,
+          NYU_INPUTS_SIGNATURES, GT_SIGNATURES)
+
 _lib = None
 
 
@@ -281,9 +285,7 @@ def load():
             except OSError:
                 continue
         lib = ctypes.CDLL(LIB_PATH)
-    tables = (SIGNATURES, EVAL_SIGNATURES, LOSS_SIGNATURES, KITTI_LOSS_SIGNATURES, HINTS_SIGNATURES,
-              INPUTS_SIGNATURES, NYU_INPUTS_SIGNATURES, GT_SIGNATURES)
-    for name, (res, args) in [item for table in tables for item in table.items()]:
+    for name, (res, args) in [item for table in TABLES for item in table.items()]:
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args

@@ -126,14 +126,22 @@ class DepthHintGenerator:
         K, inv_K, T = (t.to(dev) for t in self.cameras(right))
         depth = torch.empty((n, 1, h, w), dtype=torch.float32, device=dev)
         index = torch.empty((n, 1, h, w), dtype=torch.int32, device=dev) if return_index else None
-        nbytes = int(_lib.load().wmd_depth_hints_ws_bytes(n, h, w))
-        if nbytes == 0 and n > 0:
-            raise _lib.WmdError("wmd_depth_hints_f32 refuses %d views of %dx%d" % (n, h, w))
-        ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        _launch("depth_hints", lambda: dict(n=n, h=h, w=w)).wmd_depth_hints_f32(
-            _lib.ptr(base), _lib.ptr(lookup), _lib.ptr(maps), _lib.ptr(K), _lib.ptr(inv_K), _lib.ptr(T), n, h, w,
-            _lib.ptr(ws), ws.numel(), _lib.ptr(depth), _lib.ptr(index), _lib.stream_ptr())
+        _fuse(base, lookup, maps, K, inv_K, T, depth, index)
         return (depth, index) if return_index else depth
+
+
+def _fuse(base, lookup, maps, K, inv_K, T, depth, index):
+    """wmd_depth_hints_f32 on (N, H, W, 3) uint8 views, the matchers' (12, N, H, W) int16 maps and (N, 4, 4) float32
+    cameras: each pixel's least-error depth into depth (N, 1, H, W) float32 and, unless None, the winning matcher into
+    index (N, 1, H, W) int32"""
+    n, h, w, _ = base.shape
+    nbytes = int(_lib.load().wmd_depth_hints_ws_bytes(n, h, w))
+    if nbytes == 0 and n > 0:
+        raise _lib.WmdError("wmd_depth_hints_f32 refuses %d views of %dx%d" % (n, h, w))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=base.device)
+    _launch("depth_hints", lambda: dict(n=n, h=h, w=w)).wmd_depth_hints_f32(
+        _lib.ptr(base), _lib.ptr(lookup), _lib.ptr(maps), _lib.ptr(K), _lib.ptr(inv_K), _lib.ptr(T), n, h, w,
+        _lib.ptr(ws), ws.numel(), _lib.ptr(depth), _lib.ptr(index), _lib.stream_ptr())
 
 
 # ---------------------------------------------------------------------------------------------------------------- CLI
