@@ -22,6 +22,14 @@ from before the call (an evaluator's next frame and the rows the call writes) co
 
 Completeness: around each outermost wrapped call the harness takes the `launch_count()` delta; at the end of a workload the
 checked deltas must add up to the whole delta, and any libwmd symbol called outside a wrapped call is named.
+
+Footprint: a workload runs under footprint.Footprint, so every CUDA buffer the package allocates with torch.empty / zeros
+(outputs, workspaces, the checkers' own) sits between guards and an `empty` one starts out as NaN / -1 bytes; the test's
+plain-vs-checked comparison then also asserts that no result depends on what was in memory.  ops._scratch is swapped for
+a _Scratch without its size floors, so each range / compaction / backward / split-K workspace is exactly its size
+query.  At the end every guard must be intact and the counter header of every live range, backward and split-K
+workspace zero (SCRATCH_HEADERS).  Around each outermost call every CUDA tensor reachable from its arguments must keep its
+bits, except the arguments WRITES names.  REACH names the workload or direct case that calls each launch symbol.
 """
 import contextlib
 import inspect
@@ -48,6 +56,7 @@ from wavelet_monodepth_b200 import (_lib, kitti_eval, kitti_gt, kitti_hints, kit
 import conv_grad_ref
 import conv_ref as cr
 import disp_tail_ref
+import footprint
 import haar_ref as har
 import head_ref as hr
 from contract import Worst, errors
@@ -178,6 +187,40 @@ SYMBOLS = {
     "wmd_velo_depth_f64": ("launch", "generate_depth_maps"),
 }
 
+# launch symbol -> the workload (tests/test_gpu_production_launches.py, tests/test_gpu_workload_launches.py) or direct
+# case (tests/test_gpu_launch_footprint.py, "direct:...") that calls it under the harness; each case asserts that the
+# symbols given to it were called
+_SPARSE, _NYU_DENSE, _TRAIN = "sparse_r50_1024x320_x32_thr0.05", "nyu_dense_d161_640x480_x8", "train_wave_r18_640x192_x12"
+_KITTI_EVAL, _NYU_EVAL = "eval_kitti_sparse_r18_x16_postprocess", "eval_nyu_sparse_d161_x16_edges"
+REACH = {
+    "wmd_idwt_haar_f32": _NYU_DENSE, "wmd_idwt_haar_epi_f32": "direct:idwt_forms",
+    "wmd_idwt_bilinear_f32": "direct:idwt_forms", "wmd_dwt_haar_f32": _TRAIN,
+    "wmd_range_thresh_f32": "nyu_sparse_d161_640x480_x8_thr0.1", "wmd_level_masks": _SPARSE, "wmd_compact_mask": _SPARSE,
+    "wmd_gate_map": _SPARSE,
+    "wmd_nchw_to_rows_f32": _NYU_DENSE, "wmd_nchw_to_rows_gated_f32": "direct:gated_layout_moves",
+    "wmd_nchw_to_rows_amax_f32": _SPARSE, "wmd_nchw_to_rows_masked_amax_f32": "direct:gated_layout_moves",
+    "wmd_nchw_to_rows_gated_amax_f32": _SPARSE, "wmd_rows_to_nchw_f32": _TRAIN,
+    "wmd_gather_rows_nchw_f32": "direct:gather_scatter_rows", "wmd_gather_rows_list_f32": "direct:gather_rows_list_abi",
+    "wmd_gather_rows_list_amax_f32": _SPARSE, "wmd_scatter_rows_nchw_f32": "direct:gather_scatter_rows",
+    "wmd_amax_f32": "sparse_r50_1024x320_x16_channels_last", "wmd_amax_rows_masked_f32": "sparse_r50_1024x320_x16_channels_last",
+    "wmd_conv_rows_f32": "baseline_depthdecoder_r18_640x192_x16", "wmd_conv_rows_tc_f32": "direct:conv_rows_tc_abi",
+    "wmd_conv_rows_tc_splitk_f32": _SPARSE,
+    "wmd_head_mlp_f32": _SPARSE, "wmd_head_conv3x3_f32": _NYU_DENSE, "wmd_head_gather_f32": _SPARSE,
+    "wmd_head_idwt_f32": _SPARSE, "wmd_disp_tail16_f32": "baseline_depthdecoder_r18_640x192_x16",
+    "wmd_act_bwd_f32": _TRAIN, "wmd_conv_wgrad_f32": _TRAIN, "wmd_conv_dgrad_fold_f32": _TRAIN,
+    "wmd_eval_gt_mask": _KITTI_EVAL, "wmd_eval_gather_f32": _KITTI_EVAL, "wmd_eval_frames": _KITTI_EVAL,
+    "wmd_eval_errors_f64": _KITTI_EVAL, "wmd_post_process_disparity": _KITTI_EVAL,
+    "wmd_eval_nyu_frames": _NYU_EVAL, "wmd_eval_nyu_errors_f64": _NYU_EVAL, "wmd_eval_edges_frames": _NYU_EVAL,
+    "wmd_eval_edt": _NYU_EVAL,
+    "wmd_loss_nyu_fwd": "train_nyu_wave_d161_640x480_x8_nyuloss", "wmd_loss_nyu_bwd": "train_nyu_wave_d161_640x480_x8_nyuloss",
+    "wmd_loss_kitti_fwd": "train_baseline_r18_640x192_x12_kittiloss",
+    "wmd_loss_kitti_bwd": "train_baseline_r18_640x192_x12_kittiloss",
+    "wmd_sgbm_u8": "hints_320x1024_pair_both_sides", "wmd_depth_hints_f32": "hints_320x1024_pair_both_sides",
+    "wmd_inputs_u8": "train_wave_r18_640x192_x12_from_kitti_inputs",
+    "wmd_nyu_inputs_u8": "train_nyu_wave_d161_640x480_x8_from_nyu_inputs",
+    "wmd_velo_depth_f64": "gt_export_full_scans_then_eval",
+}
+
 # bars of the checks this file adds on top of the contract tests' (units of 2^-24 of the element's scale)
 ACT_BWD_ULP = 4        # dz = dy act'(y): at most three roundings (sigmoid: 1 - y, y (1 - y), the product with dy)
 # bars of the evaluation and loss checks: those of their own tests (test_gpu_nyu_loss, test_gpu_nyu_eval,
@@ -218,7 +261,8 @@ def _require(ok, what):
 
 
 class _LibSpy:
-    """Stands in for the loaded CDLL: records the libwmd symbols called while no wrapped entry point is running."""
+    """Stands in for the loaded CDLL: counts every launch and pack symbol it forwards, and records those called while
+    no wrapped entry point is running."""
 
     def __init__(self, lib, harness):
         self._lib, self._h = lib, harness
@@ -232,8 +276,98 @@ class _LibSpy:
         def call(*args):
             if h.depth == 0:
                 h.outside.append(name)
+            h.launched[name] = h.launched.get(name, 0) + 1
             return fn(*args)
         return call
+
+
+# ------------------------------------------------------------------------------------------ footprint
+# the arguments each entry point writes in place (outputs passed in, amax slots, an evaluator's maps and scores); every
+# other CUDA tensor reachable from a call's arguments must come back bit for bit
+WRITES = {
+    "conv_rows": ("out", "amax_out"), "head_gather": ("out",), "head_conv3x3": ("out",), "disp_tail16": ("out",),
+    "nchw_to_rows": ("amax",), "gather_rows_list": ("amax",), "scatter_rows": ("out",), "amax_rows": ("out",),
+    "act_backward": ("amax",), "_loss_fwd": ("means",), "_edt": ("out",), "_edges_frames": ("scores",),
+    "NyuDepthEvaluator.add": ("depth_out",), "stereo_sgbm": ("out",), "_fuse": ("depth", "index"),
+}
+
+# the counter header of each ops._Scratch workspace kind, which the kernels must leave zero (wmd.h: wmd_range_thresh_f32
+# and wmd_head_idwt_f32 64 KiB, wmd_act_bwd_f32 and wmd_conv_wgrad_f32 4 KiB, the balanced wmd_conv_rows_tc_splitk_f32
+# 4 KiB)
+SCRATCH_HEADERS = {"range": 1 << 16, "bwd": 4096, "splitk": 4096}
+
+
+def _tensors(value, path):
+    """(path, tensor) of every tensor in value, looking through lists, tuples and dicts"""
+    if torch.is_tensor(value):
+        yield path, value
+    elif isinstance(value, (list, tuple)):
+        for i, v in enumerate(value):
+            yield from _tensors(v, "%s[%d]" % (path, i))
+    elif isinstance(value, dict):
+        for k, v in value.items():
+            yield from _tensors(v, "%s[%r]" % (path, k))
+
+
+def _span(t):
+    """(device, first byte, end byte) of the memory a tensor's elements occupy"""
+    n = footprint._extent(t.shape, t.stride()) * t.element_size()
+    return t.device, t.data_ptr(), t.data_ptr() + n
+
+
+def snapshot(args, writes, device_type="cuda"):
+    """[(path, tensor, copy)] of every tensor on `device_type` reachable from the bound arguments `args` (a dict),
+    except those of the arguments named in `writes` and any that shares memory with one of them"""
+    out_spans = [_span(t) for name in writes for _, t in _tensors(args.get(name), name)]
+    snap = []
+    for name, value in args.items():
+        if name in writes:
+            continue
+        for path, t in _tensors(value, name):
+            if t.device.type != device_type or t.numel() == 0:
+                continue
+            d, b, e = _span(t)
+            if any(d == od and b < oe and ob < e for od, ob, oe in out_spans):
+                continue
+            snap.append((path, t, t.detach().clone()))
+    return snap
+
+
+def _bitwise(t):
+    """a tensor's bits as integers, so NaN payloads compare too"""
+    t = t.detach()
+    if t.is_floating_point() or t.is_complex():
+        return t.view({8: torch.int64, 4: torch.int32, 2: torch.int16, 1: torch.uint8}[t.element_size()])
+    return t.view(torch.uint8) if t.dtype == torch.bool else t
+
+
+def changed_inputs(snap):
+    """paths of the snapshot's tensors whose bits differ from their copies"""
+    return [path for path, t, copy in snap if not torch.equal(_bitwise(t), _bitwise(copy))]
+
+
+class _ExactScratch(ops._Scratch):
+    """ops._Scratch without its size floors: each workspace is exactly as large as its size query asks"""
+
+    def _get(self, key, device, nbytes, floor, zero):
+        return super()._get(key, device, nbytes, 0, zero)
+
+
+def scratch_header_faults(scratch):
+    """(headers checked, ["kind: byte k of its counter header is v"]) over the live workspaces of an ops._Scratch"""
+    faults, checked = [], 0
+    for key, buf in scratch.bufs.items():
+        n = SCRATCH_HEADERS.get(key[0])
+        if n is None:
+            continue
+        head = buf[:n]
+        bad = head.nonzero()
+        checked += 1
+        if bad.numel():
+            k = int(bad[0, 0])
+            faults.append("%s workspace of %d bytes: byte %d of its %d-byte counter header is %d"
+                          % (key[0], buf.numel(), k, n, int(head[k])))
+    return checked, faults
 
 
 class Harness:
@@ -247,6 +381,9 @@ class Harness:
         self.gaps = []             # kernels launched between two checked calls of a thread other than the workload's
         self.last_end = {}         # thread -> launch_count() when its last outermost checked call returned
         self.calls = {}
+        self.launched = {}         # launch / pack symbol -> calls
+        self.snapshots = 0         # input tensors compared after their call
+        self.stats = None          # the footprint figures of the last workload
         lib = _lib.load()
         monkeypatch.setattr(_lib, "_lib", _LibSpy(lib, self))
         for owner, attr in ENTRY_POINTS:
@@ -259,6 +396,7 @@ class Harness:
     def _wrap(self, name, orig, check):
         sig = inspect.signature(orig)
         before = getattr(self, hook("_before_", name), None)
+        writes = WRITES.get(name, ())
 
         def wrapped(*args, **kwargs):
             a = sig.bind(*args, **kwargs)
@@ -271,6 +409,7 @@ class Harness:
                 tid = threading.get_ident()
                 if tid != self.main and tid in self.last_end and c0 != self.last_end[tid]:
                     self.gaps.append((name, c0 - self.last_end[tid]))
+                snap = snapshot(a, writes)
             pre = before(a) if before is not None else None
             self.depth += 1
             try:
@@ -283,6 +422,10 @@ class Harness:
                 self.last_end[tid] = c1
                 if tid == self.main:
                     self.checked += c1 - c0
+                changed = changed_inputs(snap)
+                self.snapshots += len(snap)
+                del snap
+                _require(not changed, "%s: %s changed its inputs %s" % (self.current, name, changed))
             self.calls[name] = self.calls.get(name, 0) + 1
             check(a, res, pre)
             return res
@@ -292,19 +435,40 @@ class Harness:
     def workload(self, name):
         """Checks that every kernel launched inside the block ran inside a checked call.  launch_count() counts per host
         thread: on the calling thread the checked deltas must add up to the whole; autograd runs the backward on its own
-        thread, whose counter must not move between two checked calls."""
+        thread, whose counter must not move between two checked calls.  The block runs under footprint.Footprint with
+        exactly sized workspaces; its guards and the workspaces' counter headers are checked at the end (self.stats)."""
         torch.cuda.synchronize()
         self.current, self.checked, self.outside, self.gaps, self.last_end = name, 0, [], [], {}
+        self.launched, self.snapshots = {}, 0
         self.main = threading.get_ident()
-        c0 = _lib.launch_count()
-        yield self
-        torch.cuda.synchronize()
-        total = _lib.launch_count() - c0
+        saved, scratch = ops._scratch, _ExactScratch()
+        ops._scratch = scratch
+        try:
+            with footprint.Footprint() as fp:
+                c0 = _lib.launch_count()
+                yield self
+                torch.cuda.synchronize()
+                total = _lib.launch_count() - c0
+        finally:
+            ops._scratch = saved
         _require(not self.outside and not self.gaps and total == self.checked,
                  "%s: %d kernels launched, %d inside checked calls; libwmd called outside them: %s; launched between "
                  "checked calls of the backward thread, before: %s" % (name, total, self.checked, sorted(set(self.outside)),
                                                                         self.gaps))
         _require(total > 0, "%s launched nothing" % name)
+        headers, faults = scratch_header_faults(scratch)
+        _require(not faults, "%s: workspace counters left nonzero: %s" % (name, faults))
+        self.stats = dict(arenas=fp.checked, guarded=fp.guarded, snapshots=self.snapshots, headers=headers)
+
+    def report(self):
+        """the footprint figures of the last workload, one line"""
+        s = self.stats
+        return ("%d arenas checked, %.1f MB guarded, %d input snapshots compared, %d scratch headers checked"
+                % (s["arenas"], s["guarded"] / 1e6, s["snapshots"], s["headers"]))
+
+    def reached(self, case):
+        """the launch symbols REACH attributes to `case` that this harness has not seen called"""
+        return sorted(s for s, c in REACH.items() if c == case and not self.launched.get(s))
 
     def _weights(self, packed):
         key = packed.data.data_ptr() if isinstance(packed, ops.PackedW) else packed.data_ptr()

@@ -18,6 +18,7 @@ from wavelet_monodepth_b200 import kitti_layers as kl
 from wavelet_monodepth_b200 import nyu_decoders as nd
 from wavelet_monodepth_b200 import ops, synth, wavelets
 
+import footprint
 from helpers import (REL_TOL, compare_outputs, golden_names, key_str, kitti_features, load_golden, nyu_features,
                      rel_err, seeded_params)
 
@@ -289,32 +290,42 @@ def test_full_res_consumer_epilogue_matches_trainer_interpolate():
 
 def test_cuda_graph_replay_matches_eager_and_follows_input_updates():
     """graphs.GraphedSparseDecoder: same kernels captured once; replay == eager bit for bit, also after the bound
-    input tensors are overwritten in place (what a graphed encoder does)."""
+    input tensors are overwritten in place (what a graphed encoder does).  Captured under the guarded, poisoning
+    allocator (tests/footprint.py) and replayed on features A, B, then A again: the third replay equals the first and
+    the eager run on A bit for bit, so no replay reads what an earlier one left behind or a buffer no kernel wrote, and
+    no replay writes past a buffer."""
     from wavelet_monodepth_b200 import graphs
     mod, _, feats = _full_kitti(synth.RESNET18_CH, 4, 192, 640)
-    feats = [f.clone() for f in feats]
-    eager = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in mod(feats, 0.05).items()}
-    g = graphs.GraphedSparseDecoder(mod, feats, 0.05)
-    assert g.launches > 40 and g.bound_to(feats) and not g.bound_to([f.clone() for f in feats])
-    out = g.replay()
-    assert set(out) == set(eager)
-    for k, v in eager.items():
-        if torch.is_tensor(v):
-            assert torch.equal(out[k], v), key_str(k)
-        else:
-            assert out[k] == v, key_str(k)
-    # new content in the same tensors
+    feats_a = [f.clone() for f in feats]
     torch.manual_seed(7)
-    for f in feats:
-        f.mul_(0.5).add_(0.1 * torch.rand_like(f))
-    ref = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in mod(feats, 0.05).items()}
-    out = g.replay()
-    for k, v in ref.items():
-        if torch.is_tensor(v):
-            assert torch.equal(out[k], v), key_str(k)
-        else:
-            assert out[k] == v, key_str(k)
-    assert not torch.equal(ref[("disp", 0)], eager[("disp", 0)])
+    feats_b = [0.5 * f + 0.1 * torch.rand_like(f) for f in feats_a]
+
+    def copy(out):
+        return {k: (v.clone() if torch.is_tensor(v) else v) for k, v in out.items()}
+
+    def equal(got, want, what):
+        assert set(got) == set(want), what
+        for k, v in want.items():
+            assert (torch.equal(got[k], v) if torch.is_tensor(v) else got[k] == v), (what, key_str(k))
+    eager_a = copy(mod(feats_a, 0.05))
+    eager_b = copy(mod(feats_b, 0.05))
+    assert not torch.equal(eager_a[("disp", 0)], eager_b[("disp", 0)])
+    feats = [f.clone() for f in feats_a]
+    with footprint.Footprint() as fp:
+        g = graphs.GraphedSparseDecoder(mod, feats, 0.05)
+        assert g.launches > 40 and g.bound_to(feats) and not g.bound_to([f.clone() for f in feats])
+        first = copy(g.replay())
+        equal(first, eager_a, "replay on A")
+        for f, b in zip(feats, feats_b):                     # new content in the same tensors
+            f.copy_(b)
+        equal(copy(g.replay()), eager_b, "replay on B")
+        for f, a in zip(feats, feats_a):
+            f.copy_(a)
+        third = copy(g.replay())
+        torch.cuda.synchronize()
+    equal(third, first, "third replay against the first")
+    equal(third, eager_a, "third replay on A")
+    assert fp.checked >= fp.allocated > 0
 
 
 def test_layout_move_options_are_bit_identical_eager_and_graphed():

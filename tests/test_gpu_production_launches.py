@@ -6,10 +6,13 @@ production: data-dependent row counts, stream-K cuts and balanced remainders; fp
 decoders' amax slots (one per source for the whole batch); high-pass heads whose outputs cancel in flat regions; backward
 paths such as the split-pixel weight gradient of a cout-1 layer over 1.5 M rows.  Each workload runs once plainly and once
 under the harness, which checks each launch element by element at its kernel's bar, its preconditions, and that every
-kernel launched ran inside a checked call.  The two runs must agree bit for bit (outputs, and in training the gradients):
-the harness does not change what it checks, and results depend neither on timing nor on buffer reuse.
+kernel launched ran inside a checked call, with every buffer guarded and poisoned, exactly sized workspaces and inputs
+compared bit for bit after each call.  The two runs must agree bit for bit (outputs, and in training the gradients): the
+harness does not change what it checks, and results depend neither on timing, nor on buffer reuse, nor on what was in
+memory.  The launch symbols launch_check.REACH attributes to a workload must be called by it.
 """
 import gc
+import time
 
 import numpy as np
 import pytest
@@ -107,14 +110,19 @@ WORKLOADS = {
 @pytest.mark.parametrize("name", list(WORKLOADS))
 def test_every_launch_meets_its_contract(name, monkeypatch):
     run = WORKLOADS[name]
+    t0 = time.perf_counter()
     plain = run()
     torch.cuda.synchronize()
+    t1 = time.perf_counter()
     harness = lc.Harness(monkeypatch)
     with harness.workload(name):
         checked = run()
     monkeypatch.undo()
+    t2 = time.perf_counter()
     same(plain, checked, name)
-    print("%s: %s" % (name, ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
+    assert not harness.reached(name), (name, "never called", harness.reached(name))
+    print("%s (%.1f s plain, %.1f s checked; %s): %s" % (name, t1 - t0, t2 - t1, harness.report(),
+                                                         ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
     del plain, checked, harness
     gc.collect()
     torch.cuda.empty_cache()

@@ -20,7 +20,9 @@ points are called through their modules, as the package's users do: a name impor
 harness's wrapper, and the completeness check would name its symbol.
 
 Each workload runs once plainly and once under the harness, which checks each launch at its kernel's bar and that every
-kernel launched ran inside a checked call; the two runs must agree bit for bit.  Each prints its per-entry-point call
+kernel launched ran inside a checked call, with every buffer guarded and poisoned, exactly sized workspaces and inputs
+compared bit for bit after each call; the two runs must agree bit for bit, so no result depends on what was in memory.
+The launch symbols launch_check.REACH attributes to a workload must be called by it.  Each prints its per-entry-point call
 counts and wall times; the module prints the worst error of every (entry point, engine, mode) at the end.
 """
 import gc
@@ -347,8 +349,9 @@ def test_every_launch_meets_its_contract(name, monkeypatch):
     monkeypatch.undo()
     t2 = time.perf_counter()
     same(plain, checked, name)
-    print("%s (%.1f s plain, %.1f s checked): %s" % (name, t1 - t0, t2 - t1,
-                                                     ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
+    assert not harness.reached(name), (name, "never called", harness.reached(name))
+    print("%s (%.1f s plain, %.1f s checked; %s): %s" % (name, t1 - t0, t2 - t1, harness.report(),
+                                                         ", ".join("%s x%d" % kv for kv in sorted(harness.calls.items()))))
     del plain, checked, harness
     gc.collect()
     torch.cuda.empty_cache()

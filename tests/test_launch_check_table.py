@@ -1,6 +1,8 @@
 """Every libwmd symbol is classified for the launch-checking harness (tests/launch_check.py): a launch whose entry point
 has a checker, a pack, or a size / query function.  A new entry point cannot ship without one."""
 import inspect
+import os
+import re
 
 from wavelet_monodepth_b200 import (_lib, kitti_eval, kitti_gt, kitti_hints, kitti_inputs, kitti_loss, nyu_eval, nyu_inputs,
                                     nyu_loss, ops)
@@ -67,3 +69,30 @@ def test_every_ops_function_that_calls_libwmd_is_wrapped():
     assert {lc.entry_name(o, a) for o, a in lc.EVAL_LOSS + lc.PIPELINES} <= found
     for entry in set(lc.CHECKED) | set(lc.PACKS):
         assert callable(getattr(ops, entry)), entry
+
+
+def _cases():
+    """the workloads of the two workload modules and the direct cases of test_gpu_launch_footprint"""
+    import test_gpu_production_launches as tp
+    import test_gpu_workload_launches as tw
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_gpu_launch_footprint.py")) as f:
+        direct = set(re.findall(r'"(direct:\w+)"', f.read()))
+    return set(tp.WORKLOADS) | set(tw.WORKLOADS) | direct
+
+
+def test_every_launch_symbol_has_a_case_that_reaches_it():
+    """REACH names, for every launch symbol, the workload or direct case that calls it (each GPU case asserts that it
+    does), and only cases that exist"""
+    launches = {s for s, k in lc.SYMBOLS.items() if k != "query" and k[0] == "launch"}
+    assert set(lc.REACH) == launches, sorted(set(lc.REACH) ^ launches)
+    cases = _cases()
+    unknown = {s: c for s, c in lc.REACH.items() if c not in cases}
+    assert not unknown, unknown
+
+
+def test_writes_names_parameters_of_its_entry_points():
+    """every WRITES entry is a wrapped entry point and every name in it one of that entry's parameters"""
+    params = {lc.entry_name(o, a): inspect.signature(getattr(o, a)).parameters for o, a in lc.ENTRY_POINTS}
+    for entry, names in lc.WRITES.items():
+        assert entry in params, entry
+        assert names and set(names) <= set(params[entry]), (entry, names, list(params[entry]))

@@ -4,7 +4,11 @@ must see (a loss gradient one ulp off, one edge pixel toggled, one a_k count off
 off, one KITTI loss mask pixel toggled, one SGBM disparity 1/16 px off, one fused depth one ulp off or its matcher index
 changed, one input colour element one ulp off, one hint pixel toggled, one ground-truth depth one ulp off or one empty
 ground-truth pixel given a depth).  CPU only: the checkers are called directly on CPU tensors, with stand-ins for the
-evaluators' state; no GPU and no libwmd."""
+evaluators' state; no GPU and no libwmd.
+
+The footprint checks have teeth too, on CPU tensors the test owns (footprint.Footprint("cpu")): a write one element
+into either guard, a poisoned cell that reaches a result, a channels_last buffer with the wrong strides, a changed input
+that WRITES does not name, and a nonzero byte in a workspace's counter header are each caught."""
 import os
 import types
 
@@ -24,10 +28,13 @@ from oracle import nyu_loss as onl
 from oracle import sgbm as osgbm
 from wavelet_monodepth_b200 import kitti_inputs as ki
 from wavelet_monodepth_b200 import nyu_inputs as ni
+from wavelet_monodepth_b200 import ops
 
+import footprint
 import kitti_inputs_cases as kic
 import launch_check as lc
 import nyu_inputs_cases as nic
+from workloads import same
 
 
 @pytest.fixture
@@ -442,3 +449,114 @@ def test_generate_depth_maps_checker(harness):
     past = depth.copy()
     past[1, hm - 1, 0] = 1.0                                              # one pixel past frame 1's 370 rows written
     both(call, (depth,), (past,))
+
+
+# ------------------------------------------------------------------------------------------ footprint
+@pytest.mark.parametrize("dtype", [torch.float32, torch.float64, torch.int16, torch.uint8])
+@pytest.mark.parametrize("side", [-1, 1])
+def test_a_write_one_element_into_a_guard_is_caught(dtype, side):
+    with footprint.Footprint("cpu"):
+        t = torch.empty((5, 7), dtype=dtype)
+        t.fill_(3)                                                       # the whole buffer: allowed
+    with pytest.raises(footprint.FootprintError, match="guard byte %s" % ("1 before" if side < 0 else "0 after")):
+        with footprint.Footprint("cpu"):
+            t = torch.empty((5, 7), dtype=dtype)
+            at = t.storage_offset() + (-1 if side < 0 else t.numel())     # one element before / after the buffer
+            t.as_strided((1,), (1,), at).fill_(3)
+            del t                                                        # checked when it dies ...
+    with pytest.raises(footprint.FootprintError, match="test_launch_check_teeth"):
+        with footprint.Footprint("cpu"):
+            keep = torch.zeros_like(torch.ones(3, 4, dtype=dtype)).t()  # ... or on exit while it lives
+            keep.as_strided((1,), (1,), keep.storage_offset() + 12).fill_(1)
+
+
+def _kernel(x, alloc):
+    """writes every cell of its output but the first, and returns twice it: reads a cell it never wrote"""
+    out = alloc(x.shape, dtype=x.dtype)
+    out[1:] = x[1:]
+    return {"y": out * 2}
+
+
+def _kernel_ok(x, alloc):
+    out = alloc(x.shape, dtype=x.dtype)
+    out[:] = x
+    return {"y": out * 2}
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, torch.int32])
+def test_a_poisoned_cell_that_reaches_a_result_is_caught(dtype):
+    """the plain run's allocator left zeros (a fresh process); under the footprint the cell is NaN / -1"""
+    x = torch.arange(1, 9, dtype=dtype)
+    for k in (_kernel_ok, _kernel):
+        plain = k(x, torch.zeros)
+        with footprint.Footprint("cpu"):
+            checked = k(x, torch.empty)
+        if k is _kernel_ok:
+            same(plain, checked, "teeth")
+        else:
+            with pytest.raises(AssertionError, match="differs under the harness"):
+                same(plain, checked, "teeth")
+
+
+def test_buffers_have_torchs_layout_and_contents():
+    """dtype, shape and strides equal torch's own allocation (channels_last, preserve_format of a permuted tensor),
+    empty is all POISON bytes, zeros all zero, each buffer ALIGN-aligned; other devices pass through"""
+    cl4 = torch.channels_last
+    with footprint.Footprint("cpu") as fp:
+        made = [(torch.empty((2, 8, 3, 5), memory_format=cl4), torch.empty((2, 8, 3, 5), device="meta", memory_format=cl4)),
+                (torch.zeros((4, 6), dtype=torch.int64), torch.zeros((4, 6), dtype=torch.int64, device="meta")),
+                (torch.empty_like(torch.ones(3, 4, 5).permute(2, 0, 1)), torch.ones(3, 4, 5).permute(2, 0, 1)),
+                (torch.zeros_like(torch.ones(2, 3), dtype=torch.bool), torch.zeros(2, 3, dtype=torch.bool, device="meta")),
+                (torch.empty(()), torch.empty((), device="meta"))]
+        passed = torch.empty(3, device="meta")
+    assert fp.allocated == len(made) and passed.device.type == "meta"
+    for t, like in made:
+        assert t.dtype == like.dtype and t.shape == like.shape and t.stride() == like.stride()
+        assert t.data_ptr() % footprint.ALIGN == 0
+    assert bool((made[0][0].view(torch.int32) == -1).all()) and bool((made[2][0].view(torch.int32) == -1).all())
+    assert not made[1][0].any() and not made[3][0].any()
+
+
+def test_a_channels_last_buffer_with_the_wrong_strides_is_caught(monkeypatch):
+    def contiguous(arena, start, meta):
+        return arena.view(meta.dtype)[start // meta.element_size():][:meta.numel()].view(meta.shape)
+    monkeypatch.setattr(footprint, "_view", contiguous)
+    with footprint.Footprint("cpu"):
+        torch.empty((2, 4, 3, 3))                                        # contiguous: the strides agree
+        with pytest.raises(footprint.FootprintError, match="strides"):
+            torch.empty((2, 4, 3, 3), memory_format=torch.channels_last)
+
+
+def test_a_changed_input_is_caught_unless_written_is_declared():
+    args = {"x": torch.arange(12.0).reshape(3, 4), "feats": [torch.ones(5), {"s": torch.zeros(2, dtype=torch.int32)}],
+            "out": torch.zeros(4), "scale": 2.0, "empty": torch.empty(0)}
+    alias = args["out"][1:3]
+    args["view"] = alias                                                 # shares memory with a written argument
+
+    def call(mutate):
+        snap = lc.snapshot(args, ("out",), device_type="cpu")
+        mutate()
+        return lc.changed_inputs(snap)
+    assert call(lambda: args["out"].add_(1)) == []                       # named in WRITES (its alias too)
+    assert call(lambda: None) == []
+    assert call(lambda: args["x"].view(-1)[5].add_(1)) == ["x"]
+    assert call(lambda: args["feats"][1]["s"].sub_(1)) == ["feats[1]['s']"]
+    nan = args["feats"][0]
+    nan[2] = float("nan")
+    payload = torch.tensor([0x7FC00001], dtype=torch.int32).view(torch.float32)
+    assert call(lambda: nan.__setitem__(2, payload[0])) == ["feats[0]"]  # another NaN: its bits changed
+
+
+def test_a_nonzero_counter_header_is_caught():
+    scratch = ops._Scratch()
+    sizes = {"range": 1 << 17, "bwd": 8192, "splitk": 4096, "compact": 64}
+    scratch.bufs = {(kind, 0, 0, 0): torch.zeros(n, dtype=torch.uint8) for kind, n in sizes.items()}
+    scratch.bufs["compact", 0, 0, 0].fill_(7)                           # no header: not checked
+    assert lc.scratch_header_faults(scratch) == (3, [])
+    for kind, at in (("range", (1 << 16) - 1), ("bwd", 0), ("splitk", 4095)):
+        scratch.bufs[kind, 0, 0, 0][at] = 1
+        checked, faults = lc.scratch_header_faults(scratch)
+        assert checked == 3 and len(faults) == 1 and faults[0].startswith(kind) and "byte %d " % at in faults[0]
+        scratch.bufs[kind, 0, 0, 0][at] = 0
+    scratch.bufs["range", 0, 0, 0][1 << 16] = 1                          # past the header: partial sums
+    assert lc.scratch_header_faults(scratch) == (3, [])
